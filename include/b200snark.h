@@ -65,6 +65,8 @@ extern "C" {
 #define B2S_ERR_CUDA 18
 #define B2S_ERR_OOM 19
 #define B2S_ERR_NCCL 20
+#define B2S_ERR_INVALID_DATA 21             /* SerializationError::InvalidData: bad flags or length, coordinate >= p, not on
+                                               the curve, not in the prime-order subgroup */
 
 typedef struct b2s_ctx b2s_ctx;
 typedef struct b2s_r1cs b2s_r1cs;   /* device-resident A/B/C in CSR (witness independent; upload once per circuit) */
@@ -249,6 +251,34 @@ int32_t b2s_vk_serialize(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2
 uint64_t b2s_pk_serialized_size(const b2s_ctx* ctx, const b2s_pk* pk, uint64_t vk_len, int32_t compressed);
 int32_t b2s_pk_serialize(b2s_ctx* ctx, const b2s_pk* pk, const uint8_t* vk_bytes, uint64_t vk_len, int32_t compressed,
                          uint8_t* out, uint64_t cap);
+
+/* ---- CanonicalDeserialize of the same types (the inverse of the serializers above) --------------------------------------
+ * Bytes on the HOST, in the encodings above.  The raw bytes are copied to the device in chunks; flags, byte order, the
+ * canonicity check (every coordinate < p), the Montgomery conversion, the square root of compressed points and the checks
+ * run in CUDA kernels.  compressed = 1 / 0 as for the serializers; validate = 1 is ark's Validate::Yes (uncompressed points
+ * satisfy the curve equation, every point lies in the prime-order subgroup), 0 is Validate::No.  A compressed x without a
+ * square root is rejected in both modes.  Failures return B2S_ERR_INVALID_DATA and b2s_last_error names the vector, the
+ * lowest failing index and the reason, e.g. "h_query[1234]: not in the prime-order subgroup".
+ *   b2s_deserialize_g1/g2  `count` points from exactly `len` bytes -> HOST affine Montgomery (infinity = all-zero)
+ *   b2s_proof_deserialize  Proof { a, b, c } from exactly `len` bytes
+ *   b2s_vk_deserialize     VerifyingKey from the start of `in` (a ProvingKey starts with its VerifyingKey, so this reads the vk
+ *                          out of pk bytes): *n_gamma_abc = |gamma_abc_g1|, *consumed = the vk's byte length; with
+ *                          out_gamma_abc_g1 = NULL only those two are filled in, nothing is decoded
+ *   b2s_pk_deserialize     a whole ark-groth16 ProvingKey (exactly `len` bytes) -> the device-resident full key, the same
+ *                          handle b2s_pk_upload returns for the same points.  The dimensions follow from the bytes:
+ *                          n_instance = |gamma_abc_g1|, n_witness = |l_query|, domain_size = |h_query| + 1 (a power of two),
+ *                          |a_query| = |b_g1_query| = |b_g2_query| = n_instance + n_witness, else B2S_ERR_MALFORMED_VK.
+ * Every Vec length prefix is checked against the bytes that remain before anything is allocated. */
+int32_t b2s_deserialize_g1(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t count, int32_t compressed, int32_t validate,
+                           void* out_affine);
+int32_t b2s_deserialize_g2(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t count, int32_t compressed, int32_t validate,
+                           void* out_affine);
+int32_t b2s_proof_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, void* out_a_g1,
+                              void* out_b_g2, void* out_c_g1);
+int32_t b2s_vk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, void* out_alpha_g1,
+                           void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1, uint64_t cap_gamma_abc,
+                           uint64_t* n_gamma_abc, uint64_t* consumed);
+int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, b2s_pk** out);
 
 /* ---- setup helper (SURVEY 8(f) row 2): fixed-base batch multiplication -------------------------
  * out[i] = scalars[i] * G (the curve's standard generator), affine, i < n.  Used to build proving keys

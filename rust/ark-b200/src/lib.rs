@@ -53,6 +53,17 @@ extern "C" {
     pub fn b2s_pk_serialized_size(ctx: *const B2sCtx, pk: *const B2sPk, vk_len: u64, compressed: i32) -> u64;
     pub fn b2s_pk_serialize(ctx: *mut B2sCtx, pk: *const B2sPk, vk_bytes: *const u8, vk_len: u64, compressed: i32,
                             out: *mut u8, cap: u64) -> i32;
+    // CanonicalDeserialize of the same types, decoded and validated on the GPU (validate = 1: Validate::Yes)
+    pub fn b2s_deserialize_g1(ctx: *mut B2sCtx, inp: *const u8, len: u64, count: u64, compressed: i32, validate: i32,
+                              out_affine: *mut c_void) -> i32;
+    pub fn b2s_deserialize_g2(ctx: *mut B2sCtx, inp: *const u8, len: u64, count: u64, compressed: i32, validate: i32,
+                              out_affine: *mut c_void) -> i32;
+    pub fn b2s_proof_deserialize(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, out_a_g1: *mut c_void,
+                                 out_b_g2: *mut c_void, out_c_g1: *mut c_void) -> i32;
+    pub fn b2s_vk_deserialize(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, out_alpha_g1: *mut c_void,
+                              out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void, out_delta_g2: *mut c_void,
+                              out_gamma_abc_g1: *mut c_void, cap_gamma_abc: u64, n_gamma_abc: *mut u64, consumed: *mut u64) -> i32;
+    pub fn b2s_pk_deserialize(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, out: *mut *mut B2sPk) -> i32;
     // universal-setup schemes (UniversalSetupSNARK, snark/src/lib.rs:107-133): the seams a polynomial-commitment /
     // evaluation-domain backend binds (INTEGRATION.md section 8).  mem: 0 host, 1 device; s, c, z: one Montgomery Fr on the host
     pub fn b2s_ntt(ctx: *mut B2sCtx, data: *mut c_void, log_n: u32, inverse: i32, coset: i32, mem: i32) -> i32;
@@ -141,9 +152,8 @@ pub struct Groth16B200<E: Pairing>(core::marker::PhantomData<E>);
 pub struct Resident { pub ctx: *mut B2sCtx, pub pk: *mut B2sPk, pub mat: *mut B2sR1cs }
 
 impl<E: Pairing> Groth16B200<E> {
-    /// Upload the matrices and the key once per (key, circuit shape).  `curve_id`: 0 = BLS12-381, 1 = BN254.
-    pub fn make_resident(curve_id: i32, pk: &ProvingKey<E>, mats: &[Matrix<E::ScalarField>], n_inst: usize, n_wit: usize)
-        -> Result<Resident, B200Error> {
+    fn ctx_and_matrices(curve_id: i32, mats: &[Matrix<E::ScalarField>], n_inst: usize, n_wit: usize)
+        -> Result<(*mut B2sCtx, *mut B2sR1cs), B200Error> {
         let mut ctx: *mut B2sCtx = core::ptr::null_mut();
         check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
         let csr: Vec<_> = mats.iter().map(to_csr).collect();
@@ -152,6 +162,13 @@ impl<E: Pairing> Groth16B200<E> {
         let co: Vec<*const c_void> = csr.iter().map(|m| m.2.as_ptr().cast()).collect();
         let mut mat: *mut B2sR1cs = core::ptr::null_mut();
         check(ctx, unsafe { b2s_r1cs_upload(ctx, mats[0].len() as u64, n_inst as u64, n_wit as u64, rp.as_ptr(), col.as_ptr(), co.as_ptr(), &mut mat) })?;
+        Ok((ctx, mat))
+    }
+
+    /// Upload the matrices and the key once per (key, circuit shape).  `curve_id`: 0 = BLS12-381, 1 = BN254.
+    pub fn make_resident(curve_id: i32, pk: &ProvingKey<E>, mats: &[Matrix<E::ScalarField>], n_inst: usize, n_wit: usize)
+        -> Result<Resident, B200Error> {
+        let (ctx, mat) = Self::ctx_and_matrices(curve_id, mats, n_inst, n_wit)?;
         let n = (mats[0].len() + n_inst).next_power_of_two() as u64;          // the QAP domain (LibsnarkReduction)
         let (alpha, beta1, delta1) = (pack_points(&[pk.vk.alpha_g1]), pack_points(&[pk.beta_g1]), pack_points(&[pk.delta_g1]));
         let (beta2, delta2) = (pack_points(&[pk.vk.beta_g2]), pack_points(&[pk.vk.delta_g2]));
@@ -169,6 +186,17 @@ impl<E: Pairing> Groth16B200<E> {
         };
         let mut pkh: *mut B2sPk = core::ptr::null_mut();
         check(ctx, unsafe { b2s_pk_upload(ctx, &d, 0 /* B2S_MEM_HOST */, &mut pkh) })?;
+        Ok(Resident { ctx, pk: pkh, mat })
+    }
+
+    /// The same handle from the bytes of a serialized `ProvingKey` (what `serialize_compressed` / `serialize_uncompressed`
+    /// wrote after setup), without building the key on the CPU: framing is read on the host, every point is decoded and,
+    /// with `validate`, checked (curve equation, prime-order subgroup) on the GPU, straight into the resident key.
+    pub fn make_resident_from_bytes(curve_id: i32, pk_bytes: &[u8], compressed: bool, validate: bool, mats: &[Matrix<E::ScalarField>],
+                                    n_inst: usize, n_wit: usize) -> Result<Resident, B200Error> {
+        let (ctx, mat) = Self::ctx_and_matrices(curve_id, mats, n_inst, n_wit)?;
+        let mut pkh: *mut B2sPk = core::ptr::null_mut();
+        check(ctx, unsafe { b2s_pk_deserialize(ctx, pk_bytes.as_ptr(), pk_bytes.len() as u64, compressed as i32, validate as i32, &mut pkh) })?;
         Ok(Resident { ctx, pk: pkh, mat })
     }
 }

@@ -28,6 +28,12 @@ int32_t vk_serialize(Ctx* c, const void* alpha_g1, const void* beta_g2, const vo
                      uint64_t n_gamma_abc, bool compressed, uint8_t* out, uint64_t cap);
 uint64_t pk_serialized_size(Ctx* c, const b2s_pk* pk, uint64_t vk_len, bool compressed);
 int32_t pk_serialize(Ctx* c, const b2s_pk* pk, const uint8_t* vk_bytes, uint64_t vk_len, bool compressed, uint8_t* out, uint64_t cap);
+// deserialize.cu
+int32_t deserialize_points(Ctx* c, int group, const uint8_t* in, uint64_t len, uint64_t count, bool compressed, bool validate, void* out_host);
+int32_t proof_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* a, void* b, void* cc);
+int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* alpha, void* beta, void* gamma,
+                       void* delta, void* abc, uint64_t cap_abc, uint64_t* n_abc, uint64_t* consumed);
+int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, b2s_pk** out);
 }  // namespace b2s
 
 #define LOCK(ctx)                                      \
@@ -585,6 +591,40 @@ int32_t b2s_proof_serialize_compressed(b2s_ctx* ctx, const void* a_g1, const voi
     B2S_TRY(serialize_points(ctx, 1, a_g1, 1, out, fq));
     B2S_TRY(serialize_points(ctx, 2, b_g2, 1, out + fq, 2 * fq));
     return serialize_points(ctx, 1, c_g1, 1, out + 3 * fq, fq);
+}
+
+int32_t b2s_deserialize_g1(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t count, int32_t compressed, int32_t validate,
+                           void* out_affine) {
+    LOCK(ctx);
+    if ((!in && len) || (!out_affine && count)) return fail(ctx, B2S_ERR_INVALID_ARG, "deserialize: null buffer");
+    return deserialize_points(ctx, 1, in, len, count, compressed != 0, validate != 0, out_affine);
+}
+int32_t b2s_deserialize_g2(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t count, int32_t compressed, int32_t validate,
+                           void* out_affine) {
+    LOCK(ctx);
+    if ((!in && len) || (!out_affine && count)) return fail(ctx, B2S_ERR_INVALID_ARG, "deserialize: null buffer");
+    return deserialize_points(ctx, 2, in, len, count, compressed != 0, validate != 0, out_affine);
+}
+int32_t b2s_proof_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, void* out_a_g1,
+                              void* out_b_g2, void* out_c_g1) {
+    LOCK(ctx);
+    if (!in || !out_a_g1 || !out_b_g2 || !out_c_g1) return fail(ctx, B2S_ERR_INVALID_ARG, "proof_deserialize: null buffer");
+    return proof_deserialize(ctx, in, len, compressed != 0, validate != 0, out_a_g1, out_b_g2, out_c_g1);
+}
+int32_t b2s_vk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, void* out_alpha_g1,
+                           void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1, uint64_t cap_gamma_abc,
+                           uint64_t* n_gamma_abc, uint64_t* consumed) {
+    LOCK(ctx);
+    if (!in || (out_gamma_abc_g1 && (!out_alpha_g1 || !out_beta_g2 || !out_gamma_g2 || !out_delta_g2)))
+        return fail(ctx, B2S_ERR_INVALID_ARG, "vk_deserialize: null buffer");
+    return vk_deserialize(ctx, in, len, compressed != 0, validate != 0, out_alpha_g1, out_beta_g2, out_gamma_g2, out_delta_g2,
+                          out_gamma_abc_g1, cap_gamma_abc, n_gamma_abc, consumed);
+}
+int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, b2s_pk** out) {
+    LOCK(ctx);
+    if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_deserialize: null argument");
+    *out = nullptr;
+    return pk_deserialize(ctx, in, len, compressed != 0, validate != 0, out);
 }
 
 }  // extern "C"

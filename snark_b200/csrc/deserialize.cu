@@ -1,0 +1,265 @@
+// CanonicalDeserialize of points, Proof, VerifyingKey and ProvingKey (the inverse of serialize.cu).  The raw bytes go to
+// the device unchanged: flags, byte order, the canonicity check, the Montgomery conversion, the square root and the
+// curve / subgroup checks all run in the decode kernel (deserialize.cuh).  The host reads only the Vec length prefixes and
+// checks the bounds.  Input streams in chunks through two pinned staging buffers: the copy of chunk k + 1 (side stream)
+// overlaps the decoding of chunk k (ctx stream), and points land directly in their final device arrays -- for a proving
+// key the b2s_pk query buffers.
+#include <cuda_runtime.h>
+
+#include <algorithm>
+#include <cstring>
+
+#include "common.cuh"
+#include "deserialize.cuh"
+#include "r1cs.cuh"
+
+namespace b2s {
+
+int32_t pk_finish(Ctx* c, b2s_pk* pk);   // groth16.cu
+
+template <class Curve, class F>
+__global__ void decode_points_kernel(const uint8_t* in, uint32_t n, uint32_t pb, int compressed, int validate, uint64_t base,
+                                     Affine<F>* out, unsigned long long* err) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Affine<F> p = Affine<F>::inf();
+    const uint32_t st = decode_point<Curve, F>(in + (size_t)i * pb, compressed != 0, validate != 0, p);
+    if (st != DEC_OK) {
+        atomicMin(err, (unsigned long long)((base + i) << 3 | st));   // lowest failing index, with its reason
+        p = Affine<F>::inf();
+    }
+    out[i] = p;
+}
+
+static const char* reason_text(uint32_t st) {
+    switch (st) {
+        case DEC_BAD_FLAGS: return "bad flags";
+        case DEC_NONCANONICAL: return "coordinate not below p";
+        case DEC_NOT_ON_CURVE: return "not on the curve";
+        case DEC_NOT_IN_SUBGROUP: return "not in the prime-order subgroup";
+    }
+    return "invalid";
+}
+
+static size_t fq_bytes(Ctx* c) { return c->curve == B2S_CURVE_BLS12_381 ? 48 : 32; }
+static size_t enc_bytes(Ctx* c, int group, bool compressed) { return fq_bytes(c) * group * (compressed ? 1 : 2); }
+static size_t aff_bytes(Ctx* c, int group) { return 2 * fq_bytes(c) * group; }
+
+// Two pinned host buffers and two device buffers, reused by every vector of one call.
+struct Stager {
+    static constexpr uint64_t CH = 1u << 18;   // points per chunk
+    Ctx* c;
+    size_t cap = 0;
+    uint8_t* pinned[2] = {nullptr, nullptr};
+    DevBuf dev[2], err;
+    cudaEvent_t copied[2] = {nullptr, nullptr}, consumed[2] = {nullptr, nullptr};
+    explicit Stager(Ctx* ctx) : c(ctx) {}
+    ~Stager() {
+        cudaStreamSynchronize(c->side);
+        cudaStreamSynchronize(c->stream);
+        for (int s = 0; s < 2; s++) {
+            if (pinned[s]) cudaFreeHost(pinned[s]);
+            if (copied[s]) cudaEventDestroy(copied[s]);
+            if (consumed[s]) cudaEventDestroy(consumed[s]);
+        }
+    }
+    int32_t reserve(size_t bytes) {
+        if (!err.p) {
+            B2S_TRY(err.alloc(c, sizeof(unsigned long long)));
+            for (int s = 0; s < 2; s++) {
+                B2S_CUDA(c, cudaEventCreateWithFlags(&copied[s], cudaEventDisableTiming));
+                B2S_CUDA(c, cudaEventCreateWithFlags(&consumed[s], cudaEventDisableTiming));
+            }
+        }
+        if (bytes <= cap) return B2S_OK;
+        B2S_CUDA(c, cudaStreamSynchronize(c->side));
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+        for (int s = 0; s < 2; s++) {
+            if (pinned[s]) cudaFreeHost(pinned[s]);
+            pinned[s] = nullptr;
+            B2S_CUDA(c, cudaMallocHost(&pinned[s], bytes));
+            B2S_TRY(dev[s].alloc(c, bytes));
+        }
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));   // the side stream copies into dev[] allocated on the ctx stream
+        cap = bytes;
+        return B2S_OK;
+    }
+
+    // `count` encodings from the HOST -> affine Montgomery points at out_dev; `name` labels the error message
+    int32_t decode(int group, const uint8_t* in, uint64_t count, bool compressed, bool validate, void* out_dev, const char* name) {
+        if (!count) return B2S_OK;
+        const size_t pb = enc_bytes(c, group, compressed), ab = aff_bytes(c, group);
+        B2S_TRY(reserve((size_t)std::min<uint64_t>(count, CH) * pb));
+        B2S_CUDA(c, cudaMemsetAsync(err.p, 0xFF, sizeof(unsigned long long), c->stream));
+        for (uint64_t base = 0, k = 0; base < count; base += CH, k++) {
+            const int s = (int)(k & 1);
+            const uint32_t n = (uint32_t)std::min<uint64_t>(CH, count - base);
+            if (k >= 2) B2S_CUDA(c, cudaEventSynchronize(copied[s]));   // pinned[s] is free again
+            memcpy(pinned[s], in + base * pb, (size_t)n * pb);
+            if (k >= 2) B2S_CUDA(c, cudaStreamWaitEvent(c->side, consumed[s], 0));   // dev[s] has been decoded
+            B2S_CUDA(c, cudaMemcpyAsync(dev[s].p, pinned[s], (size_t)n * pb, cudaMemcpyHostToDevice, c->side));
+            B2S_CUDA(c, cudaEventRecord(copied[s], c->side));
+            B2S_CUDA(c, cudaStreamWaitEvent(c->stream, copied[s], 0));
+            char* dst = static_cast<char*>(out_dev) + base * ab;
+            const uint8_t* src = dev[s].as<uint8_t>();
+            unsigned long long* e = err.as<unsigned long long>();
+            int32_t st = dispatch_curve(c, [&](auto curve) {
+                using C = decltype(curve);
+                if (group == 1) {
+                    auto kern = decode_points_kernel<C, typename C::Fq>;
+                    B2S_LAUNCH_N(c, "decode_points_g1", kern, cdiv(n, 128), 128, 0, src, n, (uint32_t)pb, (int)compressed, (int)validate,
+                                 base, reinterpret_cast<Affine<typename C::Fq>*>(dst), e);
+                } else {
+                    auto kern = decode_points_kernel<C, typename C::Fq2>;
+                    B2S_LAUNCH_N(c, "decode_points_g2", kern, cdiv(n, 128), 128, 0, src, n, (uint32_t)pb, (int)compressed, (int)validate,
+                                 base, reinterpret_cast<Affine<typename C::Fq2>*>(dst), e);
+                }
+                return (int32_t)B2S_OK;
+            });
+            B2S_TRY(st);
+            B2S_CUDA(c, cudaEventRecord(consumed[s], c->stream));
+        }
+        unsigned long long word = 0;
+        B2S_CUDA(c, cudaMemcpyAsync(&word, err.p, sizeof(word), cudaMemcpyDeviceToHost, c->stream));
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+        if (word != ~0ull)
+            return fail(c, B2S_ERR_INVALID_DATA, "%s[%llu]: %s", name, (unsigned long long)(word >> 3), reason_text((uint32_t)(word & 7)));
+        return B2S_OK;
+    }
+    // the same into HOST memory
+    int32_t decode_host(int group, const uint8_t* in, uint64_t count, bool compressed, bool validate, void* out_host, const char* name) {
+        if (!count) return B2S_OK;
+        DevBuf out;
+        B2S_TRY(out.alloc(c, count * aff_bytes(c, group)));
+        B2S_TRY(decode(group, in, count, compressed, validate, out.p, name));
+        B2S_CUDA(c, cudaMemcpyAsync(out_host, out.p, count * aff_bytes(c, group), cudaMemcpyDeviceToHost, c->stream));
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+        return B2S_OK;
+    }
+};
+
+int32_t deserialize_points(Ctx* c, int group, const uint8_t* in, uint64_t len, uint64_t count, bool compressed, bool validate,
+                           void* out_host) {
+    const size_t pb = enc_bytes(c, group, compressed);
+    if (count > len / pb || count * pb != len)
+        return fail(c, B2S_ERR_INVALID_DATA, "deserialize: %llu bytes are not %llu points of %zu bytes", (unsigned long long)len,
+                    (unsigned long long)count, pb);
+    Stager st(c);
+    return st.decode_host(group, in, count, compressed, validate, out_host, group == 1 ? "g1" : "g2");
+}
+
+int32_t proof_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* a, void* b, void* cc) {
+    const size_t g1 = enc_bytes(c, 1, compressed), g2 = enc_bytes(c, 2, compressed);
+    if (len != 2 * g1 + g2) return fail(c, B2S_ERR_INVALID_DATA, "proof: %llu bytes, expected %zu", (unsigned long long)len, 2 * g1 + g2);
+    Stager st(c);
+    B2S_TRY(st.decode_host(1, in, 1, compressed, validate, a, "proof.a"));
+    B2S_TRY(st.decode_host(2, in + g1, 1, compressed, validate, b, "proof.b"));
+    return st.decode_host(1, in + g1 + g2, 1, compressed, validate, cc, "proof.c");
+}
+
+// Walks the framing of a serialized key: every Vec prefix is checked against the bytes that remain before anything is
+// allocated or decoded.
+struct Frame {
+    Ctx* c;
+    const uint8_t* in;
+    uint64_t len, at = 0;
+    bool compressed;
+    int32_t point(int group, uint64_t* off) {
+        const size_t pb = enc_bytes(c, group, compressed);
+        if (len - at < pb) return fail(c, B2S_ERR_INVALID_DATA, "key: truncated at byte %llu", (unsigned long long)at);
+        *off = at;
+        at += pb;
+        return B2S_OK;
+    }
+    int32_t vec(int group, const char* name, uint64_t* off, uint64_t* n) {
+        if (len - at < 8) return fail(c, B2S_ERR_INVALID_DATA, "key: truncated before the length of %s", name);
+        uint64_t v = 0;
+        for (int i = 0; i < 8; i++) v |= (uint64_t)in[at + i] << (8 * i);
+        at += 8;
+        const size_t pb = enc_bytes(c, group, compressed);
+        if (v > (len - at) / pb)
+            return fail(c, B2S_ERR_INVALID_DATA, "%s: length %llu exceeds the %llu bytes that remain", name, (unsigned long long)v,
+                        (unsigned long long)(len - at));
+        *off = at;
+        *n = v;
+        at += v * pb;
+        return B2S_OK;
+    }
+};
+struct VkFrame { uint64_t alpha, beta, gamma, delta, abc, n_abc; };
+static int32_t frame_vk(Frame& f, VkFrame& v) {
+    B2S_TRY(f.point(1, &v.alpha));
+    B2S_TRY(f.point(2, &v.beta));
+    B2S_TRY(f.point(2, &v.gamma));
+    B2S_TRY(f.point(2, &v.delta));
+    return f.vec(1, "gamma_abc_g1", &v.abc, &v.n_abc);
+}
+
+int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* alpha, void* beta, void* gamma,
+                       void* delta, void* abc, uint64_t cap_abc, uint64_t* n_abc, uint64_t* consumed) {
+    Frame f{c, in, len, 0, compressed};
+    VkFrame v;
+    B2S_TRY(frame_vk(f, v));
+    if (n_abc) *n_abc = v.n_abc;
+    if (consumed) *consumed = f.at;
+    if (!abc) return B2S_OK;
+    if (cap_abc < v.n_abc) return fail(c, B2S_ERR_INVALID_ARG, "vk_deserialize: gamma_abc_g1 has %llu points, room for %llu",
+                                       (unsigned long long)v.n_abc, (unsigned long long)cap_abc);
+    Stager st(c);
+    B2S_TRY(st.decode_host(1, in + v.alpha, 1, compressed, validate, alpha, "alpha_g1"));
+    B2S_TRY(st.decode_host(2, in + v.beta, 1, compressed, validate, beta, "beta_g2"));
+    B2S_TRY(st.decode_host(2, in + v.gamma, 1, compressed, validate, gamma, "gamma_g2"));
+    B2S_TRY(st.decode_host(2, in + v.delta, 1, compressed, validate, delta, "delta_g2"));
+    return st.decode_host(1, in + v.abc, v.n_abc, compressed, validate, abc, "gamma_abc_g1");
+}
+
+int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, b2s_pk** out) {
+    Frame f{c, in, len, 0, compressed};
+    VkFrame v;
+    uint64_t beta1, delta1;
+    struct Q { int group; const char* name; uint64_t off, n; DevBuf b2s_pk::*buf; } qs[5] = {
+        {1, "a_query", 0, 0, &b2s_pk::a_query}, {1, "b_g1_query", 0, 0, &b2s_pk::b_g1_query}, {2, "b_g2_query", 0, 0, &b2s_pk::b_g2_query},
+        {1, "h_query", 0, 0, &b2s_pk::h_query}, {1, "l_query", 0, 0, &b2s_pk::l_query}};
+    B2S_TRY(frame_vk(f, v));
+    B2S_TRY(f.point(1, &beta1));
+    B2S_TRY(f.point(1, &delta1));
+    for (Q& q : qs) B2S_TRY(f.vec(q.group, q.name, &q.off, &q.n));
+    if (f.at != len) return fail(c, B2S_ERR_INVALID_DATA, "pk: %llu trailing bytes", (unsigned long long)(len - f.at));
+    const uint64_t n_instance = v.n_abc, n_witness = qs[4].n, n_vars = n_instance + n_witness, domain = qs[3].n + 1;
+    if (qs[0].n != n_vars || qs[1].n != n_vars || qs[2].n != n_vars || (domain & (domain - 1)))
+        return fail(c, B2S_ERR_MALFORMED_VK, "pk: inconsistent dimensions (instance %llu, witness %llu, a %llu, b_g1 %llu, b_g2 %llu, h %llu)",
+                    (unsigned long long)n_instance, (unsigned long long)n_witness, (unsigned long long)qs[0].n, (unsigned long long)qs[1].n,
+                    (unsigned long long)qs[2].n, (unsigned long long)qs[3].n);
+    const size_t g1 = aff_bytes(c, 1), g2 = aff_bytes(c, 2);
+    b2s_pk* pk = new b2s_pk();
+    pk->n_instance = n_instance; pk->n_witness = n_witness; pk->domain_size = domain;
+    pk->a_len = pk->b1_len = pk->b2_len = n_vars; pk->h_len = qs[3].n; pk->l_len = n_witness;
+    auto body = [&]() -> int32_t {
+        Stager st(c);
+        DevBuf scratch;   // gamma_g2 and gamma_abc_g1: validated, not kept by the prover
+        B2S_TRY(scratch.alloc(c, std::max<size_t>(g2, std::max<uint64_t>(v.n_abc, 1) * g1)));
+        B2S_TRY(pk->consts_g1.alloc(c, 3 * g1));
+        B2S_TRY(pk->consts_g2.alloc(c, 2 * g2));
+        char* k1 = pk->consts_g1.as<char>();
+        char* k2 = pk->consts_g2.as<char>();
+        B2S_TRY(st.decode(1, in + v.alpha, 1, compressed, validate, k1, "alpha_g1"));
+        B2S_TRY(st.decode(2, in + v.beta, 1, compressed, validate, k2, "beta_g2"));
+        B2S_TRY(st.decode(2, in + v.gamma, 1, compressed, validate, scratch.p, "gamma_g2"));
+        B2S_TRY(st.decode(2, in + v.delta, 1, compressed, validate, k2 + g2, "delta_g2"));
+        B2S_TRY(st.decode(1, in + v.abc, v.n_abc, compressed, validate, scratch.p, "gamma_abc_g1"));
+        B2S_TRY(st.decode(1, in + beta1, 1, compressed, validate, k1 + g1, "beta_g1"));
+        B2S_TRY(st.decode(1, in + delta1, 1, compressed, validate, k1 + 2 * g1, "delta_g1"));
+        for (Q& q : qs) {   // room for the two extra points pk_finish appends
+            DevBuf& b = pk->*(q.buf);
+            B2S_TRY(b.alloc(c, (q.n + 2) * (q.group == 1 ? g1 : g2)));
+            B2S_TRY(st.decode(q.group, in + q.off, q.n, compressed, validate, b.p, q.name));
+        }
+        return pk_finish(c, pk);
+    };
+    const int32_t s = body();
+    if (s != B2S_OK) { delete pk; return s; }
+    *out = pk;
+    return B2S_OK;
+}
+
+}  // namespace b2s

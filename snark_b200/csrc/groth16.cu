@@ -89,16 +89,55 @@ __global__ void sum_shards_kernel(const XYZZ<F>* partials, uint32_t n_shards, ui
     sums[j] = acc;
 }
 
-// query ++ extras: `len` points from src, then (if this shard owns the end of the range) two extra points
-static int32_t copy_query(Ctx* c, DevBuf& dst, const void* src, uint64_t len, size_t pt, int32_t mem, const void* extra0,
-                          const void* extra1, cudaMemcpyKind kind) {
+// the query points of a key: `len` points from src, with room for the two extra points pk_finish appends
+static int32_t copy_query(Ctx* c, DevBuf& dst, const void* src, uint64_t len, size_t pt, cudaMemcpyKind kind) {
     B2S_TRY(dst.alloc(c, (len + 2) * pt));
-    char* d = dst.as<char>();
-    if (len) B2S_CUDA(c, cudaMemcpyAsync(d, src, len * pt, kind, c->stream));
-    B2S_CUDA(c, cudaMemsetAsync(d + len * pt, 0, 2 * pt, c->stream));   // O = all-zero bytes
-    if (extra0) B2S_CUDA(c, cudaMemcpyAsync(d + len * pt, extra0, pt, kind, c->stream));
-    if (extra1) B2S_CUDA(c, cudaMemcpyAsync(d + (len + 1) * pt, extra1, pt, kind, c->stream));
-    (void)mem;
+    if (len) B2S_CUDA(c, cudaMemcpyAsync(dst.p, src, len * pt, kind, c->stream));
+    return B2S_OK;
+}
+
+// What a key handle holds beyond its points, shared by pk_upload and pk_deserialize.  The constants and the query points
+// are on the device, each query buffer with room for two more points; this appends the extra (base, scalar) pairs of the
+// shard that owns the end of a range and builds the h-query table when it fits.  Synchronises the ctx stream.
+int32_t pk_finish(Ctx* c, b2s_pk* pk) {
+    const size_t fq = c->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
+    const size_t g1 = 2 * fq, g2 = 4 * fq;
+    const uint64_t n_vars = pk->n_instance + pk->n_witness;
+    pk->a_ext = (pk->a_off + pk->a_len == n_vars) ? 2 : 0;
+    pk->b1_ext = (pk->b1_off + pk->b1_len == n_vars) ? 2 : 0;
+    pk->b2_ext = (pk->b2_off + pk->b2_len == n_vars) ? 2 : 0;
+    const char* delta_g1 = pk->consts_g1.as<char>() + 2 * g1;
+    const char* delta_g2 = pk->consts_g2.as<char>() + g2;
+    // extras: a: [delta_1, O] (scalars r, s)   b1: [O, delta_1]   b2: [O, delta_2]   h, l: [O, O]
+    struct X { DevBuf* buf; uint64_t len; size_t pt; const char* e0; const char* e1; } xs[5] = {
+        {&pk->a_query, pk->a_len, g1, pk->a_ext ? delta_g1 : nullptr, nullptr},
+        {&pk->b_g1_query, pk->b1_len, g1, nullptr, pk->b1_ext ? delta_g1 : nullptr},
+        {&pk->b_g2_query, pk->b2_len, g2, nullptr, pk->b2_ext ? delta_g2 : nullptr},
+        {&pk->h_query, pk->h_len, g1, nullptr, nullptr},
+        {&pk->l_query, pk->l_len, g1, nullptr, nullptr}};
+    for (const X& x : xs) {
+        char* d = x.buf->as<char>() + x.len * x.pt;
+        B2S_CUDA(c, cudaMemsetAsync(d, 0, 2 * x.pt, c->stream));   // O = all-zero bytes
+        if (x.e0) B2S_CUDA(c, cudaMemcpyAsync(d, x.e0, x.pt, cudaMemcpyDeviceToDevice, c->stream));
+        if (x.e1) B2S_CUDA(c, cudaMemcpyAsync(d + x.pt, x.e1, x.pt, cudaMemcpyDeviceToDevice, c->stream));
+    }
+    // Fixed-base window table for the h query: its scalars (the quotient polynomial) are never repeated values, so this is
+    // the MSM that always pays the full Pippenger price; the other queries run over the witness, where the multiplicity-aware
+    // front end usually leaves little.  13 x the query (18 GiB at 2^24): only when it fits comfortably.
+    {
+        const char* env = getenv("B2S_PK_PRECOMP");
+        const uint64_t min_n = getenv("B2S_PK_PRECOMP_MIN") ? strtoull(getenv("B2S_PK_PRECOMP_MIN"), nullptr, 10) : (1ull << 18);
+        uint32_t cc = 0;
+        const uint32_t nw = msm_precompute_windows(c, pk->h_len, &cc);
+        size_t free_b = 0, total_b = 0;
+        cudaMemGetInfo(&free_b, &total_b);
+        const uint64_t need = (uint64_t)nw * pk->h_len * g1;
+        if (!(env && env[0] == '0') && pk->h_len >= min_n && (uint64_t)nw * pk->h_len < (1ull << 31) && need * 4 < (uint64_t)free_b) {
+            B2S_TRY(pk->h_table.alloc(c, need));
+            B2S_TRY(msm_precompute(c, 1, pk->h_query.p, pk->h_len, pk->h_table.p, &pk->h_pre));
+        }
+    }
+    B2S_CUDA(c, cudaStreamSynchronize(c->stream));
     return B2S_OK;
 }
 
@@ -116,9 +155,6 @@ int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
     pk->a_off = d->a_off; pk->a_len = d->a_len; pk->b1_off = d->b1_off; pk->b1_len = d->b1_len;
     pk->b2_off = d->b2_off; pk->b2_len = d->b2_len; pk->h_off = d->h_off; pk->h_len = d->h_len;
     pk->l_off = d->l_off; pk->l_len = d->l_len;
-    pk->a_ext = (d->a_off + d->a_len == n_vars) ? 2 : 0;
-    pk->b1_ext = (d->b1_off + d->b1_len == n_vars) ? 2 : 0;
-    pk->b2_ext = (d->b2_off + d->b2_len == n_vars) ? 2 : 0;
     const cudaMemcpyKind kind = mem == B2S_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     auto body = [&]() -> int32_t {
         B2S_TRY(pk->consts_g1.alloc(c, 3 * g1));
@@ -130,30 +166,12 @@ int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
         B2S_CUDA(c, cudaMemcpyAsync(p1 + 2 * g1, d->delta_g1, g1, kind, c->stream));
         B2S_CUDA(c, cudaMemcpyAsync(p2, d->beta_g2, g2, kind, c->stream));
         B2S_CUDA(c, cudaMemcpyAsync(p2 + g2, d->delta_g2, g2, kind, c->stream));
-        // extras: a: [delta_1, O] (scalars r, s)   b1: [O, delta_1]   b2: [O, delta_2]
-        B2S_TRY(copy_query(c, pk->a_query, d->a_query, d->a_len, g1, mem, pk->a_ext ? d->delta_g1 : nullptr, nullptr, kind));
-        B2S_TRY(copy_query(c, pk->b_g1_query, d->b_g1_query, d->b1_len, g1, mem, nullptr, pk->b1_ext ? d->delta_g1 : nullptr, kind));
-        B2S_TRY(copy_query(c, pk->b_g2_query, d->b_g2_query, d->b2_len, g2, mem, nullptr, pk->b2_ext ? d->delta_g2 : nullptr, kind));
-        B2S_TRY(copy_query(c, pk->h_query, d->h_query, d->h_len, g1, mem, nullptr, nullptr, kind));
-        B2S_TRY(copy_query(c, pk->l_query, d->l_query, d->l_len, g1, mem, nullptr, nullptr, kind));
-        // Fixed-base window table for the h query: its scalars (the quotient polynomial) are never repeated values, so this is
-        // the MSM that always pays the full Pippenger price; the other queries run over the witness, where the multiplicity-aware
-        // front end usually leaves little.  13 x the query (18 GiB at 2^24): only when it fits comfortably.
-        {
-            const char* env = getenv("B2S_PK_PRECOMP");
-            const uint64_t min_n = getenv("B2S_PK_PRECOMP_MIN") ? strtoull(getenv("B2S_PK_PRECOMP_MIN"), nullptr, 10) : (1ull << 18);
-            uint32_t cc = 0;
-            const uint32_t nw = msm_precompute_windows(c, d->h_len, &cc);
-            size_t free_b = 0, total_b = 0;
-            cudaMemGetInfo(&free_b, &total_b);
-            const uint64_t need = (uint64_t)nw * d->h_len * g1;
-            if (!(env && env[0] == '0') && d->h_len >= min_n && (uint64_t)nw * d->h_len < (1ull << 31) && need * 4 < (uint64_t)free_b) {
-                B2S_TRY(pk->h_table.alloc(c, need));
-                B2S_TRY(msm_precompute(c, 1, pk->h_query.p, d->h_len, pk->h_table.p, &pk->h_pre));
-            }
-        }
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        return B2S_OK;
+        B2S_TRY(copy_query(c, pk->a_query, d->a_query, d->a_len, g1, kind));
+        B2S_TRY(copy_query(c, pk->b_g1_query, d->b_g1_query, d->b1_len, g1, kind));
+        B2S_TRY(copy_query(c, pk->b_g2_query, d->b_g2_query, d->b2_len, g2, kind));
+        B2S_TRY(copy_query(c, pk->h_query, d->h_query, d->h_len, g1, kind));
+        B2S_TRY(copy_query(c, pk->l_query, d->l_query, d->l_len, g1, kind));
+        return pk_finish(c, pk);
     };
     const int32_t st = body();
     if (st != B2S_OK) { delete pk; return st; }

@@ -20,30 +20,12 @@
 #include <vector>
 
 #include "common.cuh"
+#include "deserialize.cuh"   // y_is_larger
 
 namespace b2s {
 
 struct CanonPoint { uint32_t x[24]; uint32_t y[24]; uint32_t flags; uint32_t pad[3]; };   // up to 2 x 12 limbs each; flags: 1 = inf, 2 = y larger
 
-template <class B>
-__device__ __forceinline__ int cmp_canon(const B& a, const B& b) {   // canonical (non-Montgomery) values
-    for (int i = B::N - 1; i >= 0; i--) {
-        if (a.v[i] != b.v[i]) return a.v[i] > b.v[i] ? 1 : -1;
-    }
-    return 0;
-}
-template <class P>
-__device__ __forceinline__ bool y_is_larger(const Fp<P>& y) {
-    const Fp<P> a = y.from_mont(), b = y.neg().from_mont();
-    return cmp_canon(a, b) > 0;
-}
-template <class P>
-__device__ __forceinline__ bool y_is_larger(const Fp2<P>& y) {
-    const Fp2<P> n = y.neg();
-    const int c1 = cmp_canon(y.c1.from_mont(), n.c1.from_mont());
-    if (c1 != 0) return c1 > 0;
-    return cmp_canon(y.c0.from_mont(), n.c0.from_mont()) > 0;
-}
 template <class P>
 __device__ __forceinline__ void put_canon(uint32_t* o, const Fp<P>& x) {
     const Fp<P> c = x.from_mont();

@@ -83,6 +83,12 @@ SIGNATURES = {
     "b2s_vk_serialize": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_uint64, c_int32, c_void_p, c_uint64]),
     "b2s_pk_serialized_size": (c_uint64, [c_void_p, c_void_p, c_uint64, c_int32]),
     "b2s_pk_serialize": (c_int32, [c_void_p, c_void_p, c_void_p, c_uint64, c_int32, c_void_p, c_uint64]),
+    "b2s_deserialize_g1": (c_int32, [c_void_p, c_void_p, c_uint64, c_uint64, c_int32, c_int32, c_void_p]),
+    "b2s_deserialize_g2": (c_int32, [c_void_p, c_void_p, c_uint64, c_uint64, c_int32, c_int32, c_void_p]),
+    "b2s_proof_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    "b2s_vk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32] + [c_void_p] * 5
+                           + [c_uint64, POINTER(c_uint64), POINTER(c_uint64)]),
+    "b2s_pk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_fixed_base_g1": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
     "b2s_fixed_base_g2": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
     "b2s_group_unique_id": (c_int32, [c_void_p]),
@@ -338,6 +344,47 @@ class Backend:
         out = np.zeros(int(self.lib.b2s_pk_serialized_size(self.h, pk, len(vk), int(compressed))), dtype=np.uint8)
         self._ck(self.lib.b2s_pk_serialize(self.h, pk, vk.ctypes.data, len(vk), int(compressed), out.ctypes.data, out.nbytes))
         return out.tobytes()
+
+    # ---- CanonicalDeserialize (decoding and validation on the GPU) ------------------------------------------------
+    def deserialize_points(self, group, data, count=None, compressed=True, validate=True):
+        """`count` encoded points (default: as many as `data` holds) -> HOST affine Montgomery limbs (uint32)."""
+        per = (self.fq_bytes if group == 1 else 2 * self.fq_bytes) * (1 if compressed else 2)
+        buf = np.frombuffer(bytes(data), dtype=np.uint8)
+        count = len(buf) // per if count is None else count
+        out = np.zeros(max(count, 1) * (self.g1_bytes if group == 1 else self.g2_bytes) // 4, dtype=np.uint32)
+        fn = self.lib.b2s_deserialize_g1 if group == 1 else self.lib.b2s_deserialize_g2
+        self._ck(fn(self.h, buf.ctypes.data, len(buf), count, int(compressed), int(validate), out.ctypes.data))
+        return out[: count * (self.g1_bytes if group == 1 else self.g2_bytes) // 4]
+
+    def proof_from_bytes(self, data, compressed=True, validate=True):
+        """Proof bytes -> (a, b, c) HOST affine arrays, the layout groth16_prove returns."""
+        buf = np.frombuffer(bytes(data), dtype=np.uint8)
+        a, b, c = self._proof_bufs()
+        self._ck(self.lib.b2s_proof_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), a.ctypes.data,
+                                                b.ctypes.data, c.ctypes.data))
+        return a, b, c
+
+    def vk_from_bytes(self, data, compressed=True, validate=True):
+        """VerifyingKey from the start of `data` -> (vk dict in the layout groth16_setup returns, bytes consumed)."""
+        buf = np.frombuffer(bytes(data), dtype=np.uint8)
+        n, used = c_uint64(), c_uint64()
+        self._ck(self.lib.b2s_vk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), None, None, None, None,
+                                             None, 0, ctypes.byref(n), ctypes.byref(used)))
+        vk = {"alpha_g1": np.zeros(self.g1_bytes // 4, dtype=np.uint32), "beta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
+              "gamma_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32), "delta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
+              "gamma_abc_g1": np.zeros(max(n.value, 1) * self.g1_bytes // 4, dtype=np.uint32)}
+        self._ck(self.lib.b2s_vk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), vk["alpha_g1"].ctypes.data,
+                                             vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data, vk["delta_g2"].ctypes.data,
+                                             vk["gamma_abc_g1"].ctypes.data, n.value, ctypes.byref(n), ctypes.byref(used)))
+        vk["gamma_abc_g1"] = vk["gamma_abc_g1"][: n.value * self.g1_bytes // 4]
+        return vk, used.value
+
+    def pk_from_bytes(self, data, compressed=True, validate=True):
+        """ark-groth16 ProvingKey bytes -> device-resident full key handle (as pk_upload returns)."""
+        buf = np.frombuffer(bytes(data), dtype=np.uint8)
+        h = c_void_p()
+        self._ck(self.lib.b2s_pk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), ctypes.byref(h)))
+        return h
 
     def pk_free(self, pk):
         self.lib.b2s_pk_free(self.h, pk)

@@ -91,15 +91,126 @@ def curve_extra(p, n, g1, g2, b, b2):
     return s
 
 
+# ---- point decoding constants (snark_b200/csrc/deserialize.cuh) ----------------------------------------------------
+# Subgroup criteria: BLS12-381 G1 phi(P) = -[x^2]P with phi(x, y) = (beta x, y); BLS12-381 G2 psi(P) = [x]P; BN254 G2
+# psi(P) = [6 x^2]P, where psi(x, y) = (conj(x) cx, conj(y) cy) is the untwist-Frobenius-twist map.  beta and the psi
+# coefficients are chosen here so that the curve's generator satisfies its criterion, so the header cannot carry the
+# wrong cube root of unity or the inverse coefficients.
+BLS_X_ABS = 0xd201000000010000     # BLS12-381 x = -0xd201000000010000
+BN_X = 4965661367192848881          # BN254 x (p = 36x^4 + 36x^3 + 24x^2 + 6x + 1)
+
+
+def f2_mul(p, a, b):
+    return ((a[0] * b[0] - a[1] * b[1]) % p, (a[0] * b[1] + a[1] * b[0]) % p)
+
+
+def f2_pow(p, a, e):
+    r = (1, 0)
+    for bit in bin(e)[2:]:
+        r = f2_mul(p, r, r)
+        if bit == "1":
+            r = f2_mul(p, r, a)
+    return r
+
+
+def f2_inv(p, a):
+    n = pow(a[0] * a[0] + a[1] * a[1], -1, p)
+    return (a[0] * n % p, (-a[1]) * n % p)
+
+
+def ec_mul(p, ext, P, k):
+    """k * P on y^2 = x^3 + b (affine, a = 0) over Fq (ext False) or Fq2 (ext True); None = infinity."""
+    mul = (lambda a, b: f2_mul(p, a, b)) if ext else (lambda a, b: a * b % p)
+    inv = (lambda a: f2_inv(p, a)) if ext else (lambda a: pow(a, -1, p))
+    sub = (lambda a, b: ((a[0] - b[0]) % p, (a[1] - b[1]) % p)) if ext else (lambda a, b: (a - b) % p)
+    three = (3, 0) if ext else 3
+    two = (2, 0) if ext else 2
+
+    def add(A, B):
+        if A is None:
+            return B
+        if B is None:
+            return A
+        if A[0] == B[0]:
+            if A[1] != B[1]:
+                return None
+            lam = mul(mul(three, mul(A[0], A[0])), inv(mul(two, A[1])))
+        else:
+            lam = mul(sub(B[1], A[1]), inv(sub(B[0], A[0])))
+        x3 = sub(sub(mul(lam, lam), A[0]), B[0])
+        return (x3, sub(mul(lam, sub(A[0], x3)), A[1]))
+
+    acc = None
+    for bit in bin(k)[2:]:
+        acc = add(acc, acc)
+        if bit == "1":
+            acc = add(acc, P)
+    return acc
+
+
+def bls_beta():
+    p, r = BLS_P, BLS_R
+    for g in range(2, 100):
+        w = pow(g, (p - 1) // 3, p)
+        if w != 1:
+            break
+    lam = (-BLS_X_ABS * BLS_X_ABS) % r
+    target = ec_mul(p, False, BLS_G1, lam)
+    hits = [b for b in (w, w * w % p) if (b * BLS_G1[0] % p, BLS_G1[1]) == target]
+    assert len(hits) == 1
+    return hits[0]
+
+
+def psi_coeffs(p, r, xi, gen, lam):
+    """(cx, cy) with psi(gen) = [lam] gen for cx = xi^(e (p-1)/3), cy = xi^(e (p-1)/2), e = +1 or -1."""
+    x, y = (gen[0], gen[1]), (gen[2], gen[3])
+    target = ec_mul(p, True, (x, y), lam % r)
+    hits = []
+    for e in (1, -1):
+        base = xi if e == 1 else f2_inv(p, xi)
+        cx, cy = f2_pow(p, base, (p - 1) // 3), f2_pow(p, base, (p - 1) // 2)
+        if (f2_mul(p, (x[0], -x[1] % p), cx), f2_mul(p, (y[0], -y[1] % p), cy)) == target:
+            hits.append((cx, cy))
+    assert len(hits) == 1
+    return hits[0]
+
+
+def words(x, n):
+    return "{" + ", ".join("0x%08xu" % w for w in limbs(x, n)) + "}"
+
+
+def decode_extra(p, n, beta, psi, endo_scalar, endo_words):
+    """Constants of deserialize.cuh: sqrt exponent, 1/2, beta, psi coefficients (Montgomery) and the subgroup scalar (plain)."""
+    R = 1 << (32 * n)
+    fn = lambda nm, val: (
+        "    B2S_HD static constexpr uint32_t %s(int i) { constexpr uint32_t t[%d] = %s; return t[i]; }\n"
+        % (nm, n, arr(val * R % p, n))
+    )
+    s = "    // point decoding (deserialize.cuh): (p - 3) / 4 in plain words; Montgomery forms of 1/2, the cube root of unity\n"
+    s += "    // beta of the G1 endomorphism (1 when unused) and the psi coefficients cx, cy of G2; the subgroup-test scalar in\n"
+    s += "    // plain words (BLS12-381: |x|; BN254: 6 x^2)\n"
+    s += "    B2S_HD static constexpr uint32_t sqrt_exp(int i) { constexpr uint32_t t[%d] = %s; return t[i]; }\n" % (n, words((p - 3) // 4, n))
+    s += fn("fq_half", pow(2, -1, p)) + fn("beta", beta)
+    s += fn("psi_x0", psi[0][0]) + fn("psi_x1", psi[0][1]) + fn("psi_y0", psi[1][0]) + fn("psi_y1", psi[1][1])
+    s += "    static constexpr int ENDO_WORDS = %d;\n" % endo_words
+    s += "    B2S_HD static constexpr uint32_t endo_scalar(int i) { constexpr uint32_t t[%d] = %s; return t[i]; }\n" % (
+        endo_words, words(endo_scalar, endo_words))
+    return s
+
+
 def main():
     out = "// GENERATED by tools/gen_field_params.py -- do not edit.\n"
     out += "// Montgomery constants (R = 2^(32 N)) for BLS12-381 / BN254 base and scalar fields.\n"
     out += "#pragma once\n#include <cstdint>\n#include \"ff.cuh\"\n\nnamespace b2s {\n\n"
     inv82 = pow(82, -1, BN_P)
     bn_b2 = (27 * inv82 % BN_P, (-3 * inv82) % BN_P)
-    out += field_struct("BlsFqP", BLS_P, 12, curve_extra(BLS_P, 12, BLS_G1, BLS_G2, 4, (4, 4)))
+    bls_psi = psi_coeffs(BLS_P, BLS_R, (1, 1), BLS_G2, -BLS_X_ABS)
+    bn_psi = psi_coeffs(BN_P, BN_R, (9, 1), BN_G2, 6 * BN_X * BN_X)
+    out += field_struct("BlsFqP", BLS_P, 12, curve_extra(BLS_P, 12, BLS_G1, BLS_G2, 4, (4, 4))
+                        + decode_extra(BLS_P, 12, bls_beta(), bls_psi, BLS_X_ABS, 2))
     out += field_struct("BlsFrP", BLS_R, 8, fr_extra(BLS_R, 8, 7, 32))
-    out += field_struct("BnFqP", BN_P, 8, curve_extra(BN_P, 8, BN_G1, BN_G2, 3, bn_b2))
+    out += field_struct("BnFqP", BN_P, 8, curve_extra(BN_P, 8, BN_G1, BN_G2, 3, bn_b2)
+                        + decode_extra(BN_P, 8, 1, bn_psi, 6 * BN_X * BN_X, 4))
     out += field_struct("BnFrP", BN_R, 8, fr_extra(BN_R, 8, 5, 28))
     out += "}  // namespace b2s\n"
     path = os.path.join(os.path.dirname(__file__), "..", "snark_b200", "csrc", "field_params.h")
