@@ -21,8 +21,8 @@ int32_t poly_geom_run(Ctx* c, const void* c_host, const void* s_host, uint64_t n
 int32_t poly_eval_run(Ctx* c, const void* coeffs, uint64_t n, const void* z_host, int32_t mem, void* out_host);
 int32_t fixed_base_run(Ctx* c, int group, const void* scalars_dev, uint64_t n, bool mont, void* out_dev);
 void fixed_base_free(Ctx* c);
-int32_t serialize_points(Ctx* c, int group, const void* affine_host, uint32_t count, uint8_t* out, uint64_t cap);
 int32_t serialize_points_ex(Ctx* c, int group, const void* affine, int32_t mem, uint64_t count, bool compressed, uint8_t* out, uint64_t cap);
+int32_t proof_serialize(Ctx* c, const void* a_g1, const void* b_g2, const void* c_g1, bool compressed, uint8_t* out, uint64_t cap);
 uint64_t vk_serialized_size(Ctx* c, uint64_t n_gamma_abc, bool compressed);
 int32_t vk_serialize(Ctx* c, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2, const void* gamma_abc,
                      uint64_t n_gamma_abc, bool compressed, uint8_t* out, uint64_t cap);
@@ -40,11 +40,6 @@ int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed,
     if (!(ctx)) return B2S_ERR_INVALID_ARG;            \
     std::lock_guard<std::mutex> guard__((ctx)->mu);    \
     if (cudaSetDevice((ctx)->device) != cudaSuccess) return fail(ctx, B2S_ERR_NO_DEVICE, "cudaSetDevice(%d) failed", (ctx)->device)
-
-static void sizes_for(int curve, uint32_t out[6]) {
-    const uint32_t fq = curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    out[0] = 32; out[1] = fq; out[2] = 2 * fq; out[3] = 4 * fq; out[4] = 4 * fq; out[5] = 8 * fq;
-}
 
 extern "C" {
 
@@ -121,7 +116,8 @@ const char* b2s_last_error(const b2s_ctx* ctx) { return ctx ? ctx->err.c_str() :
 
 int32_t b2s_sizes(const b2s_ctx* ctx, uint32_t out[6]) {
     if (!ctx || !out) return B2S_ERR_INVALID_ARG;
-    sizes_for(ctx->curve, out);
+    const Sizes z = sizes(ctx);
+    out[0] = z.fr; out[1] = z.fq; out[2] = z.g1; out[3] = z.g2; out[4] = z.g1x; out[5] = z.g2x;
     return B2S_OK;
 }
 
@@ -156,9 +152,8 @@ static int32_t msm_common(b2s_ctx* ctx, int group, const void* bases, const void
                           int32_t mem, void* out, bool affine) {
     if ((!bases || !scalars) && n) return fail(ctx, B2S_ERR_INVALID_ARG, "msm: null input");
     if (!out) return fail(ctx, B2S_ERR_INVALID_ARG, "msm: null output");
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
-    const size_t pt = sz[1 + group], xyzz = sz[3 + group];
+    const Sizes z = sizes(ctx);
+    const size_t pt = z.aff(group), xyzz = z.xyzz(group);
     InBuf b, s;
     B2S_TRY(b.bind(ctx, bases, n * pt, mem));
     B2S_TRY(s.bind(ctx, scalars, n * 32, mem));
@@ -199,14 +194,13 @@ int32_t b2s_msm_g2_partial(b2s_ctx* ctx, const void* bases, const void* scalars,
 
 static int32_t sum_common(b2s_ctx* ctx, int group, const void* xyzz, uint32_t count, void* out_affine) {
     if (!xyzz || !out_affine || count == 0) return fail(ctx, B2S_ERR_INVALID_ARG, "group sum: bad arguments");
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
+    const Sizes z = sizes(ctx);
     InBuf in;
-    B2S_TRY(in.bind(ctx, xyzz, (size_t)count * sz[3 + group], B2S_MEM_HOST));
+    B2S_TRY(in.bind(ctx, xyzz, (size_t)count * z.xyzz(group), B2S_MEM_HOST));
     DevBuf aff;
-    B2S_TRY(aff.alloc(ctx, sz[1 + group]));
+    B2S_TRY(aff.alloc(ctx, z.aff(group)));
     B2S_TRY(group_sum_to_affine(ctx, group, in.dptr, count, aff.p));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_affine, aff.p, sz[1 + group], cudaMemcpyDeviceToHost, ctx->stream));
+    B2S_CUDA(ctx, cudaMemcpyAsync(out_affine, aff.p, z.aff(group), cudaMemcpyDeviceToHost, ctx->stream));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2S_OK;
 }
@@ -250,9 +244,7 @@ int32_t b2s_group_op(b2s_ctx* ctx, int32_t group, int32_t op, const void* a, con
 // ---- fixed-base batch multiplication -----------------------------------------------------------
 static int32_t fixed_base_common(b2s_ctx* ctx, int group, const void* scalars, uint64_t n, int32_t mont, int32_t mem, void* out) {
     if ((!scalars || !out) && n) return fail(ctx, B2S_ERR_INVALID_ARG, "fixed_base: null buffer");
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
-    const size_t pt = sz[1 + group];
+    const size_t pt = sizes(ctx).aff(group);
     InBuf s;
     B2S_TRY(s.bind(ctx, scalars, n * 32, mem));
     if (mem == B2S_MEM_DEVICE) return fixed_base_run(ctx, group, s.dptr, n, mont != 0, out);
@@ -275,11 +267,40 @@ int32_t b2s_fixed_base_g2(b2s_ctx* ctx, const void* scalars, uint64_t n, int32_t
 }  // extern "C"
 
 // ---- R1CS / witness map / Groth16 --------------------------------------------------------------
-static int32_t check_full_key(b2s_ctx* ctx, const b2s_pk* pk) {
-    const uint64_t n_vars = pk->n_instance + pk->n_witness;
-    if (pk->a_len != n_vars || pk->b1_len != n_vars || pk->b2_len != n_vars || pk->l_len != pk->n_witness ||
-        pk->h_len + 1 != pk->domain_size)
-        return fail(ctx, B2S_ERR_MALFORMED_VK, "prove: needs a full (unsharded) proving key");
+// The prove entry points take z as two host pieces (z_dev == nullptr) or as one device array.
+static bool z_missing(const b2s_r1cs* m, const void* z_inst, const void* z_wit, const void* z_dev) {
+    return !z_dev && (!z_inst || (!z_wit && m->n_witness));
+}
+
+// one proof on one GPU with a full key
+static int32_t prove_full(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_inst, const void* z_wit, const void* z_dev,
+                          const void* r, const void* s, void* out_a_g1, void* out_b_g2, void* out_c_g1) {
+    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove: null key or matrices");
+    if (z_missing(m, z_inst, z_wit, z_dev) || !r || !s) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove: null assignment");
+    if (!out_a_g1 || !out_b_g2 || !out_c_g1) return fail(ctx, B2S_ERR_INVALID_ARG, "prove: null output");
+    if (!pk_is_full(pk)) return fail(ctx, B2S_ERR_MALFORMED_VK, "prove: needs a full (unsharded) proving key");
+    const Sizes z = sizes(ctx);
+    DevBuf g1, g2;
+    B2S_TRY(g1.alloc(ctx, 4 * z.g1x));
+    B2S_TRY(g2.alloc(ctx, z.g2x));
+    B2S_TRY(groth16_shard(ctx, pk, m, z_inst, z_wit, z_dev, r, s, g1.p, g2.p));
+    return groth16_finish(ctx, pk, g1.p, g2.p, 1, r, s, out_a_g1, out_b_g2, out_c_g1);
+}
+
+// one shard's partial sums, to the host
+static int32_t prove_partial(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_inst, const void* z_wit, const void* z_dev,
+                             const void* r, const void* s, void* out_g1_partials, void* out_g2_partial) {
+    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove_shard: null key or matrices");
+    if (z_missing(m, z_inst, z_wit, z_dev) || !r || !s || !out_g1_partials || !out_g2_partial)
+        return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove_shard: null assignment or output");
+    const Sizes z = sizes(ctx);
+    DevBuf g1, g2;
+    B2S_TRY(g1.alloc(ctx, 4 * z.g1x));
+    B2S_TRY(g2.alloc(ctx, z.g2x));
+    B2S_TRY(groth16_shard(ctx, pk, m, z_inst, z_wit, z_dev, r, s, g1.p, g2.p));
+    B2S_CUDA(ctx, cudaMemcpyAsync(out_g1_partials, g1.p, 4 * z.g1x, cudaMemcpyDeviceToHost, ctx->stream));
+    B2S_CUDA(ctx, cudaMemcpyAsync(out_g2_partial, g2.p, z.g2x, cudaMemcpyDeviceToHost, ctx->stream));
+    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2S_OK;
 }
 extern "C" {
@@ -391,19 +412,7 @@ int32_t b2s_groth16_prove_shard(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* 
                                 const void* z_witness, const void* r, const void* s, void* out_g1_partials,
                                 void* out_g2_partial) {
     LOCK(ctx);
-    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove_shard: null key or matrices");
-    if (!z_instance || (!z_witness && m->n_witness) || !r || !s || !out_g1_partials || !out_g2_partial)
-        return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove_shard: null assignment or output");
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
-    DevBuf g1, g2;
-    B2S_TRY(g1.alloc(ctx, 4 * sz[4]));
-    B2S_TRY(g2.alloc(ctx, sz[5]));
-    B2S_TRY(groth16_shard(ctx, pk, m, z_instance, z_witness, nullptr, r, s, g1.p, g2.p));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_g1_partials, g1.p, 4 * sz[4], cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_g2_partial, g2.p, sz[5], cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    return prove_partial(ctx, pk, m, z_instance, z_witness, nullptr, r, s, out_g1_partials, out_g2_partial);
 }
 
 int32_t b2s_groth16_finish(b2s_ctx* ctx, const b2s_pk* pk, const void* g1_partials, const void* g2_partials,
@@ -412,62 +421,29 @@ int32_t b2s_groth16_finish(b2s_ctx* ctx, const b2s_pk* pk, const void* g1_partia
     if (!pk) return fail(ctx, B2S_ERR_MISSING_CS, "finish: null key");
     if (!g1_partials || !g2_partials || !n_shards || !r || !s || !out_a_g1 || !out_b_g2 || !out_c_g1)
         return fail(ctx, B2S_ERR_INVALID_ARG, "finish: null argument");
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
+    const Sizes z = sizes(ctx);
     InBuf p1, p2;
-    B2S_TRY(p1.bind(ctx, g1_partials, (size_t)n_shards * 4 * sz[4], B2S_MEM_HOST));
-    B2S_TRY(p2.bind(ctx, g2_partials, (size_t)n_shards * sz[5], B2S_MEM_HOST));
+    B2S_TRY(p1.bind(ctx, g1_partials, (size_t)n_shards * 4 * z.g1x, B2S_MEM_HOST));
+    B2S_TRY(p2.bind(ctx, g2_partials, (size_t)n_shards * z.g2x, B2S_MEM_HOST));
     return groth16_finish(ctx, pk, p1.dptr, p2.dptr, n_shards, r, s, out_a_g1, out_b_g2, out_c_g1);
 }
 
 int32_t b2s_groth16_prove(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_instance, const void* z_witness,
                           const void* r, const void* s, void* out_a_g1, void* out_b_g2, void* out_c_g1) {
     LOCK(ctx);
-    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove: null key or matrices");
-    if (!z_instance || (!z_witness && m->n_witness) || !r || !s) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove: null assignment");
-    if (!out_a_g1 || !out_b_g2 || !out_c_g1) return fail(ctx, B2S_ERR_INVALID_ARG, "prove: null output");
-    B2S_TRY(check_full_key(ctx, pk));
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
-    DevBuf g1, g2;
-    B2S_TRY(g1.alloc(ctx, 4 * sz[4]));
-    B2S_TRY(g2.alloc(ctx, sz[5]));
-    B2S_TRY(groth16_shard(ctx, pk, m, z_instance, z_witness, nullptr, r, s, g1.p, g2.p));
-    return groth16_finish(ctx, pk, g1.p, g2.p, 1, r, s, out_a_g1, out_b_g2, out_c_g1);
+    return prove_full(ctx, pk, m, z_instance, z_witness, nullptr, r, s, out_a_g1, out_b_g2, out_c_g1);
 }
-
 
 int32_t b2s_groth16_prove_resident(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void* r,
                                    const void* s, void* out_a_g1, void* out_b_g2, void* out_c_g1) {
     LOCK(ctx);
-    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove: null key or matrices");
-    if (!z_dev || !r || !s) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove: null assignment");
-    if (!out_a_g1 || !out_b_g2 || !out_c_g1) return fail(ctx, B2S_ERR_INVALID_ARG, "prove: null output");
-    B2S_TRY(check_full_key(ctx, pk));
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
-    DevBuf g1, g2;
-    B2S_TRY(g1.alloc(ctx, 4 * sz[4]));
-    B2S_TRY(g2.alloc(ctx, sz[5]));
-    B2S_TRY(groth16_shard(ctx, pk, m, nullptr, nullptr, z_dev, r, s, g1.p, g2.p));
-    return groth16_finish(ctx, pk, g1.p, g2.p, 1, r, s, out_a_g1, out_b_g2, out_c_g1);
+    return prove_full(ctx, pk, m, nullptr, nullptr, z_dev, r, s, out_a_g1, out_b_g2, out_c_g1);
 }
 
 int32_t b2s_groth16_prove_shard_resident(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void* r,
                                          const void* s, void* out_g1_partials, void* out_g2_partial) {
     LOCK(ctx);
-    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove_shard: null key or matrices");
-    if (!z_dev || !r || !s || !out_g1_partials || !out_g2_partial) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove_shard: null argument");
-    uint32_t sz[6];
-    sizes_for(ctx->curve, sz);
-    DevBuf g1, g2;
-    B2S_TRY(g1.alloc(ctx, 4 * sz[4]));
-    B2S_TRY(g2.alloc(ctx, sz[5]));
-    B2S_TRY(groth16_shard(ctx, pk, m, nullptr, nullptr, z_dev, r, s, g1.p, g2.p));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_g1_partials, g1.p, 4 * sz[4], cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_g2_partial, g2.p, sz[5], cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    return prove_partial(ctx, pk, m, nullptr, nullptr, z_dev, r, s, out_g1_partials, out_g2_partial);
 }
 
 int32_t b2s_profile_enable(b2s_ctx* ctx, int32_t on) {
@@ -536,12 +512,12 @@ int32_t b2s_pk_query(b2s_ctx* ctx, const b2s_pk* pk, int32_t which, void* out, u
 int32_t b2s_serialize_g1_compressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap) {
     LOCK(ctx);
     if ((!affine || !out) && count) return fail(ctx, B2S_ERR_INVALID_ARG, "serialize: null buffer");
-    return serialize_points(ctx, 1, affine, count, out, cap);
+    return serialize_points_ex(ctx, 1, affine, B2S_MEM_HOST, count, true, out, cap);
 }
 int32_t b2s_serialize_g2_compressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap) {
     LOCK(ctx);
     if ((!affine || !out) && count) return fail(ctx, B2S_ERR_INVALID_ARG, "serialize: null buffer");
-    return serialize_points(ctx, 2, affine, count, out, cap);
+    return serialize_points_ex(ctx, 2, affine, B2S_MEM_HOST, count, true, out, cap);
 }
 int32_t b2s_serialize_g1_uncompressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap) {
     LOCK(ctx);
@@ -556,11 +532,7 @@ int32_t b2s_serialize_g2_uncompressed(b2s_ctx* ctx, const void* affine, uint32_t
 int32_t b2s_proof_serialize_uncompressed(b2s_ctx* ctx, const void* a_g1, const void* b_g2, const void* c_g1, uint8_t* out, uint64_t cap) {
     LOCK(ctx);
     if (!a_g1 || !b_g2 || !c_g1 || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "proof_serialize: null buffer");
-    const uint64_t fq = ctx->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    if (cap < 8 * fq) return fail(ctx, B2S_ERR_INVALID_ARG, "proof_serialize: output buffer too small");
-    B2S_TRY(serialize_points_ex(ctx, 1, a_g1, B2S_MEM_HOST, 1, false, out, 2 * fq));
-    B2S_TRY(serialize_points_ex(ctx, 2, b_g2, B2S_MEM_HOST, 1, false, out + 2 * fq, 4 * fq));
-    return serialize_points_ex(ctx, 1, c_g1, B2S_MEM_HOST, 1, false, out + 6 * fq, 2 * fq);
+    return proof_serialize(ctx, a_g1, b_g2, c_g1, false, out, cap);
 }
 uint64_t b2s_vk_serialized_size(const b2s_ctx* ctx, uint64_t n_gamma_abc, int32_t compressed) {
     return ctx ? vk_serialized_size(const_cast<b2s_ctx*>(ctx), n_gamma_abc, compressed != 0) : 0;
@@ -586,11 +558,7 @@ int32_t b2s_proof_serialize_compressed(b2s_ctx* ctx, const void* a_g1, const voi
                                        uint64_t cap) {
     LOCK(ctx);
     if (!a_g1 || !b_g2 || !c_g1 || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "proof_serialize: null buffer");
-    const uint64_t fq = ctx->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    if (cap < 4 * fq) return fail(ctx, B2S_ERR_INVALID_ARG, "proof_serialize: output buffer too small");
-    B2S_TRY(serialize_points(ctx, 1, a_g1, 1, out, fq));
-    B2S_TRY(serialize_points(ctx, 2, b_g2, 1, out + fq, 2 * fq));
-    return serialize_points(ctx, 1, c_g1, 1, out + 3 * fq, fq);
+    return proof_serialize(ctx, a_g1, b_g2, c_g1, true, out, cap);
 }
 
 int32_t b2s_deserialize_g1(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t count, int32_t compressed, int32_t validate,

@@ -177,6 +177,30 @@ inline int32_t dispatch_curve(Ctx* c, F&& f) {
     return fail(c, B2S_ERR_INVALID_ARG, "unknown curve id %d", c->curve);
 }
 
+// Byte sizes of the ctx curve's elements as the kernels lay them out, in the order of b2s_sizes' out[6].
+struct Sizes {
+    size_t fr, fq, g1, g2, g1x, g2x;   // Fr, Fq, affine G1 / G2, XYZZ G1 / G2
+    size_t aff(int group) const { return group == 1 ? g1 : g2; }
+    size_t xyzz(int group) const { return group == 1 ? g1x : g2x; }
+    // ark-serialize encoding of one point: x only when compressed, x || y otherwise
+    size_t enc(int group, bool compressed) const { return compressed ? aff(group) / 2 : aff(group); }
+};
+inline Sizes sizes(const Ctx* c) {
+    Sizes s{};
+    // fail() writes the ctx only for an unknown curve, which b2s_ctx_create rejects
+    dispatch_curve(const_cast<Ctx*>(c), [&](auto curve) {
+        using C = decltype(curve);
+        using Fq = typename C::Fq;
+        static_assert(sizeof(typename C::G1Affine) == 2 * sizeof(Fq) && sizeof(typename C::G2Affine) == 4 * sizeof(Fq) &&
+                          sizeof(typename C::G1) == 4 * sizeof(Fq) && sizeof(typename C::G2) == 8 * sizeof(Fq),
+                      "the ABI points are packed coordinates: 2, 4, 4 and 8 Fq");
+        s = {sizeof(typename C::Fr), sizeof(Fq), sizeof(typename C::G1Affine), sizeof(typename C::G2Affine), sizeof(typename C::G1),
+             sizeof(typename C::G2)};
+        return (int32_t)B2S_OK;
+    });
+    return s;
+}
+
 // ---- entry points implemented per translation unit (all take the ctx lock in api.cu) -----------
 int32_t ntt_run(Ctx* c, void* data_dev, uint32_t log_n, bool inverse, bool coset);
 void ntt_free_plans(Ctx* c);

@@ -41,10 +41,6 @@ static const char* reason_text(uint32_t st) {
     return "invalid";
 }
 
-static size_t fq_bytes(Ctx* c) { return c->curve == B2S_CURVE_BLS12_381 ? 48 : 32; }
-static size_t enc_bytes(Ctx* c, int group, bool compressed) { return fq_bytes(c) * group * (compressed ? 1 : 2); }
-static size_t aff_bytes(Ctx* c, int group) { return 2 * fq_bytes(c) * group; }
-
 // Two pinned host buffers and two device buffers, reused by every vector of one call.
 struct Stager {
     static constexpr uint64_t CH = 1u << 18;   // points per chunk
@@ -88,7 +84,7 @@ struct Stager {
     // `count` encodings from the HOST -> affine Montgomery points at out_dev; `name` labels the error message
     int32_t decode(int group, const uint8_t* in, uint64_t count, bool compressed, bool validate, void* out_dev, const char* name) {
         if (!count) return B2S_OK;
-        const size_t pb = enc_bytes(c, group, compressed), ab = aff_bytes(c, group);
+        const size_t pb = sizes(c).enc(group, compressed), ab = sizes(c).aff(group);
         B2S_TRY(reserve((size_t)std::min<uint64_t>(count, CH) * pb));
         B2S_CUDA(c, cudaMemsetAsync(err.p, 0xFF, sizeof(unsigned long long), c->stream));
         for (uint64_t base = 0, k = 0; base < count; base += CH, k++) {
@@ -130,9 +126,9 @@ struct Stager {
     int32_t decode_host(int group, const uint8_t* in, uint64_t count, bool compressed, bool validate, void* out_host, const char* name) {
         if (!count) return B2S_OK;
         DevBuf out;
-        B2S_TRY(out.alloc(c, count * aff_bytes(c, group)));
+        B2S_TRY(out.alloc(c, count * sizes(c).aff(group)));
         B2S_TRY(decode(group, in, count, compressed, validate, out.p, name));
-        B2S_CUDA(c, cudaMemcpyAsync(out_host, out.p, count * aff_bytes(c, group), cudaMemcpyDeviceToHost, c->stream));
+        B2S_CUDA(c, cudaMemcpyAsync(out_host, out.p, count * sizes(c).aff(group), cudaMemcpyDeviceToHost, c->stream));
         B2S_CUDA(c, cudaStreamSynchronize(c->stream));
         return B2S_OK;
     }
@@ -140,7 +136,7 @@ struct Stager {
 
 int32_t deserialize_points(Ctx* c, int group, const uint8_t* in, uint64_t len, uint64_t count, bool compressed, bool validate,
                            void* out_host) {
-    const size_t pb = enc_bytes(c, group, compressed);
+    const size_t pb = sizes(c).enc(group, compressed);
     if (count > len / pb || count * pb != len)
         return fail(c, B2S_ERR_INVALID_DATA, "deserialize: %llu bytes are not %llu points of %zu bytes", (unsigned long long)len,
                     (unsigned long long)count, pb);
@@ -149,7 +145,7 @@ int32_t deserialize_points(Ctx* c, int group, const uint8_t* in, uint64_t len, u
 }
 
 int32_t proof_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* a, void* b, void* cc) {
-    const size_t g1 = enc_bytes(c, 1, compressed), g2 = enc_bytes(c, 2, compressed);
+    const size_t g1 = sizes(c).enc(1, compressed), g2 = sizes(c).enc(2, compressed);
     if (len != 2 * g1 + g2) return fail(c, B2S_ERR_INVALID_DATA, "proof: %llu bytes, expected %zu", (unsigned long long)len, 2 * g1 + g2);
     Stager st(c);
     B2S_TRY(st.decode_host(1, in, 1, compressed, validate, a, "proof.a"));
@@ -165,7 +161,7 @@ struct Frame {
     uint64_t len, at = 0;
     bool compressed;
     int32_t point(int group, uint64_t* off) {
-        const size_t pb = enc_bytes(c, group, compressed);
+        const size_t pb = sizes(c).enc(group, compressed);
         if (len - at < pb) return fail(c, B2S_ERR_INVALID_DATA, "key: truncated at byte %llu", (unsigned long long)at);
         *off = at;
         at += pb;
@@ -176,7 +172,7 @@ struct Frame {
         uint64_t v = 0;
         for (int i = 0; i < 8; i++) v |= (uint64_t)in[at + i] << (8 * i);
         at += 8;
-        const size_t pb = enc_bytes(c, group, compressed);
+        const size_t pb = sizes(c).enc(group, compressed);
         if (v > (len - at) / pb)
             return fail(c, B2S_ERR_INVALID_DATA, "%s: length %llu exceeds the %llu bytes that remain", name, (unsigned long long)v,
                         (unsigned long long)(len - at));
@@ -216,24 +212,21 @@ int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed,
 int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, b2s_pk** out) {
     Frame f{c, in, len, 0, compressed};
     VkFrame v;
-    uint64_t beta1, delta1;
-    struct Q { int group; const char* name; uint64_t off, n; DevBuf b2s_pk::*buf; } qs[5] = {
-        {1, "a_query", 0, 0, &b2s_pk::a_query}, {1, "b_g1_query", 0, 0, &b2s_pk::b_g1_query}, {2, "b_g2_query", 0, 0, &b2s_pk::b_g2_query},
-        {1, "h_query", 0, 0, &b2s_pk::h_query}, {1, "l_query", 0, 0, &b2s_pk::l_query}};
+    uint64_t beta1, delta1, at[PK_QUERIES], n[PK_QUERIES];
     B2S_TRY(frame_vk(f, v));
     B2S_TRY(f.point(1, &beta1));
     B2S_TRY(f.point(1, &delta1));
-    for (Q& q : qs) B2S_TRY(f.vec(q.group, q.name, &q.off, &q.n));
+    for (int w = 0; w < PK_QUERIES; w++) B2S_TRY(f.vec(PK_QUERY[w].group, PK_QUERY[w].name, &at[w], &n[w]));
     if (f.at != len) return fail(c, B2S_ERR_INVALID_DATA, "pk: %llu trailing bytes", (unsigned long long)(len - f.at));
-    const uint64_t n_instance = v.n_abc, n_witness = qs[4].n, n_vars = n_instance + n_witness, domain = qs[3].n + 1;
-    if (qs[0].n != n_vars || qs[1].n != n_vars || qs[2].n != n_vars || (domain & (domain - 1)))
+    const uint64_t n_instance = v.n_abc, n_witness = n[Q_L], n_vars = n_instance + n_witness, domain = n[Q_H] + 1;
+    if (n[Q_A] != n_vars || n[Q_B_G1] != n_vars || n[Q_B_G2] != n_vars || (domain & (domain - 1)))
         return fail(c, B2S_ERR_MALFORMED_VK, "pk: inconsistent dimensions (instance %llu, witness %llu, a %llu, b_g1 %llu, b_g2 %llu, h %llu)",
-                    (unsigned long long)n_instance, (unsigned long long)n_witness, (unsigned long long)qs[0].n, (unsigned long long)qs[1].n,
-                    (unsigned long long)qs[2].n, (unsigned long long)qs[3].n);
-    const size_t g1 = aff_bytes(c, 1), g2 = aff_bytes(c, 2);
+                    (unsigned long long)n_instance, (unsigned long long)n_witness, (unsigned long long)n[Q_A], (unsigned long long)n[Q_B_G1],
+                    (unsigned long long)n[Q_B_G2], (unsigned long long)n[Q_H]);
+    const size_t g1 = sizes(c).g1, g2 = sizes(c).g2;
     b2s_pk* pk = new b2s_pk();
     pk->n_instance = n_instance; pk->n_witness = n_witness; pk->domain_size = domain;
-    pk->a_len = pk->b1_len = pk->b2_len = n_vars; pk->h_len = qs[3].n; pk->l_len = n_witness;
+    for (int w = 0; w < PK_QUERIES; w++) pk->q[w].len = n[w];   // a full key: every range starts at 0
     auto body = [&]() -> int32_t {
         Stager st(c);
         DevBuf scratch;   // gamma_g2 and gamma_abc_g1: validated, not kept by the prover
@@ -249,10 +242,11 @@ int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed,
         B2S_TRY(st.decode(1, in + v.abc, v.n_abc, compressed, validate, scratch.p, "gamma_abc_g1"));
         B2S_TRY(st.decode(1, in + beta1, 1, compressed, validate, k1 + g1, "beta_g1"));
         B2S_TRY(st.decode(1, in + delta1, 1, compressed, validate, k1 + 2 * g1, "delta_g1"));
-        for (Q& q : qs) {   // room for the two extra points pk_finish appends
-            DevBuf& b = pk->*(q.buf);
-            B2S_TRY(b.alloc(c, (q.n + 2) * (q.group == 1 ? g1 : g2)));
-            B2S_TRY(st.decode(q.group, in + q.off, q.n, compressed, validate, b.p, q.name));
+        for (int w = 0; w < PK_QUERIES; w++) {   // room for the two extra points pk_finish appends
+            const PkQueryInfo& info = PK_QUERY[w];
+            DevBuf& b = pk->q[w].pts;
+            B2S_TRY(b.alloc(c, (n[w] + 2) * sizes(c).aff(info.group)));
+            B2S_TRY(st.decode(info.group, in + at[w], n[w], compressed, validate, b.p, info.name));
         }
         return pk_finish(c, pk);
     };

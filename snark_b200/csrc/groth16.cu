@@ -89,38 +89,23 @@ __global__ void sum_shards_kernel(const XYZZ<F>* partials, uint32_t n_shards, ui
     sums[j] = acc;
 }
 
-// the query points of a key: `len` points from src, with room for the two extra points pk_finish appends
-static int32_t copy_query(Ctx* c, DevBuf& dst, const void* src, uint64_t len, size_t pt, cudaMemcpyKind kind) {
-    B2S_TRY(dst.alloc(c, (len + 2) * pt));
-    if (len) B2S_CUDA(c, cudaMemcpyAsync(dst.p, src, len * pt, kind, c->stream));
-    return B2S_OK;
-}
-
 // What a key handle holds beyond its points, shared by pk_upload and pk_deserialize.  The constants and the query points
 // are on the device, each query buffer with room for two more points; this appends the extra (base, scalar) pairs of the
 // shard that owns the end of a range and builds the h-query table when it fits.  Synchronises the ctx stream.
 int32_t pk_finish(Ctx* c, b2s_pk* pk) {
-    const size_t fq = c->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    const size_t g1 = 2 * fq, g2 = 4 * fq;
+    const Sizes z = sizes(c);
     const uint64_t n_vars = pk->n_instance + pk->n_witness;
-    pk->a_ext = (pk->a_off + pk->a_len == n_vars) ? 2 : 0;
-    pk->b1_ext = (pk->b1_off + pk->b1_len == n_vars) ? 2 : 0;
-    pk->b2_ext = (pk->b2_off + pk->b2_len == n_vars) ? 2 : 0;
-    const char* delta_g1 = pk->consts_g1.as<char>() + 2 * g1;
-    const char* delta_g2 = pk->consts_g2.as<char>() + g2;
-    // extras: a: [delta_1, O] (scalars r, s)   b1: [O, delta_1]   b2: [O, delta_2]   h, l: [O, O]
-    struct X { DevBuf* buf; uint64_t len; size_t pt; const char* e0; const char* e1; } xs[5] = {
-        {&pk->a_query, pk->a_len, g1, pk->a_ext ? delta_g1 : nullptr, nullptr},
-        {&pk->b_g1_query, pk->b1_len, g1, nullptr, pk->b1_ext ? delta_g1 : nullptr},
-        {&pk->b_g2_query, pk->b2_len, g2, nullptr, pk->b2_ext ? delta_g2 : nullptr},
-        {&pk->h_query, pk->h_len, g1, nullptr, nullptr},
-        {&pk->l_query, pk->l_len, g1, nullptr, nullptr}};
-    for (const X& x : xs) {
-        char* d = x.buf->as<char>() + x.len * x.pt;
-        B2S_CUDA(c, cudaMemsetAsync(d, 0, 2 * x.pt, c->stream));   // O = all-zero bytes
-        if (x.e0) B2S_CUDA(c, cudaMemcpyAsync(d, x.e0, x.pt, cudaMemcpyDeviceToDevice, c->stream));
-        if (x.e1) B2S_CUDA(c, cudaMemcpyAsync(d + x.pt, x.e1, x.pt, cudaMemcpyDeviceToDevice, c->stream));
+    const char* delta[3] = {nullptr, pk->consts_g1.as<char>() + 2 * z.g1, pk->consts_g2.as<char>() + z.g2};   // by group
+    for (int w = 0; w < PK_QUERIES; w++) {
+        PkQuery& q = pk->q[w];
+        const PkQueryInfo& info = PK_QUERY[w];
+        const size_t pt = z.aff(info.group);
+        q.ext = (info.delta_at >= 0 && q.off + q.len == n_vars) ? 2 : 0;
+        char* d = q.pts.as<char>() + q.len * pt;
+        B2S_CUDA(c, cudaMemsetAsync(d, 0, 2 * pt, c->stream));   // O = all-zero bytes
+        if (q.ext) B2S_CUDA(c, cudaMemcpyAsync(d + info.delta_at * pt, delta[info.group], pt, cudaMemcpyDeviceToDevice, c->stream));
     }
+    const PkQuery& h = pk->q[Q_H];
     // Fixed-base window table for the h query: its scalars (the quotient polynomial) are never repeated values, so this is
     // the MSM that always pays the full Pippenger price; the other queries run over the witness, where the multiplicity-aware
     // front end usually leaves little.  13 x the query (18 GiB at 2^24): only when it fits comfortably.
@@ -128,13 +113,13 @@ int32_t pk_finish(Ctx* c, b2s_pk* pk) {
         const char* env = getenv("B2S_PK_PRECOMP");
         const uint64_t min_n = getenv("B2S_PK_PRECOMP_MIN") ? strtoull(getenv("B2S_PK_PRECOMP_MIN"), nullptr, 10) : (1ull << 18);
         uint32_t cc = 0;
-        const uint32_t nw = msm_precompute_windows(c, pk->h_len, &cc);
+        const uint32_t nw = msm_precompute_windows(c, h.len, &cc);
         size_t free_b = 0, total_b = 0;
         cudaMemGetInfo(&free_b, &total_b);
-        const uint64_t need = (uint64_t)nw * pk->h_len * g1;
-        if (!(env && env[0] == '0') && pk->h_len >= min_n && (uint64_t)nw * pk->h_len < (1ull << 31) && need * 4 < (uint64_t)free_b) {
+        const uint64_t need = (uint64_t)nw * h.len * z.g1;
+        if (!(env && env[0] == '0') && h.len >= min_n && (uint64_t)nw * h.len < (1ull << 31) && need * 4 < (uint64_t)free_b) {
             B2S_TRY(pk->h_table.alloc(c, need));
-            B2S_TRY(msm_precompute(c, 1, pk->h_query.p, pk->h_len, pk->h_table.p, &pk->h_pre));
+            B2S_TRY(msm_precompute(c, 1, h.pts.p, h.len, pk->h_table.p, &pk->h_pre));
         }
     }
     B2S_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -142,21 +127,25 @@ int32_t pk_finish(Ctx* c, b2s_pk* pk) {
 }
 
 int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
-    const size_t fq = c->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    const size_t g1 = 2 * fq, g2 = 4 * fq;
+    const Sizes z = sizes(c);
     const uint64_t n_vars = d->n_instance + d->n_witness;
-    if (d->a_off + d->a_len > n_vars || d->b1_off + d->b1_len > n_vars || d->b2_off + d->b2_len > n_vars ||
-        d->l_off + d->l_len > d->n_witness || d->h_off + d->h_len > d->domain_size)
-        return fail(c, B2S_ERR_MALFORMED_VK, "pk: a query range exceeds the key dimensions");
+    // [off, off + len) must lie in [0, bound).  h is held to domain_size only, although a full key's h is domain_size - 1 long
+    struct { const void* pts; uint64_t off, len, bound; } src[PK_QUERIES] = {
+        {d->a_query, d->a_off, d->a_len, n_vars},
+        {d->b_g1_query, d->b1_off, d->b1_len, n_vars},
+        {d->b_g2_query, d->b2_off, d->b2_len, n_vars},
+        {d->h_query, d->h_off, d->h_len, d->domain_size},
+        {d->l_query, d->l_off, d->l_len, d->n_witness}};
+    for (const auto& s : src)
+        if (s.off + s.len > s.bound) return fail(c, B2S_ERR_MALFORMED_VK, "pk: a query range exceeds the key dimensions");
     if (!d->alpha_g1 || !d->beta_g1 || !d->delta_g1 || !d->beta_g2 || !d->delta_g2)
         return fail(c, B2S_ERR_MALFORMED_VK, "pk: missing group constants");
     b2s_pk* pk = new b2s_pk();
     pk->n_instance = d->n_instance; pk->n_witness = d->n_witness; pk->domain_size = d->domain_size;
-    pk->a_off = d->a_off; pk->a_len = d->a_len; pk->b1_off = d->b1_off; pk->b1_len = d->b1_len;
-    pk->b2_off = d->b2_off; pk->b2_len = d->b2_len; pk->h_off = d->h_off; pk->h_len = d->h_len;
-    pk->l_off = d->l_off; pk->l_len = d->l_len;
+    for (int w = 0; w < PK_QUERIES; w++) { pk->q[w].off = src[w].off; pk->q[w].len = src[w].len; }
     const cudaMemcpyKind kind = mem == B2S_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     auto body = [&]() -> int32_t {
+        const size_t g1 = z.g1, g2 = z.g2;
         B2S_TRY(pk->consts_g1.alloc(c, 3 * g1));
         B2S_TRY(pk->consts_g2.alloc(c, 2 * g2));
         char* p1 = pk->consts_g1.as<char>();
@@ -166,11 +155,11 @@ int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
         B2S_CUDA(c, cudaMemcpyAsync(p1 + 2 * g1, d->delta_g1, g1, kind, c->stream));
         B2S_CUDA(c, cudaMemcpyAsync(p2, d->beta_g2, g2, kind, c->stream));
         B2S_CUDA(c, cudaMemcpyAsync(p2 + g2, d->delta_g2, g2, kind, c->stream));
-        B2S_TRY(copy_query(c, pk->a_query, d->a_query, d->a_len, g1, kind));
-        B2S_TRY(copy_query(c, pk->b_g1_query, d->b_g1_query, d->b1_len, g1, kind));
-        B2S_TRY(copy_query(c, pk->b_g2_query, d->b_g2_query, d->b2_len, g2, kind));
-        B2S_TRY(copy_query(c, pk->h_query, d->h_query, d->h_len, g1, kind));
-        B2S_TRY(copy_query(c, pk->l_query, d->l_query, d->l_len, g1, kind));
+        for (int w = 0; w < PK_QUERIES; w++) {   // with room for the two extra points pk_finish appends
+            const size_t pt = z.aff(PK_QUERY[w].group);
+            B2S_TRY(pk->q[w].pts.alloc(c, (src[w].len + 2) * pt));
+            if (src[w].len) B2S_CUDA(c, cudaMemcpyAsync(pk->q[w].pts.p, src[w].pts, src[w].len * pt, kind, c->stream));
+        }
         return pk_finish(c, pk);
     };
     const int32_t st = body();
@@ -185,7 +174,7 @@ struct ReplicatedH : HSource {
     int32_t get(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void** h_for_shard) override {
         B2S_TRY(h.alloc(c, (size_t)32 << m->log_domain));
         B2S_TRY(witness_map_run(c, m, z_dev, h.p));
-        *h_for_shard = h.as<char>() + pk->h_off * 32;
+        *h_for_shard = h.as<char>() + pk->q[Q_H].off * 32;
         return B2S_OK;
     }
 };
@@ -262,18 +251,25 @@ static int32_t shard_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* 
         explicit DedupScope(Ctx* ctx) : c(ctx) { msm_dedup_scope_begin(c); }
         ~DedupScope() { msm_dedup_scope_end(c); }
     } dedup_scope(c);
-    B2S_TRY(msm_run(c, 2, pk->b_g2_query.p, zd + pk->b2_off, pk->b2_len + pk->b2_ext, true, g2_out, w2));
-    B2S_TRY(msm_run(c, 1, pk->a_query.p, zd + pk->a_off, pk->a_len + pk->a_ext, true, g1 + 2, w1 + 2 * 64));
-    B2S_TRY(msm_run(c, 1, pk->b_g1_query.p, zd + pk->b1_off, pk->b1_len + pk->b1_ext, true, g1 + 3, w1 + 3 * 64));
-    B2S_TRY(msm_run(c, 1, pk->l_query.p, zd + m->n_instance + pk->l_off, pk->l_len, true, g1 + 1, w1 + 1 * 64));
+    // the MSM of query w over its points (or `bases`, the h-query table) and the scalars PK_QUERY[w] names
+    auto msm = [&](int w, void* out, void* wins, const void* bases = nullptr, const MsmPre* pre = nullptr) {
+        const PkQuery& q = pk->q[w];
+        const PkScalars from = PK_QUERY[w].scalars;
+        const void* scalars = from == FROM_H ? h_shard : zd + (from == FROM_WITNESS ? m->n_instance : 0) + q.off;
+        return msm_run(c, PK_QUERY[w].group, bases ? bases : q.pts.p, scalars, q.len + q.ext, true, out, wins, pre);
+    };
+    B2S_TRY(msm(Q_B_G2, g2_out, w2));
+    B2S_TRY(msm(Q_A, g1 + 2, w1 + 2 * 64));
+    B2S_TRY(msm(Q_B_G1, g1 + 3, w1 + 3 * 64));
+    B2S_TRY(msm(Q_L, g1 + 1, w1 + 1 * 64));
     if (fork) {
         B2S_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_join, 0));
         side_guard.active = false;
     } else {
         B2S_TRY(hs->get(c, pk, m, zd, &h_shard));
     }
-    if (pk->h_table.p) B2S_TRY(msm_run(c, 1, pk->h_table.p, h_shard, pk->h_len, true, g1 + 0, w1 + 0 * 64, &pk->h_pre));
-    else B2S_TRY(msm_run(c, 1, pk->h_query.p, h_shard, pk->h_len, true, g1 + 0, w1 + 0 * 64));
+    if (pk->h_table.p) B2S_TRY(msm(Q_H, g1 + 0, w1 + 0 * 64, pk->h_table.p, &pk->h_pre));
+    else B2S_TRY(msm(Q_H, g1 + 0, w1 + 0 * 64));
     B2S_TRY(msm_join_tails(c));
     return B2S_OK;
 }

@@ -128,7 +128,7 @@ struct DistributedH : HSource {
 static bool slab_aligned(const b2s_pk* pk, const b2s_r1cs* m, int rank, int world) {
     const uint64_t N = 1ull << m->log_domain, per = N / (uint64_t)world, off = per * (uint64_t)rank;
     const uint64_t len = std::min<uint64_t>(per, N - 1 - off);
-    return pk->h_off == off && pk->h_len == len;
+    return pk->q[Q_H].off == off && pk->q[Q_H].len == len;
 }
 
 namespace b2s {
@@ -143,8 +143,8 @@ static int32_t prove_group(b2s_group* g, const b2s_pk* pk, const b2s_r1cs* m, co
     if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove_group: null key or matrices");
     if ((!z_dev && (!z_inst || (!z_wit && m->n_witness))) || !r || !s) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove_group: null assignment");
     if (g->rank == 0 && (!out_a || !out_b || !out_c)) return fail(ctx, B2S_ERR_INVALID_ARG, "prove_group: rank 0 needs the proof buffers");
-    const size_t fq = ctx->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    const size_t p1 = 4 * fq, p2 = 8 * fq, per = 4 * p1 + p2;   // XYZZ sizes; one rank's packet
+    const Sizes z = sizes(ctx);
+    const size_t p1 = z.g1x, p2 = z.g2x, per = 4 * p1 + p2;   // XYZZ sizes; one rank's packet
     DevBuf mine, all;
     B2S_TRY(mine.alloc(ctx, per));
     B2S_TRY(all.alloc(ctx, per * (size_t)g->world));

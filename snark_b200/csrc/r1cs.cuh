@@ -15,19 +15,51 @@ struct b2s_r1cs {
     uint32_t pool_size = 0;
 };
 
+namespace b2s {
+// The five query vectors of a proving key, in the order of b2s_pk_query's `which`.
+enum PkQueryId { Q_A, Q_B_G1, Q_B_G2, Q_H, Q_L, PK_QUERIES };
+// Where the scalars of a query's MSM start: z + off, z + n_instance + off (the witness), or the h shard (HSource).
+enum PkScalars { FROM_Z, FROM_WITNESS, FROM_H };
+// What is fixed per query.  The shard that owns the end of an a / b range also owns two extra (base, scalar) pairs with
+// scalars (r, s): a appends [delta, O], b_g1 and b_g2 append [O, delta] (delta of the query's group).  h and l append
+// [O, O] and never use them.
+struct PkQueryInfo {
+    const char* name;       // in error messages
+    int group;
+    int delta_at;           // which extra pair holds delta: 0, 1, or -1 for none (no extra pairs)
+    PkScalars scalars;
+};
+inline constexpr PkQueryInfo PK_QUERY[PK_QUERIES] = {{"a_query", 1, 0, FROM_Z},
+                                                     {"b_g1_query", 1, 1, FROM_Z},
+                                                     {"b_g2_query", 2, 1, FROM_Z},
+                                                     {"h_query", 1, -1, FROM_H},
+                                                     {"l_query", 1, -1, FROM_WITNESS}};
+struct PkQuery {
+    DevBuf pts;                       // affine points [len + 2]: the two extra points follow the range
+    uint64_t off = 0, len = 0;        // indices into the full vector held by this shard
+    uint32_t ext = 0;                 // 2 when the extra pairs belong to the MSM (this shard owns the end of the range)
+};
+}  // namespace b2s
+
 struct b2s_pk {
     uint64_t n_instance = 0, n_witness = 0, domain_size = 0;
     b2s::DevBuf consts_g1;            // alpha_g1, beta_g1, delta_g1 (affine)
     b2s::DevBuf consts_g2;            // beta_g2, delta_g2 (affine)
-    b2s::DevBuf a_query, b_g1_query, b_g2_query, h_query, l_query;
-    // fixed-base window table of h_query (msm_precompute): [h_pre.nwin][h_len] affine points; empty when switched off / too big
+    b2s::PkQuery q[b2s::PK_QUERIES];  // indexed by PkQueryId
+    // fixed-base window table of h_query (msm_precompute): [h_pre.nwin][q[Q_H].len] affine points; empty when switched off / too big
     b2s::DevBuf h_table;
     b2s::MsmPre h_pre{0, 0, 0};
-    uint32_t a_ext = 0, b1_ext = 0, b2_ext = 0;   // 2 when this shard owns the end of the range (extra delta pairs)
-    uint64_t a_off = 0, a_len = 0, b1_off = 0, b1_len = 0, b2_off = 0, b2_len = 0, h_off = 0, h_len = 0, l_off = 0, l_len = 0;
 };
 
 namespace b2s {
+// a full (unsharded) key: every query covers its whole vector, h being domain_size - 1 long
+inline bool pk_is_full(const b2s_pk* pk) {
+    const uint64_t n_vars = pk->n_instance + pk->n_witness;
+    const PkQuery* q = pk->q;
+    return q[Q_A].len == n_vars && q[Q_B_G1].len == n_vars && q[Q_B_G2].len == n_vars && q[Q_L].len == pk->n_witness &&
+           q[Q_H].len + 1 == pk->domain_size;
+}
+
 int32_t r1cs_upload(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness, const uint64_t* const row_ptr[3],
                     const uint32_t* const col[3], const void* const coeff[3], b2s_r1cs** out);
 // lcmap.cu: the same handle from the constraint system's LcMap, CSR built by kernels
@@ -45,8 +77,8 @@ int32_t pk_query_download(Ctx* c, const b2s_pk* pk, int which, void* out_host, u
 // Where the h-query MSM of a shard takes its scalars from: the default computes the whole h on this GPU (replicated
 // witness_map); the multi-GPU group computes it distributed and hands back this rank's coefficient slab (group.cu).
 struct HSource {
-    // z_dev: the full assignment on the device.  On return *h_for_shard points at the scalars matching pk->h_query
-    // (pk->h_len elements starting at coefficient pk->h_off); the memory stays valid until the HSource is destroyed.
+    // z_dev: the full assignment on the device.  On return *h_for_shard points at the scalars matching pk->q[Q_H]
+    // (its len elements starting at coefficient off); the memory stays valid until the HSource is destroyed.
     virtual int32_t get(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void** h_for_shard) = 0;
     virtual ~HSource() = default;
 };

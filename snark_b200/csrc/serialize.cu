@@ -80,16 +80,11 @@ static void encode_point(bool bls, int group, bool compressed, size_t fq, const 
     }
 }
 
-static size_t point_bytes(Ctx* c, int group, bool compressed) {
-    const size_t fq = c->curve == B2S_CURVE_BLS12_381 ? 48 : 32;
-    return (group == 1 ? 1 : 2) * fq * (compressed ? 1 : 2);
-}
-
 // `count` affine Montgomery points (HOST or DEVICE) -> encoded bytes on the host; chunked so that keys of any size stream through
 int32_t serialize_points_ex(Ctx* c, int group, const void* affine, int32_t mem, uint64_t count, bool compressed, uint8_t* out, uint64_t cap) {
     const bool bls = c->curve == B2S_CURVE_BLS12_381;
-    const size_t fq = bls ? 48 : 32;
-    const size_t in_bytes = (group == 1 ? 2 : 4) * fq, out_bytes = point_bytes(c, group, compressed);
+    const Sizes z = sizes(c);
+    const size_t in_bytes = z.aff(group), out_bytes = z.enc(group, compressed);
     if (count * out_bytes > cap) return fail(c, B2S_ERR_INVALID_ARG, "serialize: output buffer too small");
     const uint64_t CH = 1u << 18;
     DevBuf d, stage;
@@ -112,26 +107,31 @@ int32_t serialize_points_ex(Ctx* c, int group, const void* affine, int32_t mem, 
         B2S_TRY(st);
         B2S_CUDA(c, cudaMemcpyAsync(h.data(), d.p, (size_t)n * sizeof(CanonPoint), cudaMemcpyDeviceToHost, c->stream));
         B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        for (uint32_t i = 0; i < n; i++) encode_point(bls, group, compressed, fq, h[i], out + (base + i) * out_bytes);
+        for (uint32_t i = 0; i < n; i++) encode_point(bls, group, compressed, z.fq, h[i], out + (base + i) * out_bytes);
     }
     return B2S_OK;
 }
 
-// host: bytes of `count` points of `group` (HOST affine Montgomery in) -> compressed bytes
-int32_t serialize_points(Ctx* c, int group, const void* affine_host, uint32_t count, uint8_t* out, uint64_t cap) {
-    return serialize_points_ex(c, group, affine_host, B2S_MEM_HOST, count, true, out, cap);
-}
-
 static void put_u64(uint8_t* o, uint64_t v) { for (int i = 0; i < 8; i++) o[i] = (uint8_t)(v >> (8 * i)); }
 
+// A || B || C; HOST affine Montgomery
+int32_t proof_serialize(Ctx* c, const void* a_g1, const void* b_g2, const void* c_g1, bool compressed, uint8_t* out, uint64_t cap) {
+    const Sizes z = sizes(c);
+    const size_t g1 = z.enc(1, compressed), g2 = z.enc(2, compressed);
+    if (cap < 2 * g1 + g2) return fail(c, B2S_ERR_INVALID_ARG, "proof_serialize: output buffer too small");
+    B2S_TRY(serialize_points_ex(c, 1, a_g1, B2S_MEM_HOST, 1, compressed, out, g1));
+    B2S_TRY(serialize_points_ex(c, 2, b_g2, B2S_MEM_HOST, 1, compressed, out + g1, g2));
+    return serialize_points_ex(c, 1, c_g1, B2S_MEM_HOST, 1, compressed, out + g1 + g2, g1);
+}
+
 uint64_t vk_serialized_size(Ctx* c, uint64_t n_gamma_abc, bool compressed) {
-    return point_bytes(c, 1, compressed) * (1 + n_gamma_abc) + 3 * point_bytes(c, 2, compressed) + 8;
+    return sizes(c).enc(1, compressed) * (1 + n_gamma_abc) + 3 * sizes(c).enc(2, compressed) + 8;
 }
 // alpha_g1, beta_g2, gamma_g2, delta_g2, Vec(gamma_abc_g1); all HOST affine Montgomery
 int32_t vk_serialize(Ctx* c, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2, const void* gamma_abc,
                      uint64_t n_gamma_abc, bool compressed, uint8_t* out, uint64_t cap) {
     if (vk_serialized_size(c, n_gamma_abc, compressed) > cap) return fail(c, B2S_ERR_INVALID_ARG, "vk_serialize: output buffer too small");
-    const size_t g1 = point_bytes(c, 1, compressed), g2 = point_bytes(c, 2, compressed);
+    const size_t g1 = sizes(c).enc(1, compressed), g2 = sizes(c).enc(2, compressed);
     uint8_t* o = out;
     B2S_TRY(serialize_points_ex(c, 1, alpha_g1, B2S_MEM_HOST, 1, compressed, o, g1)); o += g1;
     B2S_TRY(serialize_points_ex(c, 2, beta_g2, B2S_MEM_HOST, 1, compressed, o, g2)); o += g2;
@@ -147,28 +147,28 @@ int32_t vk_serialize(Ctx* c, const void* alpha_g1, const void* beta_g2, const vo
 namespace b2s {
 
 uint64_t pk_serialized_size(Ctx* c, const b2s_pk* pk, uint64_t vk_len, bool compressed) {
-    const uint64_t g1 = point_bytes(c, 1, compressed), g2 = point_bytes(c, 2, compressed);
-    return vk_len + 2 * g1 + 5 * 8 + g1 * (pk->a_len + pk->b1_len + pk->h_len + pk->l_len) + g2 * pk->b2_len;
+    const Sizes z = sizes(c);
+    uint64_t n = vk_len + 2 * z.enc(1, compressed) + PK_QUERIES * 8;
+    for (int w = 0; w < PK_QUERIES; w++) n += z.enc(PK_QUERY[w].group, compressed) * pk->q[w].len;
+    return n;
 }
 // vk bytes (from vk_serialize) || beta_g1 || delta_g1 || the five query vectors of the device-resident FULL key
 int32_t pk_serialize(Ctx* c, const b2s_pk* pk, const uint8_t* vk_bytes, uint64_t vk_len, bool compressed, uint8_t* out, uint64_t cap) {
     if (pk_serialized_size(c, pk, vk_len, compressed) > cap) return fail(c, B2S_ERR_INVALID_ARG, "pk_serialize: output buffer too small");
-    const uint64_t n_vars = pk->n_instance + pk->n_witness;
-    if (pk->a_len != n_vars || pk->b1_len != n_vars || pk->b2_len != n_vars || pk->l_len != pk->n_witness || pk->h_len + 1 != pk->domain_size)
-        return fail(c, B2S_ERR_MALFORMED_VK, "pk_serialize: needs a full (unsharded) proving key");
-    const size_t g1 = point_bytes(c, 1, compressed), g2 = point_bytes(c, 2, compressed);
-    const size_t a1 = c->curve == B2S_CURVE_BLS12_381 ? 96 : 64;
+    if (!pk_is_full(pk)) return fail(c, B2S_ERR_MALFORMED_VK, "pk_serialize: needs a full (unsharded) proving key");
+    const Sizes z = sizes(c);
+    const size_t g1 = z.enc(1, compressed);
     uint8_t* o = out;
     memcpy(o, vk_bytes, vk_len); o += vk_len;
     const char* k1 = pk->consts_g1.as<char>();   // alpha, beta, delta
-    B2S_TRY(serialize_points_ex(c, 1, k1 + a1, B2S_MEM_DEVICE, 1, compressed, o, g1)); o += g1;
-    B2S_TRY(serialize_points_ex(c, 1, k1 + 2 * a1, B2S_MEM_DEVICE, 1, compressed, o, g1)); o += g1;
-    struct Q { int group; const DevBuf* buf; uint64_t len; } qs[5] = {{1, &pk->a_query, pk->a_len}, {1, &pk->b_g1_query, pk->b1_len},
-                                                                    {2, &pk->b_g2_query, pk->b2_len}, {1, &pk->h_query, pk->h_len}, {1, &pk->l_query, pk->l_len}};
-    for (const Q& q : qs) {
-        const size_t pb = q.group == 1 ? g1 : g2;
+    B2S_TRY(serialize_points_ex(c, 1, k1 + z.g1, B2S_MEM_DEVICE, 1, compressed, o, g1)); o += g1;
+    B2S_TRY(serialize_points_ex(c, 1, k1 + 2 * z.g1, B2S_MEM_DEVICE, 1, compressed, o, g1)); o += g1;
+    for (int w = 0; w < PK_QUERIES; w++) {
+        const PkQuery& q = pk->q[w];
+        const int group = PK_QUERY[w].group;
+        const size_t pb = z.enc(group, compressed);
         put_u64(o, q.len); o += 8;
-        B2S_TRY(serialize_points_ex(c, q.group, q.buf->p, B2S_MEM_DEVICE, q.len, compressed, o, pb * q.len));
+        B2S_TRY(serialize_points_ex(c, group, q.pts.p, B2S_MEM_DEVICE, q.len, compressed, o, pb * q.len));
         o += pb * q.len;
     }
     return B2S_OK;

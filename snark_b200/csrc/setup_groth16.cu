@@ -214,19 +214,13 @@ int32_t groth16_setup(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s_
 
 // copy one query vector of a device-resident key to the host (which: 0 a, 1 b_g1, 2 b_g2, 3 h, 4 l, 5 [alpha,beta,delta]_g1, 6 [beta,delta]_g2)
 int32_t pk_query_download(Ctx* c, const b2s_pk* pk, int which, void* out_host, uint64_t cap_bytes) {
-    const size_t fq = c->curve == B2S_CURVE_BLS12_381 ? 48 : 32, g1 = 2 * fq, g2 = 4 * fq;
+    const Sizes z = sizes(c);
     const DevBuf* src = nullptr;
     size_t bytes = 0;
-    switch (which) {
-        case 0: src = &pk->a_query; bytes = pk->a_len * g1; break;
-        case 1: src = &pk->b_g1_query; bytes = pk->b1_len * g1; break;
-        case 2: src = &pk->b_g2_query; bytes = pk->b2_len * g2; break;
-        case 3: src = &pk->h_query; bytes = pk->h_len * g1; break;
-        case 4: src = &pk->l_query; bytes = pk->l_len * g1; break;
-        case 5: src = &pk->consts_g1; bytes = 3 * g1; break;
-        case 6: src = &pk->consts_g2; bytes = 2 * g2; break;
-        default: return fail(c, B2S_ERR_INVALID_ARG, "pk_query: unknown vector %d", which);
-    }
+    if (which >= 0 && which < PK_QUERIES) { src = &pk->q[which].pts; bytes = pk->q[which].len * z.aff(PK_QUERY[which].group); }
+    else if (which == 5) { src = &pk->consts_g1; bytes = 3 * z.g1; }
+    else if (which == 6) { src = &pk->consts_g2; bytes = 2 * z.g2; }
+    else return fail(c, B2S_ERR_INVALID_ARG, "pk_query: unknown vector %d", which);
     if (bytes > cap_bytes) return fail(c, B2S_ERR_INVALID_ARG, "pk_query: buffer too small (%zu > %llu)", bytes, (unsigned long long)cap_bytes);
     if (bytes) B2S_CUDA(c, cudaMemcpyAsync(out_host, src->p, bytes, cudaMemcpyDeviceToHost, c->stream));
     B2S_CUDA(c, cudaStreamSynchronize(c->stream));
