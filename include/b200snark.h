@@ -71,6 +71,7 @@ extern "C" {
 typedef struct b2s_ctx b2s_ctx;
 typedef struct b2s_r1cs b2s_r1cs;   /* device-resident A/B/C in CSR (witness independent; upload once per circuit) */
 typedef struct b2s_pk b2s_pk;       /* device-resident Groth16 proving key (or one base-range shard of it) */
+typedef struct b2s_pvk b2s_pvk;     /* device-resident PreparedVerifyingKey (b2s_vk_prepare) */
 
 /* ---- context ------------------------------------------------------------------------------ */
 int32_t b2s_ctx_create(int32_t curve_id, int32_t device_ordinal, b2s_ctx** out);
@@ -279,6 +280,33 @@ int32_t b2s_vk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
                            void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1, uint64_t cap_gamma_abc,
                            uint64_t* n_gamma_abc, uint64_t* consumed);
 int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, b2s_pk** out);
+
+/* ---- verification: pairings and batched Groth16 verify ----------------------------------------------------------------
+ * The optimal ate pairing in CUDA (snark_b200/csrc/pairing.cuh): BLS12-381 loops over |x| and conjugates, BN254 over the
+ * signed digits of 6x + 2 with the two Frobenius lines.  GT is ark's Fp12 in memory (c0 = Fp6 {c0, c1, c2 : Fp2}, c1),
+ * Montgomery limbs, fully reduced.  The value is a fixed power of the textbook reduced ate pairing
+ * o(P, Q) = f_{|t-1|,Q}(P)^((p^12 - 1) / r):  e = o^k with k = -3 mod r (BLS12-381) and
+ * k = 147946756881789319005730692170996259610 (BN254), both coprime to r (pairing.cuh derives them).
+ *   b2s_vk_prepare   SNARK::process_vk (snark/src/lib.rs:68-71): HOST affine points, as returned by b2s_groth16_setup /
+ *                    b2s_vk_deserialize.  Computes e(alpha_g1, beta_g2) in GT, the line coefficients of -gamma_g2 and
+ *                    -delta_g2 (ark's G2Prepared), and per gamma_abc base j >= 1 a fixed-base table of 32 x 255 affine
+ *                    points for the public-input sum: 765 KiB (BLS12-381) / 510 KiB (BN254) of device memory per public
+ *                    input.  B2S_ERR_MALFORMED_VK if n_gamma_abc == 0.
+ *   b2s_groth16_verify_batch  SNARK::verify_with_processed_vk (lib.rs:76-80) for n_proofs proofs at once, one verdict each:
+ *                    ok[i] = [ e(A_i, B_i) * e(IC_i, -gamma) * e(C_i, -delta) == e(alpha, beta) ],
+ *                    IC_i = gamma_abc[0] + sum_j x_ij gamma_abc[j+1].  inputs: n_proofs x n_inputs Montgomery Fr, row-major
+ *                    (NULL when n_inputs == 0); a, b, c: affine arrays; ok: n_proofs bytes (1 = accepted).  All buffers
+ *                    share `mem`; host batches go through bounded device scratch in chunks, so n_proofs is not limited by
+ *                    device memory.  n_inputs + 1 != n_gamma_abc -> B2S_ERR_MALFORMED_VK (ark's prepare_inputs error);
+ *                    n_proofs == 0 -> B2S_OK.  Points are assumed valid, as in ark: decode untrusted bytes with validate = 1.
+ *   b2s_pairing      Pairing::pairing, element-wise: out[i] = e(P_i, Q_i), i < n; a pair with P or Q at infinity (all-zero)
+ *                    gives 1.  All buffers share `mem`. */
+int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,
+                       const void* gamma_abc_g1, uint64_t n_gamma_abc, b2s_pvk** out);
+void b2s_pvk_free(b2s_ctx* ctx, b2s_pvk* pvk);
+int32_t b2s_groth16_verify_batch(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                 const void* a_g1, const void* b_g2, const void* c_g1, int32_t mem, uint8_t* ok);
+int32_t b2s_pairing(b2s_ctx* ctx, const void* p_g1, const void* q_g2, uint64_t n, int32_t mem, void* out_gt);
 
 /* ---- setup helper (SURVEY 8(f) row 2): fixed-base batch multiplication -------------------------
  * out[i] = scalars[i] * G (the curve's standard generator), affine, i < n.  Used to build proving keys

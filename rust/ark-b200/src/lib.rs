@@ -13,6 +13,7 @@ use ark_std::{rand::{CryptoRng, RngCore}, UniformRand};
 #[repr(C)] pub struct B2sCtx { _p: [u8; 0] }
 #[repr(C)] pub struct B2sR1cs { _p: [u8; 0] }
 #[repr(C)] pub struct B2sPk { _p: [u8; 0] }
+#[repr(C)] pub struct B2sPvk { _p: [u8; 0] }
 
 #[repr(C)]
 pub struct B2sPkDesc {
@@ -64,6 +65,13 @@ extern "C" {
                               out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void, out_delta_g2: *mut c_void,
                               out_gamma_abc_g1: *mut c_void, cap_gamma_abc: u64, n_gamma_abc: *mut u64, consumed: *mut u64) -> i32;
     pub fn b2s_pk_deserialize(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, out: *mut *mut B2sPk) -> i32;
+    // verification (SNARK::process_vk / verify_with_processed_vk for many proofs; pairings in CUDA)
+    pub fn b2s_vk_prepare(ctx: *mut B2sCtx, alpha_g1: *const c_void, beta_g2: *const c_void, gamma_g2: *const c_void,
+                          delta_g2: *const c_void, gamma_abc_g1: *const c_void, n_gamma_abc: u64, out: *mut *mut B2sPvk) -> i32;
+    pub fn b2s_pvk_free(ctx: *mut B2sCtx, pvk: *mut B2sPvk);
+    pub fn b2s_groth16_verify_batch(ctx: *mut B2sCtx, pvk: *const B2sPvk, n_proofs: u64, inputs: *const c_void, n_inputs: u64,
+                                    a_g1: *const c_void, b_g2: *const c_void, c_g1: *const c_void, mem: i32, ok: *mut u8) -> i32;
+    pub fn b2s_pairing(ctx: *mut B2sCtx, p_g1: *const c_void, q_g2: *const c_void, n: u64, mem: i32, out_gt: *mut c_void) -> i32;
     // universal-setup schemes (UniversalSetupSNARK, snark/src/lib.rs:107-133): the seams a polynomial-commitment /
     // evaluation-domain backend binds (INTEGRATION.md section 8).  mem: 0 host, 1 device; s, c, z: one Montgomery Fr on the host
     pub fn b2s_ntt(ctx: *mut B2sCtx, data: *mut c_void, log_n: u32, inverse: i32, coset: i32, mem: i32) -> i32;
@@ -199,6 +207,44 @@ impl<E: Pairing> Groth16B200<E> {
         check(ctx, unsafe { b2s_pk_deserialize(ctx, pk_bytes.as_ptr(), pk_bytes.len() as u64, compressed as i32, validate as i32, &mut pkh) })?;
         Ok(Resident { ctx, pk: pkh, mat })
     }
+
+    /// `verify_with_processed_vk` for many proofs under one key, one verdict per proof (`inputs[i]` belongs to
+    /// `proofs[i]`).  The key is prepared on the GPU (e(alpha, beta), the lines of -gamma and -delta, window tables for the
+    /// public-input sum) and every proof runs its Miller loop and final exponentiation in CUDA; host memory streams through
+    /// bounded device scratch.  A wrong input count is `MalformedVerifyingKey`, as in ark.  The points are used as given,
+    /// as in ark: proofs from untrusted bytes are decoded with validation first.
+    pub fn verify_batch(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>], proofs: &[Proof<E>]) -> Result<Vec<bool>, B200Error> {
+        if inputs.len() != proofs.len() { return Err(SynthesisError::AssignmentMissing.into()); }
+        let ni = vk.gamma_abc_g1.len().saturating_sub(1);
+        if inputs.iter().any(|x| x.len() != ni) { return Err(SynthesisError::MalformedVerifyingKey.into()); }
+        // the curve from the base field width: 48-byte Fq is BLS12-381, 32-byte Fq BN254
+        let curve_id = if core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>() == 48 { 0 } else { 1 };
+        let mut ctx: *mut B2sCtx = core::ptr::null_mut();
+        check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
+        let run = || -> Result<Vec<bool>, B200Error> {
+            let (alpha, beta, gamma, delta) = (pack_points(&[vk.alpha_g1]), pack_points(&[vk.beta_g2]), pack_points(&[vk.gamma_g2]),
+                                               pack_points(&[vk.delta_g2]));
+            let abc = pack_points(&vk.gamma_abc_g1);
+            let mut pvk: *mut B2sPvk = core::ptr::null_mut();
+            check(ctx, unsafe { b2s_vk_prepare(ctx, alpha.as_ptr().cast(), beta.as_ptr().cast(), gamma.as_ptr().cast(),
+                                               delta.as_ptr().cast(), abc.as_ptr().cast(), vk.gamma_abc_g1.len() as u64, &mut pvk) })?;
+            let x: Vec<E::ScalarField> = inputs.iter().flat_map(|v| v.iter().copied()).collect();
+            let a = pack_points(&proofs.iter().map(|p| p.a).collect::<Vec<_>>());
+            let b = pack_points(&proofs.iter().map(|p| p.b).collect::<Vec<_>>());
+            let c = pack_points(&proofs.iter().map(|p| p.c).collect::<Vec<_>>());
+            let mut ok = vec![0u8; proofs.len()];
+            let st = unsafe { b2s_groth16_verify_batch(ctx, pvk, proofs.len() as u64,
+                                                       if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
+                                                       a.as_ptr().cast(), b.as_ptr().cast(), c.as_ptr().cast(), 0 /* B2S_MEM_HOST */,
+                                                       ok.as_mut_ptr()) };
+            unsafe { b2s_pvk_free(ctx, pvk) };
+            check(ctx, st)?;
+            Ok(ok.into_iter().map(|v| v != 0).collect())
+        };
+        let out = run();
+        unsafe { b2s_ctx_destroy(ctx) };
+        out
+    }
 }
 
 impl Drop for Resident {
@@ -247,6 +293,8 @@ impl<E: Pairing + B200Curve> SNARK<E::ScalarField> for Groth16B200<E> {
         Ok(ark_groth16::prepare_verifying_key(vk))
     }
 
+    // One proof stays on ark: its verification is a short, latency-bound chain (three Miller loops and one final
+    // exponentiation) that a GPU launch would only slow down.  Many proofs under one key: Groth16B200::verify_batch.
     fn verify_with_processed_vk(
         pvk: &Self::ProcessedVerifyingKey, x: &[E::ScalarField], proof: &Self::Proof,
     ) -> Result<bool, Self::Error> {

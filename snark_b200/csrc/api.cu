@@ -34,6 +34,13 @@ int32_t proof_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compress
 int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* alpha, void* beta, void* gamma,
                        void* delta, void* abc, uint64_t cap_abc, uint64_t* n_abc, uint64_t* consumed);
 int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, b2s_pk** out);
+// verify.cu
+int32_t vk_prepare(Ctx* c, const void* alpha, const void* beta, const void* gamma, const void* delta, const void* abc, uint64_t n_abc,
+                   b2s_pvk** out);
+void pvk_free(b2s_pvk* pvk);
+int32_t groth16_verify_batch(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const void* a, const void* b,
+                             const void* cc, int32_t mem, uint8_t* ok);
+int32_t pairing_batch(Ctx* c, const void* p, const void* q, uint64_t n, int32_t mem, void* out);
 }  // namespace b2s
 
 #define LOCK(ctx)                                      \
@@ -593,6 +600,32 @@ int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
     if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_deserialize: null argument");
     *out = nullptr;
     return pk_deserialize(ctx, in, len, compressed != 0, validate != 0, out);
+}
+
+int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,
+                       const void* gamma_abc_g1, uint64_t n_gamma_abc, b2s_pvk** out) {
+    LOCK(ctx);
+    if (!out || !alpha_g1 || !beta_g2 || !gamma_g2 || !delta_g2 || (!gamma_abc_g1 && n_gamma_abc))
+        return fail(ctx, B2S_ERR_INVALID_ARG, "vk_prepare: null argument");
+    *out = nullptr;
+    return vk_prepare(ctx, alpha_g1, beta_g2, gamma_g2, delta_g2, gamma_abc_g1, n_gamma_abc, out);
+}
+void b2s_pvk_free(b2s_ctx* ctx, b2s_pvk* pvk) {
+    if (!ctx || !pvk) return;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    cudaSetDevice(ctx->device);
+    pvk_free(pvk);
+}
+int32_t b2s_groth16_verify_batch(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                 const void* a_g1, const void* b_g2, const void* c_g1, int32_t mem, uint8_t* ok) {
+    LOCK(ctx);
+    if (!pvk) return fail(ctx, B2S_ERR_INVALID_ARG, "verify_batch: null prepared key");
+    return groth16_verify_batch(ctx, pvk, n_proofs, inputs, n_inputs, a_g1, b_g2, c_g1, mem, ok);
+}
+int32_t b2s_pairing(b2s_ctx* ctx, const void* p_g1, const void* q_g2, uint64_t n, int32_t mem, void* out_gt) {
+    LOCK(ctx);
+    if (n && (!p_g1 || !q_g2 || !out_gt)) return fail(ctx, B2S_ERR_INVALID_ARG, "pairing: null buffer");
+    return pairing_batch(ctx, p_g1, q_g2, n, mem, out_gt);
 }
 
 }  // extern "C"

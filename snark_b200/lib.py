@@ -89,6 +89,11 @@ SIGNATURES = {
     "b2s_vk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32] + [c_void_p] * 5
                            + [c_uint64, POINTER(c_uint64), POINTER(c_uint64)]),
     "b2s_pk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, POINTER(c_void_p)]),
+    "b2s_vk_prepare": (c_int32, [c_void_p] * 6 + [c_uint64, POINTER(c_void_p)]),
+    "b2s_pvk_free": (None, [c_void_p, c_void_p]),
+    "b2s_groth16_verify_batch": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_int32,
+                                           c_void_p]),
+    "b2s_pairing": (c_int32, [c_void_p, c_void_p, c_void_p, c_uint64, c_int32, c_void_p]),
     "b2s_fixed_base_g1": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
     "b2s_fixed_base_g2": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
     "b2s_group_unique_id": (c_int32, [c_void_p]),
@@ -388,6 +393,54 @@ class Backend:
 
     def pk_free(self, pk):
         self.lib.b2s_pk_free(self.h, pk)
+
+    # ---- verification (pairings in CUDA) ----------------------------------------------------------------------------
+    def vk_prepare(self, vk):
+        """vk dict in the layout groth16_setup / vk_from_bytes return (HOST arrays) -> device-resident prepared key handle."""
+        n_abc = len(vk["gamma_abc_g1"]) * 4 // self.g1_bytes
+        h = c_void_p()
+        self._ck(self.lib.b2s_vk_prepare(self.h, vk["alpha_g1"].ctypes.data, vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data,
+                                         vk["delta_g2"].ctypes.data, vk["gamma_abc_g1"].ctypes.data if n_abc else None, n_abc,
+                                         ctypes.byref(h)))
+        return h
+
+    def pvk_free(self, pvk):
+        self.lib.b2s_pvk_free(self.h, pvk)
+
+    def groth16_verify_batch(self, pvk, inputs, n_inputs, a, b, c, n_proofs=None, ok=None):
+        """One verdict per proof.  inputs: n_proofs x n_inputs Montgomery Fr (None when n_inputs == 0); a, b, c: affine
+        arrays; all HOST numpy or all CUDA torch tensors.  Returns a bool numpy array (host), or fills the uint8 tensor
+        `ok` (device) and returns it."""
+        pa, mem = _ptr(a)
+        pb, mem_b = _ptr(b)
+        pc, mem_c = _ptr(c)
+        px, mem_x = _ptr(inputs)
+        assert mem == mem_b == mem_c and (inputs is None or mem_x == mem)
+        if n_proofs is None:
+            n_proofs = (a.nbytes if isinstance(a, np.ndarray) else a.numel() * a.element_size()) // self.g1_bytes
+        if mem == MEM_HOST:
+            out = np.zeros(max(n_proofs, 1), dtype=np.uint8)
+            self._ck(self.lib.b2s_groth16_verify_batch(self.h, pvk, n_proofs, px, n_inputs, pa, pb, pc, mem, out.ctypes.data))
+            return out[:n_proofs].astype(bool)
+        po, _ = _ptr(ok)
+        self._ck(self.lib.b2s_groth16_verify_batch(self.h, pvk, n_proofs, px, n_inputs, pa, pb, pc, mem, po))
+        return ok
+
+    def pairing(self, p, q, n=None, out=None):
+        """e(P_i, Q_i) element-wise.  p, q: affine G1 / G2 arrays (HOST numpy, or CUDA torch tensors with `out` a device
+        tensor of n * 12 Fq).  Returns GT elements as uint32 limbs (ark's Fp12 layout, Montgomery)."""
+        pp, mem = _ptr(p)
+        pq, mem_q = _ptr(q)
+        assert mem == mem_q
+        if n is None:
+            n = (p.nbytes if isinstance(p, np.ndarray) else p.numel() * p.element_size()) // self.g1_bytes
+        if out is None:
+            assert mem == MEM_HOST
+            out = np.zeros(n * 12 * self.fq_bytes // 4, dtype=np.uint32)
+        po, mem_o = _ptr(out)
+        assert mem_o == mem
+        self._ck(self.lib.b2s_pairing(self.h, pp, pq, n, mem, po))
+        return out
 
     def _proof_bufs(self):
         return (np.zeros(self.g1_bytes // 4, dtype=np.uint32), np.zeros(self.g2_bytes // 4, dtype=np.uint32),

@@ -198,6 +198,98 @@ def decode_extra(p, n, beta, psi, endo_scalar, endo_words):
     return s
 
 
+# ---- pairing constants (snark_b200/csrc/pairing.cuh) ---------------------------------------------------------------
+# Fq12 = Fq2[w] / (w^6 - xi) as Fq6 = Fq2[v] / (v^3 - xi), Fq12 = Fq6[w] / (w^2 - v).  The p^j-power Frobenius sends the
+# coefficient a_k of w^k to conj^j(a_k) * xi^(k (p^j - 1) / 6).  Each table is checked against a plain polynomial Fq12
+# raised to p^j, and the p^1 coefficients of w^2 and w^3 against the psi coefficients (psi is the Frobenius read through
+# the twist, so the p^1 coefficients equal them for BN254's D-type twist and are their inverses for BLS12-381's M-type).
+def f12_mul(p, xi, a, b):
+    """a * b for a, b lists of six Fq2 coefficients of w^0..w^5, w^6 = xi"""
+    t = [(0, 0)] * 11
+    for i in range(6):
+        for j in range(6):
+            m = f2_mul(p, a[i], b[j])
+            t[i + j] = ((t[i + j][0] + m[0]) % p, (t[i + j][1] + m[1]) % p)
+    for k in range(10, 5, -1):
+        m = f2_mul(p, t[k], xi)
+        t[k - 6] = ((t[k - 6][0] + m[0]) % p, (t[k - 6][1] + m[1]) % p)
+    return t[:6]
+
+
+def f12_pow(p, xi, a, e):
+    r = [(1, 0)] + [(0, 0)] * 5
+    for bit in bin(e)[2:]:
+        r = f12_mul(p, xi, r, r)
+        if bit == "1":
+            r = f12_mul(p, xi, r, a)
+    return r
+
+
+def frobenius_coeffs(p, xi, psi, m_type):
+    """{j: [xi^(k (p^j - 1) / 6) for k = 0..5]} for j = 1, 2, 3, checked as described above"""
+    import random
+    rng = random.Random(12)
+    g = {j: [f2_pow(p, xi, k * (p ** j - 1) // 6) for k in range(6)] for j in (1, 2, 3)}
+    a = [(rng.randrange(p), rng.randrange(p)) for _ in range(6)]
+    ap = a
+    for j in (1, 2, 3):
+        ap = f12_pow(p, xi, ap, p)
+        conj = [(c[0], (-c[1]) % p) if j % 2 else c for c in a]
+        assert [f2_mul(p, conj[k], g[j][k]) for k in range(6)] == ap, j
+        assert all(c[1] == 0 for c in g[2])                   # p^2 coefficients lie in Fq
+    cx, cy = (f2_inv(p, g[1][2]), f2_inv(p, g[1][3])) if m_type else (g[1][2], g[1][3])
+    assert (cx, cy) == psi
+    return g
+
+
+def naf(n):
+    """signed binary digits of n, most significant first (the first digit is 1)"""
+    d = []
+    while n:
+        z = (2 - n % 4) if n & 1 else 0
+        n = (n - z) // 2
+        d.append(z)
+    return d[::-1]
+
+
+def pairing_extra(p, n, r, xi, frob, x, loop, signed):
+    """Constants of pairing.cuh: xi, the Frobenius coefficients, the Miller loop's digits (non-adjacent form when `signed`,
+    which saves additions for BN254's 6x + 2 but not for BLS12-381's sparse |x|) and |x| (plain words)."""
+    R = 1 << (32 * n)
+    digits = naf(loop) if signed else [int(b) for b in bin(loop)[2:]]
+    assert sum(d << (len(digits) - 1 - i) for i, d in enumerate(digits)) == loop and digits[0] == 1
+    pos = sum(1 << (len(digits) - 1 - i) for i, d in enumerate(digits) if d == 1)
+    neg = sum(1 << (len(digits) - 1 - i) for i, d in enumerate(digits) if d == -1)
+    lw = (len(digits) + 31) // 32
+    rows = [frob[j][k][c] for j in (1, 2, 3) for k in range(1, 6) for c in (0, 1)]
+    s = "    // pairing (pairing.cuh): xi = XI0 + u; frob(2 (5 (j - 1) + k - 1) + c, i) = component c of xi^(k (p^j - 1) / 6),\n"
+    s += "    // Montgomery, j = 1..3, k = 1..5; the Miller loop's signed digits (+1 in ate_pos, -1 in ate_neg, ATE_BITS digits,\n"
+    s += "    // the top one 1); |x| of the curve family in plain words and its sign\n"
+    s += "    static constexpr int XI0 = %d;\n" % xi[0]
+    s += "    B2S_HD static constexpr uint32_t frob(int j, int i) { constexpr uint32_t t[30][%d] = {%s}; return t[j][i]; }\n" % (
+        n, ", ".join(arr(v * R % p, n) for v in rows))
+    s += "    static constexpr int ATE_BITS = %d;\n" % len(digits)
+    s += "    static constexpr int ATE_WORDS = %d;\n" % lw
+    s += "    B2S_HD static constexpr uint32_t ate_pos(int i) { constexpr uint32_t t[%d] = %s; return t[i]; }\n" % (lw, words(pos, lw))
+    s += "    B2S_HD static constexpr uint32_t ate_neg(int i) { constexpr uint32_t t[%d] = %s; return t[i]; }\n" % (lw, words(neg, lw))
+    s += "    static constexpr bool X_NEG = %s;\n" % ("true" if x < 0 else "false")
+    s += "    B2S_HD static constexpr uint32_t x_abs(int i) { constexpr uint32_t t[2] = %s; return t[i]; }\n" % words(abs(x), 2)
+    return s
+
+
+def check_pairing_params():
+    """The loop lengths and the hard-part chains of pairing.cuh, as identities in the curve parameters."""
+    x, p, r = -BLS_X_ABS, BLS_P, BLS_R
+    h = (p ** 4 - p ** 2 + 1) // r
+    assert (x - 1) ** 2 * (x + p) * (x * x + p * p - 1) + 3 == 3 * h           # BLS12-381 hard part: f^(3 h)
+    x, p, r = BN_X, BN_P, BN_R
+    assert (6 * x + 2 + p - p * p + p ** 3) % r == 0                           # BN254 optimal ate loop
+    h = (p ** 4 - p ** 2 + 1) // r
+    lam = [1 + 6 * x + 12 * x * x + 12 * x ** 3, 4 * x + 6 * x * x + 12 * x ** 3, 6 * x + 6 * x * x + 12 * x ** 3,
+           -1 + 4 * x + 6 * x * x + 12 * x ** 3]
+    assert sum(l * p ** i for i, l in enumerate(lam)) == 2 * x * (6 * x * x + 3 * x + 1) * h   # BN254 hard part
+
+
 def main():
     out = "// GENERATED by tools/gen_field_params.py -- do not edit.\n"
     out += "// Montgomery constants (R = 2^(32 N)) for BLS12-381 / BN254 base and scalar fields.\n"
@@ -206,11 +298,16 @@ def main():
     bn_b2 = (27 * inv82 % BN_P, (-3 * inv82) % BN_P)
     bls_psi = psi_coeffs(BLS_P, BLS_R, (1, 1), BLS_G2, -BLS_X_ABS)
     bn_psi = psi_coeffs(BN_P, BN_R, (9, 1), BN_G2, 6 * BN_X * BN_X)
+    check_pairing_params()
+    bls_frob = frobenius_coeffs(BLS_P, (1, 1), bls_psi, True)
+    bn_frob = frobenius_coeffs(BN_P, (9, 1), bn_psi, False)
     out += field_struct("BlsFqP", BLS_P, 12, curve_extra(BLS_P, 12, BLS_G1, BLS_G2, 4, (4, 4))
-                        + decode_extra(BLS_P, 12, bls_beta(), bls_psi, BLS_X_ABS, 2))
+                        + decode_extra(BLS_P, 12, bls_beta(), bls_psi, BLS_X_ABS, 2)
+                        + pairing_extra(BLS_P, 12, BLS_R, (1, 1), bls_frob, -BLS_X_ABS, BLS_X_ABS, False))
     out += field_struct("BlsFrP", BLS_R, 8, fr_extra(BLS_R, 8, 7, 32))
     out += field_struct("BnFqP", BN_P, 8, curve_extra(BN_P, 8, BN_G1, BN_G2, 3, bn_b2)
-                        + decode_extra(BN_P, 8, 1, bn_psi, 6 * BN_X * BN_X, 4))
+                        + decode_extra(BN_P, 8, 1, bn_psi, 6 * BN_X * BN_X, 4)
+                        + pairing_extra(BN_P, 8, BN_R, (9, 1), bn_frob, BN_X, 6 * BN_X + 2, True))
     out += field_struct("BnFrP", BN_R, 8, fr_extra(BN_R, 8, 5, 28))
     out += "}  // namespace b2s\n"
     path = os.path.join(os.path.dirname(__file__), "..", "snark_b200", "csrc", "field_params.h")

@@ -1,0 +1,135 @@
+#!/usr/bin/env python3
+"""Batched Groth16 verification throughput (b2s_groth16_verify_batch) on one GPU.
+
+    python tools/verify_bench.py --curve bls12_381 --log-n 20 --n-inputs 16 --mem host
+
+Proofs are simulated (a verifying key with known logs, c = (ab - alpha beta - gamma IC) / delta), 2^12 distinct ones tiled
+to 2^log_n: the work per proof does not depend on its values.  One proof in 64 of the distinct set is broken (A + G1) and
+every verdict is checked.  Prints one JSON line: proofs/s over the timed calls, the per-kernel split from a separate profiled
+call, the time outside the kernels (host copies), the card and its power limit, and the algorithmic Fq-multiplication count
+per verification with that count times proofs/s as a fraction of the 2.6e10 Fq mul/s ceiling of DESIGN.md section 4 (that
+ceiling is the 381-bit one; for BN254 the fraction is against the same figure)."""
+import argparse
+import json
+import os
+import random
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+
+import gen_field_params as gp  # noqa: E402  (loop constants)
+
+CEILING = 2.6e10
+
+
+def fq_mul_count(curve, n_inputs):
+    """Fq multiplications of one verification, from the loop constants and the operation counts of pairing.cuh
+    (Fq2 mul 3, Fq2 square 2, Fq2 x Fq 2; Fq inverse ~ bits + bits / 2)."""
+    bls = curve == "bls12_381"
+    bits = 381 if bls else 254
+    inv_fq = bits + bits // 2
+    digits = [int(b) for b in bin(gp.BLS_X_ABS)[2:]] if bls else gp.naf(6 * gp.BN_X + 2)
+    steps, adds = len(digits) - 1, sum(1 for d in digits[1:] if d)
+    sqr12, mul12, cyc, ell, dbl, add = 36, 54, 18, 43, 28, 37
+    miller = (steps - 1) * sqr12 + steps * (dbl + 3 * ell) + adds * (add + 3 * ell)
+    if not bls:
+        miller += 2 * (6 + add + ell) + 2 * 2 * ell      # pi(Q), -pi^2(Q) lines: on the fly for B, prepared for the other two
+    inv12 = 36 + 15 + 9 + (4 + inv_fq + 2) + 9 + 36
+    xabs = gp.BLS_X_ABS if bls else gp.BN_X
+    exp_x = (xabs.bit_length() - 1) * cyc + (bin(xabs).count("1") - 1) * mul12
+    easy = inv12 + 2 * mul12 + 10
+    hard = (5 * exp_x + 5 * mul12 + 15 + 10 + cyc) if bls else (3 * exp_x + 3 * cyc + 9 * mul12 + 15 + 10 + 15)
+    ic = n_inputs * 32 * 255 / 256 * 10 + inv_fq + 3
+    return int(miller + easy + hard + ic)
+
+
+def gpu_info():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                             text=True, timeout=30).stdout.strip()
+        name, power = [s.strip() for s in out.split(",")]
+        return name, power
+    except Exception as e:   # noqa: BLE001
+        return f"unknown ({e})", "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--curve", choices=["bls12_381", "bn254"], default="bls12_381")
+    ap.add_argument("--log-n", type=int, default=20)
+    ap.add_argument("--n-inputs", type=int, default=1)
+    ap.add_argument("--mem", choices=["host", "device"], default="host")
+    ap.add_argument("--steps", type=int, default=3)
+    args = ap.parse_args()
+
+    from snark_b200 import Backend
+    from tests.test_gpu_verify import Sim
+
+    be = Backend(curve=0 if args.curve == "bls12_381" else 1)
+    rng = random.Random(20)
+    sim = Sim(be, rng, args.n_inputs)
+    base = 1 << min(12, args.log_n)
+    x, a, b = sim.scalars(rng, base)
+    c = sim.c_of(x, a, b)
+    broken = set(range(0, base, 64))
+    a = [(v + 1) % sim.curve.r if i in broken else v for i, v in enumerate(a)]
+    inputs, A, B, C = sim.arrays(x, a, b, c)
+    n = 1 << args.log_n
+    reps = n // base
+    inputs = np.tile(inputs, reps) if inputs is not None else None
+    A, B, C = np.tile(A, reps), np.tile(B, reps), np.tile(C, reps)
+    want = np.tile(np.array([i not in broken for i in range(base)]), reps)
+    if args.mem == "device":
+        import torch
+
+        dev = torch.device("cuda")
+        t = lambda arr: torch.from_numpy(arr.view(np.int32)).to(dev)
+        inputs = t(inputs) if inputs is not None else None
+        A, B, C = t(A), t(B), t(C)
+        okd = torch.zeros(n, dtype=torch.uint8, device=dev)
+
+        def run():
+            be.groth16_verify_batch(sim.pvk, inputs, args.n_inputs, A, B, C, n_proofs=n, ok=okd)
+            be.sync()
+            return okd.cpu().numpy().astype(bool)
+    else:
+        def run():
+            return be.groth16_verify_batch(sim.pvk, inputs, args.n_inputs, A, B, C)
+
+    assert np.array_equal(run(), want), "verdicts differ from the expected ones"   # warm-up, and the check
+    times = []
+    for _ in range(args.steps):
+        t0 = time.perf_counter()
+        ok = run()
+        times.append(time.perf_counter() - t0)
+        assert np.array_equal(ok, want)
+    be.profile(True)
+    t0 = time.perf_counter()
+    run()
+    prof_s = time.perf_counter() - t0
+    rep = be.profile_report()
+    be.profile(False)
+    kern = {k: round(v[1], 3) for k, v in rep.items()}
+    best = min(times)
+    pps = n / best
+    muls = fq_mul_count(args.curve, args.n_inputs)
+    name, power = gpu_info()
+    print(json.dumps({
+        "curve": args.curve, "n_proofs": n, "n_inputs": args.n_inputs, "mem": args.mem,
+        "seconds": [round(s, 4) for s in times], "proofs_per_s": round(pps, 1),
+        "kernel_ms": kern, "outside_kernels_ms": round(prof_s * 1e3 - sum(kern.values()), 3),
+        "fq_mul_per_verification": muls, "fq_mul_per_s": round(muls * pps, 1), "fraction_of_ceiling": round(muls * pps / CEILING, 4),
+        "gpu": name, "power_limit": power, "invalid_checked": int((~want).sum()),
+    }))
+    be.pvk_free(sim.pvk)
+    be.close()
+
+
+if __name__ == "__main__":
+    main()
