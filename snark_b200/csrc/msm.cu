@@ -13,7 +13,10 @@
 //               (a bucket of s points is cut into ceil(s / L) tasks so that no thread ever owns more
 //               than L points -- this is what keeps degenerate scalar distributions, e.g. the all-equal
 //               witness of the reference's DummyCircuit (relations/src/sr1cs/mod.rs:306-309), balanced)
-//   3 scatter   counting-sort the point indices (sign in bit 31) by bucket
+//   3 sort      the point indices (sign in bit 31) by bucket, in two passes that write whole runs instead of one entry per
+//               atomic: partition (per tile of 4096 scalars and per window, a shared-memory counting sort by coarse bin
+//               key >> F, one global atomic per non-empty coarse bin) and place (per coarse bin, a shared-memory counting
+//               sort by fine key into the exact bucket offsets); 6 B of scratch per entry
 //   3a rank     buckets are ranked by decreasing size (second counting sort) and task numbers follow the ranks, so
 //               the 32 tasks a warp runs in lockstep have equal length (uniform scalars give Poisson bucket sizes)
 //   3b for big problems (windows * n >= 2^27; B2S_MSM_AFFINE_ROUNDS overrides) three batched-affine halving rounds,
@@ -40,6 +43,17 @@ namespace b2s {
 // ---- signed-digit recoding -------------------------------------------------------------------------
 // Digits of a canonical 256-bit scalar, least significant window first.  Windows other than the
 // last are recoded into [-2^(c-1), 2^(c-1)); the last keeps the carry (shape guarantees it fits B).
+// v holds the scalar words around window w (bit w * c sits at bit `off` of v); carry is the recoding state between windows
+__device__ __forceinline__ int32_t recode_digit(uint64_t v, uint32_t off, uint32_t& carry, uint32_t w, uint32_t c, uint32_t nwin) {
+    uint32_t d = (uint32_t)((v >> off) & ((1u << c) - 1u)) + carry;
+    carry = 0;
+    if (w != nwin - 1 && d >= (1u << (c - 1))) {
+        carry = 1;
+        return (int32_t)d - (int32_t)(1u << c);
+    }
+    return (int32_t)d;
+}
+
 struct DigitIter {
     uint32_t k[8];
     uint32_t carry;
@@ -49,13 +63,7 @@ struct DigitIter {
         uint64_t v = 0;
         if (word < 8) v = k[word];
         if (word + 1 < 8) v |= (uint64_t)k[word + 1] << 32;
-        uint32_t d = (uint32_t)((v >> off) & ((1u << c) - 1u)) + carry;
-        carry = 0;
-        if (w != nwin - 1 && d >= (1u << (c - 1))) {
-            carry = 1;
-            return (int32_t)d - (int32_t)(1u << c);
-        }
-        return (int32_t)d;
+        return recode_digit(v, off, carry, w, c, nwin);
     }
 };
 
@@ -246,29 +254,236 @@ msm_scan_apply_kernel(const uint32_t* __restrict__ counts, const uint32_t* __res
     }
 }
 
-template <class Fr>
-__global__ void msm_scatter_kernel(const Fr* __restrict__ scalars, const uint32_t* __restrict__ index_map, uint64_t n, bool mont, MsmShape sh,
-                                   const uint32_t* __restrict__ offsets, uint32_t* __restrict__ cursor,
-                                   uint32_t* __restrict__ sorted) {
-    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const unsigned active = __activemask();
-    const unsigned lane = threadIdx.x & 31;
-    DigitIter it;
-    load_scalar(it, scalars, i, mont);
-    const uint32_t base_idx = index_map ? index_map[i] : (uint32_t)i;
-    for (uint32_t w = 0; w < sh.nwin; w++) {
-        const int32_t d = it.next(w, sh.c, sh.nwin);
-        const uint32_t key = d != 0 ? (sh.pre_stride ? 0u : w * sh.B) + (uint32_t)(d < 0 ? -d : d) - 1 : 0xffffffffu;
-        const unsigned peers = __match_any_sync(active, key);
-        const unsigned leader = (unsigned)(__ffs(peers) - 1);
-        uint32_t base = 0;
-        if (key != 0xffffffffu && lane == leader) base = atomicAdd(&cursor[key], (uint32_t)__popc(peers));
-        base = __shfl_sync(peers, base, leader);
-        if (key != 0xffffffffu) {
-            const uint32_t rank = __popc(peers & ((1u << lane) - 1u));
-            sorted[offsets[key] + base + rank] = (base_idx + w * sh.pre_stride) | (d < 0 ? 0x80000000u : 0u);
+// ---- sort of the digits by bucket, in two passes ----------------------------------------------------------------------
+// The entries of bucket g go to sorted[offsets[g] .. offsets[g+1]).  Scattering them one by one costs a returning global
+// atomic and a lone 4 B store per entry (uniform scalars almost never share a bucket within a warp).  Instead:
+//   partition  per CTA of SORT_TILE scalars and per window, a counting sort in shared memory by coarse bin (key >> F);
+//              one global atomic per non-empty (CTA, coarse bin) reserves a run inside the bin's region, which starts at
+//              offsets[bin << F] because offsets are exact.  Runs leave as u32 entries plus the u16 fine key key & (2^F - 1).
+//   place      per coarse bin, chunks of SORT_CHUNK entries are counting-sorted by fine key in shared memory and written
+//              to offsets[key] + (shared-memory cursor).  A bin above SORT_SPLIT entries (skewed scalars: a window whose
+//              digits all agree) is cut into parts for the split CTAs, which reserve per (part, fine bucket) on cursor[key].
+// F is chosen so that uniform scalars give ~16 entries per (CTA, window, coarse bin): 64 B runs instead of 4 B stores.
+static constexpr uint32_t SORT_THREADS = 1024;
+static constexpr uint32_t SORT_TILE = 4096;           // scalars per partition CTA
+static constexpr uint32_t SORT_PER = SORT_TILE / SORT_THREADS;
+static constexpr uint32_t SORT_CHUNK = 16384;         // entries per place chunk
+static constexpr uint32_t SORT_CHUNK_PER = SORT_CHUNK / SORT_THREADS;
+static constexpr uint32_t SORT_SPLIT = 8 * SORT_CHUNK;
+static constexpr uint32_t SORT_MAX_F = 11;            // fine keys fit in u16, fine-bucket arrays of one place CTA in 24 KiB
+
+// coarse bins per window = SORT_TILE / 16 = 256 where the window has that many buckets, with at most 2^SORT_MAX_F buckets each
+static uint32_t sort_fine_bits(uint32_t c) { return std::min<uint32_t>(SORT_MAX_F, c > 9 ? c - 9 : 0); }
+static size_t partition_smem(uint32_t nbw) { return ((size_t)10 * SORT_TILE + 3 * (size_t)nbw + 1) * sizeof(uint32_t); }
+static size_t place_smem(uint32_t F) {
+    return (size_t)SORT_CHUNK * (sizeof(uint32_t) + sizeof(uint16_t)) + ((size_t)3 * (1u << F) + 1 + SORT_THREADS + 1) * sizeof(uint32_t);
+}
+
+// in[0..n) -> out[0..n]: exclusive prefix sums, out[n] = total.  Called by every thread of the CTA; ends with a barrier.
+__device__ void block_excl_scan(const uint32_t* in, uint32_t* out, uint32_t n) {
+    __shared__ uint32_t wsum[32];
+    const uint32_t per = (n + blockDim.x - 1) / blockDim.x;
+    const uint32_t lo = min(threadIdx.x * per, n), hi = min(lo + per, n);
+    uint32_t s = 0;
+    for (uint32_t i = lo; i < hi; i++) s += in[i];
+    const unsigned lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    uint32_t incl = s;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t o = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= (unsigned)d) incl += o;
+    }
+    if (lane == 31) wsum[wid] = incl;
+    __syncthreads();
+    if (wid == 0) {
+        uint32_t w = lane < (blockDim.x >> 5) ? wsum[lane] : 0u;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t o = __shfl_up_sync(0xffffffffu, w, d);
+            if (lane >= (unsigned)d) w += o;
         }
+        wsum[lane] = w;
+    }
+    __syncthreads();
+    uint32_t run = incl - s + (wid ? wsum[wid - 1] : 0u);
+    for (uint32_t i = lo; i < hi; i++) { out[i] = run; run += in[i]; }
+    if (threadIdx.x == 0) out[n] = wsum[31];
+    __syncthreads();
+}
+
+// Pass 1.  Scalars are kept canonical in shared memory, word-major, so that each window reads its two words without bank
+// conflicts and the recoding carry walks the windows in order.
+template <class Fr>
+__global__ void __launch_bounds__(SORT_THREADS, 1)
+msm_partition_kernel(const Fr* __restrict__ scalars, const uint32_t* __restrict__ index_map, uint64_t n, bool mont, MsmShape sh, uint32_t F,
+                     const uint32_t* __restrict__ offsets, uint32_t* __restrict__ bin_cursor, uint32_t* __restrict__ part_val,
+                     uint16_t* __restrict__ part_fine) {
+    extern __shared__ uint4 sort_smem[];
+    const uint32_t nbw = sh.B >> F;                          // coarse bins per window
+    uint32_t* sc = reinterpret_cast<uint32_t*>(sort_smem);   // [8][SORT_TILE] scalar words
+    uint32_t* sv = sc + 8 * SORT_TILE;                       // staged entries of one window, ordered by coarse bin
+    uint32_t* sk = sv + SORT_TILE;                           // their window-local bucket |digit| - 1
+    uint32_t* hist = sk + SORT_TILE;                         // [nbw]
+    uint32_t* start = hist + nbw;                            // [nbw + 1]
+    uint32_t* dest = start + nbw + 1;                        // [nbw] staged entry i of bin b goes to dest[b] + i
+    const uint64_t tile = (uint64_t)blockIdx.x * SORT_TILE;
+    const uint32_t cnt = (uint32_t)min((uint64_t)SORT_TILE, n - tile);
+    uint32_t base[SORT_PER];
+#pragma unroll
+    for (uint32_t j = 0; j < SORT_PER; j++) {
+        const uint32_t s = threadIdx.x + j * SORT_THREADS;
+        if (s < cnt) {
+            DigitIter it;
+            load_scalar(it, scalars, tile + s, mont);
+#pragma unroll
+            for (int q = 0; q < 8; q++) sc[q * SORT_TILE + s] = it.k[q];
+            base[j] = index_map ? index_map[tile + s] : (uint32_t)(tile + s);
+        }
+    }
+    for (uint32_t b = threadIdx.x; b < nbw; b += SORT_THREADS) hist[b] = 0;
+    uint32_t carry = 0;                                      // bit j: recoding carry of scalar j
+    __syncthreads();
+    for (uint32_t w = 0; w < sh.nwin; w++) {
+        const uint32_t bit = w * sh.c, word = bit >> 5, off = bit & 31;
+        uint32_t ent[SORT_PER], rank[SORT_PER];              // ent: bucket | sign << 31, or ~0u for a zero digit
+#pragma unroll
+        for (uint32_t j = 0; j < SORT_PER; j++) {
+            const uint32_t s = threadIdx.x + j * SORT_THREADS;
+            ent[j] = ~0u;
+            if (s < cnt) {
+                uint64_t v = 0;
+                if (word < 8) v = sc[word * SORT_TILE + s];
+                if (word + 1 < 8) v |= (uint64_t)sc[(word + 1) * SORT_TILE + s] << 32;
+                uint32_t cy = (carry >> j) & 1u;
+                const int32_t d = recode_digit(v, off, cy, w, sh.c, sh.nwin);
+                carry = (carry & ~(1u << j)) | (cy << j);
+                if (d != 0) {
+                    const uint32_t lk = (uint32_t)(d < 0 ? -d : d) - 1;
+                    ent[j] = lk | (d < 0 ? 0x80000000u : 0u);
+                    rank[j] = atomicAdd(&hist[lk >> F], 1u);
+                }
+            }
+        }
+        __syncthreads();
+        block_excl_scan(hist, start, nbw);
+        const uint32_t bin0 = sh.pre_stride ? 0u : w * nbw;
+        for (uint32_t b = threadIdx.x; b < nbw; b += SORT_THREADS) {
+            const uint32_t k = hist[b];
+            if (k) dest[b] = offsets[(bin0 + b) << F] + atomicAdd(&bin_cursor[bin0 + b], k) - start[b];
+            hist[b] = 0;
+        }
+#pragma unroll
+        for (uint32_t j = 0; j < SORT_PER; j++) {
+            if (ent[j] != ~0u) {
+                const uint32_t lk = ent[j] & 0x7fffffffu;
+                const uint32_t p = start[lk >> F] + rank[j];
+                sv[p] = (base[j] + w * sh.pre_stride) | (ent[j] & 0x80000000u);
+                sk[p] = lk;
+            }
+        }
+        __syncthreads();
+        const uint32_t total = start[nbw];
+        for (uint32_t i = threadIdx.x; i < total; i += SORT_THREADS) {
+            const uint32_t lk = sk[i];
+            const uint32_t o = dest[lk >> F] + i;
+            part_val[o] = sv[i];
+            part_fine[o] = (uint16_t)(lk & ((1u << F) - 1u));
+        }
+        __syncthreads();
+    }
+}
+
+// One chunk of a coarse bin: entries [c0, c0 + len) sorted by fine key; cur[f] is where the next entry of fine bucket f goes
+// and is advanced past this chunk's entries.
+__device__ __forceinline__ void place_chunk(uint32_t c0, uint32_t len, uint32_t nf, const uint32_t* __restrict__ part_val,
+                                            const uint16_t* __restrict__ part_fine, uint32_t* __restrict__ sorted, uint32_t* sv, uint16_t* sf,
+                                            uint32_t* hist, uint32_t* start, uint32_t* cur) {
+    uint32_t fr[SORT_CHUNK_PER];                             // fine key | rank << 16, or ~0u past the end
+#pragma unroll
+    for (uint32_t j = 0; j < SORT_CHUNK_PER; j++) {
+        const uint32_t i = threadIdx.x + j * SORT_THREADS;
+        fr[j] = ~0u;
+        if (i < len) {
+            const uint32_t f = part_fine[c0 + i];
+            fr[j] = f | atomicAdd(&hist[f], 1u) << 16;
+        }
+    }
+    __syncthreads();
+    block_excl_scan(hist, start, nf);
+#pragma unroll
+    for (uint32_t j = 0; j < SORT_CHUNK_PER; j++) {
+        if (fr[j] != ~0u) {
+            const uint32_t f = fr[j] & 0xffffu;
+            const uint32_t p = start[f] + (fr[j] >> 16);
+            sv[p] = part_val[c0 + threadIdx.x + j * SORT_THREADS];
+            sf[p] = (uint16_t)f;
+        }
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < len; i += SORT_THREADS) {
+        const uint32_t f = sf[i];
+        sorted[cur[f] + i - start[f]] = sv[i];
+    }
+    __syncthreads();
+    for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) {
+        cur[f] += hist[f];
+        hist[f] = 0;
+    }
+    __syncthreads();
+}
+
+// Pass 2.  CTA b < nbins places coarse bin b when it holds at most SORT_SPLIT entries, with its cursors in shared memory.
+// The CTAs after them share the larger bins, in parts of SORT_SPLIT entries dealt round-robin: a part counts its fine keys
+// first and reserves one run per non-empty fine bucket with an atomic on cursor[key] (zeroed by the caller).
+__global__ void __launch_bounds__(SORT_THREADS, 1)
+msm_place_kernel(const uint32_t* __restrict__ offsets, uint32_t nbins, uint32_t F, const uint32_t* __restrict__ part_val,
+                 const uint16_t* __restrict__ part_fine, uint32_t* __restrict__ cursor, uint32_t* __restrict__ sorted) {
+    extern __shared__ uint4 sort_smem[];
+    const uint32_t nf = 1u << F;
+    uint32_t* sv = reinterpret_cast<uint32_t*>(sort_smem);  // [SORT_CHUNK]
+    uint16_t* sf = reinterpret_cast<uint16_t*>(sv + SORT_CHUNK);
+    uint32_t* hist = reinterpret_cast<uint32_t*>(sf + SORT_CHUNK);   // [nf]
+    uint32_t* start = hist + nf;                             // [nf + 1]
+    uint32_t* cur = start + nf + 1;                          // [nf]
+    uint32_t* big = cur + nf;                                // [SORT_THREADS] bins to split, then their number
+    uint32_t* nbig = big + SORT_THREADS;
+    for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) hist[f] = 0;
+    if (blockIdx.x < nbins) {
+        const uint32_t k0 = blockIdx.x << F;
+        const uint32_t lo = offsets[k0], hi = offsets[k0 + nf];
+        if (hi == lo || hi - lo > SORT_SPLIT) return;
+        for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) cur[f] = offsets[k0 + f];
+        __syncthreads();
+        for (uint32_t c0 = lo; c0 < hi; c0 += SORT_CHUNK) place_chunk(c0, min(SORT_CHUNK, hi - c0), nf, part_val, part_fine, sorted, sv, sf, hist, start, cur);
+        return;
+    }
+    const uint32_t s = blockIdx.x - nbins, S = gridDim.x - nbins;
+    for (uint32_t b0 = 0; b0 < nbins; b0 += SORT_THREADS) {
+        const uint32_t b = b0 + threadIdx.x;
+        const bool is_big = b < nbins && offsets[(b + 1) << F] - offsets[b << F] > SORT_SPLIT;
+        if (threadIdx.x == 0) *nbig = 0;
+        if (!__syncthreads_or(is_big)) continue;
+        if (is_big) big[atomicAdd(nbig, 1u)] = b;
+        __syncthreads();
+        const uint32_t m = *nbig;
+        for (uint32_t q = 0; q < m; q++) {
+            const uint32_t bb = big[q], k0 = bb << F;
+            const uint32_t lo = offsets[k0], hi = offsets[k0 + nf];
+            const uint32_t parts = (hi - lo + SORT_SPLIT - 1) / SORT_SPLIT;
+            for (uint32_t p = (s + S - bb % S) % S; p < parts; p += S) {
+                const uint32_t p0 = lo + p * SORT_SPLIT, p1 = min(hi, p0 + SORT_SPLIT);
+                for (uint32_t i = p0 + threadIdx.x; i < p1; i += SORT_THREADS) atomicAdd(&hist[part_fine[i]], 1u);
+                __syncthreads();
+                for (uint32_t f = threadIdx.x; f < nf; f += SORT_THREADS) {
+                    const uint32_t k = hist[f];
+                    if (k) cur[f] = offsets[k0 + f] + atomicAdd(&cursor[k0 + f], k);
+                    hist[f] = 0;
+                }
+                __syncthreads();
+                for (uint32_t c0 = p0; c0 < p1; c0 += SORT_CHUNK) place_chunk(c0, min(SORT_CHUNK, p1 - c0), nf, part_val, part_fine, sorted, sv, sf, hist, start, cur);
+            }
+        }
+        __syncthreads();
     }
 }
 
@@ -633,7 +848,23 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
     B2S_LAUNCH(c, msm_scan_tiles_kernel, ntiles, SCAN_THREADS, 0, counts, no_perm, sh, tiles.as<Scan3>());
     B2S_LAUNCH(c, msm_scan_spine_kernel, 1, 1024, 0, tiles.as<Scan3>(), ntiles, sh, offsets, task_off, heavy);
     B2S_LAUNCH(c, msm_scan_apply_kernel, ntiles, SCAN_THREADS, 0, counts, no_perm, sh, tiles.as<Scan3>(), offsets, task_off, heavy);
-    B2S_LAUNCH(c, msm_scatter_kernel<Fr>, cdiv(n, 256), 256, 0, scalars, index_map, n, mont, sh, offsets, cursor, sorted.as<uint32_t>());
+    {
+        // the partitioned entries (u32 value + u16 fine key) go back to the pool before bucket_sums_t allocates its rounds
+        const uint32_t fine_bits = sort_fine_bits(sh.c), nbins = sh.G >> fine_bits, nbw = sh.B >> fine_bits;
+        const uint64_t T = (uint64_t)sh.nwin * n;
+        DevBuf part;
+        B2S_TRY(part.alloc(c, (size_t)T * (sizeof(uint32_t) + sizeof(uint16_t)) + (size_t)nbins * sizeof(uint32_t)));
+        uint32_t* part_val = part.as<uint32_t>();
+        uint32_t* bin_cursor = part_val + T;
+        uint16_t* part_fine = reinterpret_cast<uint16_t*>(bin_cursor + nbins);
+        B2S_CUDA(c, cudaMemsetAsync(bin_cursor, 0, (size_t)nbins * sizeof(uint32_t), c->stream));
+        B2S_SMEM_ATTR(c, msm_partition_kernel<Fr>, partition_smem(nbw));
+        B2S_SMEM_ATTR(c, msm_place_kernel, place_smem(fine_bits));
+        B2S_LAUNCH(c, msm_partition_kernel<Fr>, cdiv(n, SORT_TILE), SORT_THREADS, partition_smem(nbw), scalars, index_map, n, mont, sh, fine_bits,
+                   (const uint32_t*)offsets, bin_cursor, part_val, part_fine);
+        B2S_LAUNCH(c, msm_place_kernel, nbins + c->sm_count, SORT_THREADS, place_smem(fine_bits), (const uint32_t*)offsets, nbins, fine_bits,
+                   (const uint32_t*)part_val, (const uint16_t*)part_fine, cursor, sorted.as<uint32_t>());
+    }
     B2S_TRY((bucket_sums_t<Curve, F>(c, bases, sorted.as<uint32_t>(), counts, offsets, (uint64_t)sh.nwin * n, sh.G, rp, bucket_acc.as<Pt>())));
     // bucket reduction: compiled with the multiplication inlined (msm_acc_g1.cu), 2 general additions per bucket
     if (is_g1) B2S_TRY(msm_bucket_reduce_g1(c, bucket_acc.p, sh_red, MSM_SEG, segs.p, segs_per_win, wins_p));
