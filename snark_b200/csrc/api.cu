@@ -71,19 +71,10 @@ int32_t b2s_ctx_create(int32_t curve_id, int32_t device_ordinal, b2s_ctx** out) 
     if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&c->aux, cudaStreamNonBlocking) != cudaSuccess ||
         cudaStreamCreateWithFlags(&c->side, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->ev_tail, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&c->ev_done, cudaEventDisableTiming) != cudaSuccess) {
         delete c;
         return B2S_ERR_CUDA;
-    }
-    // gathers of 96-byte points: a 32-byte L2 fetch granularity (instead of the default 64) avoids fetching bytes
-    // next to a randomly addressed point (a hint; B2S_L2_GRAN overrides, 0 leaves the driver default)
-    {
-        const char* g = getenv("B2S_L2_GRAN");
-        const long gran = g ? strtol(g, nullptr, 10) : 0;
-        if (gran > 0) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)gran);
     }
     if (cudaMalloc(&c->aux_ring, b2s::Ctx::AUX_SLOT_BYTES * b2s::Ctx::AUX_SLOTS) != cudaSuccess) {
         delete c;
@@ -109,8 +100,6 @@ void b2s_ctx_destroy(b2s_ctx* ctx) {
     cudaStreamSynchronize(ctx->aux);
     cudaStreamSynchronize(ctx->side);
     if (ctx->aux_ring) cudaFree(ctx->aux_ring);
-    cudaEventDestroy(ctx->ev_fork);
-    cudaEventDestroy(ctx->ev_join);
     cudaStreamDestroy(ctx->side);
     cudaEventDestroy(ctx->ev_tail);
     cudaEventDestroy(ctx->ev_done);

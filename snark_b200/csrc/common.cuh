@@ -27,10 +27,8 @@ struct Ctx {
     // second stream for latency-bound MSM tails (Horner) so they overlap the next MSM's bucket work
     cudaStream_t aux = nullptr;
     cudaEvent_t ev_tail = nullptr, ev_done = nullptr;
-    // third stream: the witness map of a proof runs here, side by side with the MSMs that only need z (their latency-bound
-    // phases -- sampling synchronisations, inversion levels, small reductions -- leave the SMs to the transforms)
+    // third stream: host-to-device copies of the point loader (deserialize.cu) overlap the decoding of the previous chunk
     cudaStream_t side = nullptr;
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
     bool aux_pending = false;
     std::mutex mu;
     std::string err;

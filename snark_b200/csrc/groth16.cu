@@ -221,28 +221,7 @@ static int32_t shard_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* 
     P1* g1 = reinterpret_cast<P1*>(g1_out);
     P1* w1 = tails.as<P1>();
     void* w2 = w1 + 4 * 64;
-    // Fork: the witness map (SpMV, six transforms, quotient -- or its distributed form) is enqueued on the side stream and
-    // runs side by side with the four MSMs that only need z; the h-query MSM joins them.  The ctx's launch stream is swapped
-    // for the duration of the enqueue (everything below the C ABI launches and allocates on c->stream).
     const void* h_shard = nullptr;
-    // OFF by default: both sides are fmaheavy-bound, so the transforms only run slower next to the MSM kernels.  Measured at
-    // domain 2^24 on an H100 80GB HBM3 at a 400 W limit: 342 vs 260 ms per proof with z resident, 271 vs 264 ms with z in
-    // host memory.  B2S_SIDE_STREAM=1 enables it
-    const bool fork = getenv("B2S_SIDE_STREAM") != nullptr;
-    struct SideGuard {   // an error return must not leave work in flight on the side stream over buffers being released
-        Ctx* c; cudaStream_t main; bool active;
-        ~SideGuard() { if (active) { c->stream = main; cudaStreamSynchronize(c->side); } }
-    } side_guard{c, c->stream, false};
-    if (fork) {
-        B2S_CUDA(c, cudaEventRecord(c->ev_fork, c->stream));
-        B2S_CUDA(c, cudaStreamWaitEvent(c->side, c->ev_fork, 0));
-        side_guard.active = true;
-        c->stream = c->side;
-        const int32_t st = hs->get(c, pk, m, zd, &h_shard);
-        c->stream = side_guard.main;
-        if (st != B2S_OK) return st;
-        B2S_CUDA(c, cudaEventRecord(c->ev_join, c->side));
-    }
     // the MSMs that only need z (their Horner tails run on the aux stream under the following work); G2 first because its
     // tail is the longest
     // a, b_g1, b_g2 (and l, when its range coincides) run over the same scalars: classify them once (msm.cu)
@@ -262,12 +241,9 @@ static int32_t shard_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* 
     B2S_TRY(msm(Q_A, g1 + 2, w1 + 2 * 64));
     B2S_TRY(msm(Q_B_G1, g1 + 3, w1 + 3 * 64));
     B2S_TRY(msm(Q_L, g1 + 1, w1 + 1 * 64));
-    if (fork) {
-        B2S_CUDA(c, cudaStreamWaitEvent(c->stream, c->ev_join, 0));
-        side_guard.active = false;
-    } else {
-        B2S_TRY(hs->get(c, pk, m, zd, &h_shard));
-    }
+    // the witness map (SpMV, six transforms, quotient -- or its distributed form) runs after those MSMs, not beside them on a
+    // side stream: both are fmaheavy-bound (domain 2^24, H100 80GB HBM3 at 400 W: 342 vs 260 ms per proof with z resident)
+    B2S_TRY(hs->get(c, pk, m, zd, &h_shard));
     if (pk->h_table.p) B2S_TRY(msm(Q_H, g1 + 0, w1 + 0 * 64, pk->h_table.p, &pk->h_pre));
     else B2S_TRY(msm(Q_H, g1 + 0, w1 + 0 * 64));
     B2S_TRY(msm_join_tails(c));

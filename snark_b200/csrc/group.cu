@@ -153,9 +153,7 @@ static int32_t prove_group(b2s_group* g, const b2s_pk* pk, const b2s_r1cs* m, co
     uint32_t lg = 0;
     while ((1 << lg) < g->world) lg++;
     if (g->world > 1 && (g->agreed_pk != pk || g->agreed_m != m)) {
-        const char* env = getenv("B2S_DIST_WITNESS");
-        const int32_t mine_ok = ((1 << lg) == g->world && dist_supported(m->log_domain, lg) && slab_aligned(pk, m, g->rank, g->world) &&
-                                 !(env && env[0] == '0')) ? 1 : 0;
+        const int32_t mine_ok = ((1 << lg) == g->world && dist_supported(m->log_domain, lg) && slab_aligned(pk, m, g->rank, g->world)) ? 1 : 0;
         DevBuf flags;
         B2S_TRY(flags.alloc(ctx, sizeof(int32_t) * (size_t)(g->world + 1)));
         int32_t* fd = flags.as<int32_t>();

@@ -33,7 +33,6 @@
 // bound by the fma pipe by two orders of magnitude over HBM (DESIGN.md has the numbers).
 #include <algorithm>
 #include <array>
-#include <chrono>
 #include <cstring>
 
 #include "msm_affine.cuh"
@@ -609,10 +608,10 @@ static MsmShape msm_shape(uint64_t n, uint32_t scalar_bits, size_t point_bytes, 
 
 // ---- bucket sums of an arbitrary bucket structure ---------------------------------------------------------------
 // How many batched-affine rounds pay for T entries in G buckets, and the XYZZ task length after them.
-struct RoundPlan { uint32_t rounds, L; uint64_t max_tasks; bool stage; };
+struct RoundPlan { uint32_t rounds, L; uint64_t max_tasks; };
 template <class F>
-static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_t L_default, bool random_gathers) {
-    RoundPlan rp{0, L_default, T / L_default + G + 1, false};
+static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_t L_default) {
+    RoundPlan rp{0, L_default, T / L_default + G + 1};
     uint32_t ba_auto = 0;
     const uint64_t per_bucket = G ? T / G : 0;
     while ((1ull << ba_auto) < per_bucket) ba_auto++;
@@ -642,14 +641,7 @@ static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_
             }
         }
         if (need + ((uint64_t)2 << 30) > (uint64_t)free_b + pool_held) rp.rounds = 0;
-        // staged first round (the points of a random-access first round are fetched once and written out as pairs; 2 more
-        // points per output).  OFF by default: the gather count is the same and pass 1 now also writes 192 B per pair.  Measured
-        // with tools/msm_probe.py (2^24 uniform G1, H100 80GB HBM3 at a 400 W limit): 174 vs 161 ms per MSM, pass 1 23.8 -> 45.5 ms
-        // for pass 2 67.0 -> 60.9 ms
-        const uint64_t need_stage = need + 2 * t0 * sizeof(Affine<F>);
-        rp.stage = rp.rounds && random_gathers && env_u32("B2S_MSM_STAGE", 0) && need_stage + ((uint64_t)4 << 30) <= (uint64_t)free_b + pool_held;
     }
-    if (rp.rounds && getenv("B2S_MSM_AFFINE_ROUNDS")) rp.stage = random_gathers && env_u32("B2S_MSM_STAGE", 0);
     if (rp.rounds && !getenv("B2S_MSM_L")) {
         // what the XYZZ kernel sees after the rounds is 2^-R of the input: cut its tasks accordingly, otherwise the heavy
         // buckets of skewed scalars (a few thousand tasks of ~1000 points) leave most of the machine idle
@@ -685,7 +677,7 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
     const uint32_t* acc_sorted = sorted;
     const uint32_t* acc_offsets = offsets;
     const uint32_t* acc_counts = counts;
-    DevBuf ba_ints, ba_out[2], ba_prefix, ba_tot, ba_bits, ba_staged;
+    DevBuf ba_ints, ba_out[2], ba_prefix, ba_tot, ba_bits;
     if (rp.rounds) {
         // two internal (counts, offsets) pairs: the caller's arrays are only READ (round 0), so a bucket structure can be
         // shared by several calls (the heavy lists of a, b_g1, b_g2 of one proof)
@@ -693,7 +685,6 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
         uint32_t* pp_cnt[2] = {ba_ints.as<uint32_t>(), ba_ints.as<uint32_t>() + 2 * G + 1};
         uint32_t* pp_off[2] = {pp_cnt[0] + G, pp_cnt[1] + G};
         const uint32_t* cnt_in = counts;
-        const uint32_t* off_in = offsets;
         uint64_t t_in = T;
         // outputs of a round: every bucket keeps ceil(count / 2) points -- at most (t_in + G) / 2 and never more than t_in
         auto round_bound = [&](uint64_t tin) { return std::min<uint64_t>(tin, (tin + G) / 2 + 1); };
@@ -714,7 +705,6 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
         B2S_CUDA(c, cudaMemsetAsync(ba_ctr.p, 0, (size_t)2 * rp.rounds * sizeof(uint32_t), c->stream));
         // the two ping-pong output buffers, sized for the rounds that use them (even rounds write [1], odd rounds [0])
         B2S_TRY(ba_out[1].alloc(c, out_bound0 * sizeof(Affine<F>)));
-        if (rp.stage) B2S_TRY(ba_staged.alloc(c, 2 * out_bound0 * sizeof(Affine<F>)));
         if (rp.rounds > 1) B2S_TRY(ba_out[0].alloc(c, round_bound(out_bound0) * sizeof(Affine<F>)));
         const void* prev = nullptr;
         for (uint32_t r = 0; r < rp.rounds; r++) {
@@ -740,15 +730,12 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
             ra.target_units = target_units;
             ra.unit_ctr = ba_ctr.as<uint32_t>() + 2 * r;
             ra.prefix = ba_prefix.p; ra.tot = ba_tot.p; ra.inv_scratch = ba_tot.as<F>() + tot_bound; ra.out = ba_out[nxt ^ 1].p;   // even rounds write [1], odd rounds [0]
-            ra.staged = (r == 0 && rp.stage) ? ba_staged.p : nullptr;
             if (is_g1) B2S_TRY(msm_ba_round_g1(c, ra));
             else B2S_TRY(msm_ba_round_g2(c, ra));
             prev = ba_out[nxt ^ 1].p;
             t_in = out_bound;
             cnt_in = cnt_out;
-            off_in = off_out;
         }
-        (void)off_in;
         acc_bases = prev;
         acc_sorted = nullptr;
         acc_offsets = pp_off[(rp.rounds - 1) & 1u];
@@ -762,7 +749,7 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
     // task ranks by decreasing bucket size (skipped after affine rounds, which leave the natural order)
     const uint32_t* perm = nullptr;
     DevBuf perm_buf;
-    if (!rp.rounds && G >= 1024 && env_u32("B2S_MSM_SIZE_SORT", 1)) {
+    if (!rp.rounds && G >= 1024) {
         B2S_TRY(perm_buf.alloc(c, ((size_t)G + 2 * SIZE_BINS) * sizeof(uint32_t)));
         uint32_t* pm = perm_buf.as<uint32_t>();
         uint32_t* hist = pm + G;
@@ -802,21 +789,12 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
         B2S_CUDA(c, cudaMemsetAsync(out, 0, sizeof(Pt), c->stream));
         return B2S_OK;
     }
-    const bool host_timing = getenv("B2S_HOST_TIMING") != nullptr;
-    auto t_host0 = std::chrono::steady_clock::now();
-    auto lap = [&](const char* what) {
-        if (!host_timing) return;
-        auto t1 = std::chrono::steady_clock::now();
-        fprintf(stderr, "[b2s-host] msm_core n=%llu %-14s %.3f ms\n", (unsigned long long)n, what, std::chrono::duration<double, std::milli>(t1 - t_host0).count());
-        t_host0 = t1;
-    };
     MsmShape sh = msm_shape(n, Curve::FrP::BITS, sizeof(Pt), pre);
     if ((uint64_t)sh.nwin * n >= (1ull << 32)) return fail(c, B2S_ERR_INVALID_ARG, "msm: n * windows exceeds 2^32");
     if (pre && (uint64_t)pre->nwin * pre->stride >= (1ull << 31)) return fail(c, B2S_ERR_INVALID_ARG, "msm: precomputed table exceeds 2^31 points");
-    const RoundPlan rp = plan_rounds<F>(c, (uint64_t)sh.nwin * n, sh.G, is_g1, sh.L, true);   // digits of distinct scalars: random gathers
+    const RoundPlan rp = plan_rounds<F>(c, (uint64_t)sh.nwin * n, sh.G, is_g1, sh.L);
     sh.L = rp.L; sh.max_tasks = rp.max_tasks;
-    lap("plan_rounds");
-    const uint32_t MSM_SEG = env_u32("B2S_MSM_SEG", sh.B >= (1u << 16) ? 32u : 16u);
+    const uint32_t MSM_SEG = sh.B >= (1u << 16) ? 32u : 16u;
     const uint32_t ntiles = (sh.G + SCAN_TILE - 1) / SCAN_TILE;
     DevBuf ibuf, sorted, bucket_acc, segs, wins, tiles;
     B2S_TRY(tiles.alloc(c, (size_t)ntiles * sizeof(Scan3)));
@@ -838,11 +816,9 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
     if (pre) sh_red.nwin = 1;
     B2S_TRY(segs.alloc(c, (size_t)segs_per_win * sh_red.nwin * sizeof(Pt)));
     if (sh.nwin > 64) wins_ext = nullptr;   // caller scratch holds 64 window sums; tiny windows take the in-stream path
-    if (getenv("B2S_NO_AUX")) wins_ext = nullptr;   // debugging knob: keep the Horner tail on the main stream
     if (!wins_ext) B2S_TRY(wins.alloc(c, (size_t)sh.nwin * sizeof(Pt)));
     Pt* wins_p = wins_ext ? reinterpret_cast<Pt*>(wins_ext) : wins.as<Pt>();
 
-    lap("allocations");
     B2S_LAUNCH(c, msm_count_kernel<Fr>, cdiv(n, 256), 256, 0, scalars, n, mont, sh, counts);
     const uint32_t* no_perm = nullptr;
     B2S_LAUNCH(c, msm_scan_tiles_kernel, ntiles, SCAN_THREADS, 0, counts, no_perm, sh, tiles.as<Scan3>());
@@ -1116,15 +1092,15 @@ static int32_t msm_run_t(Ctx* c, const void* bases_dev, const void* scalars_dev,
     // step 3: heavy bucket sums (<= DEDUP_MAX buckets)
     B2S_CUDA(c, cudaMemsetAsync(hsums, 0, DEDUP_MAX * sizeof(Pt), c->stream));
     {
-        const RoundPlan rp = plan_rounds<F>(c, n_heavy, DEDUP_MAX, is_g1, (uint32_t)std::max<uint64_t>(64, n_heavy >> 18), false);   // lists in index order: the gathers stream
+        const RoundPlan rp = plan_rounds<F>(c, n_heavy, DEDUP_MAX, is_g1, (uint32_t)std::max<uint64_t>(64, n_heavy >> 18));
         B2S_TRY((bucket_sums_t<Curve, F>(c, bases, heavy_sorted.as<uint32_t>(), counts, offs, n_heavy, DEDUP_MAX, rp, hsums)));
     }
-    if (n_rest <= TINY_REST && !getenv("B2S_MSM_NO_TINY")) {
+    if (n_rest <= TINY_REST) {
         // steps 4 + 5 for a tiny rest: every product v * P (rest) and v_j * S_j (heavy) in its own warp, then one sum
         const uint32_t count = (uint32_t)n_rest + cd.k;
         Pt* const prods = prods_ring;
         // latency-bound (255 dependent doublings): inside a proof it goes to the aux stream, under the next MSM
-        const bool on_aux = wins_ext != nullptr && !getenv("B2S_NO_AUX");
+        const bool on_aux = wins_ext != nullptr;
         cudaStream_t ts = on_aux ? c->aux : c->stream;
         if (on_aux) {
             B2S_CUDA(c, cudaEventRecord(c->ev_tail, c->stream));

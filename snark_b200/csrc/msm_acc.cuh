@@ -5,17 +5,9 @@
 #include "common.cuh"
 #include "ec_team.cuh"
 
-#ifndef B2S_G2_MIN_BLOCKS
-#define B2S_G2_MIN_BLOCKS 1   // CTAs/SM the G2 accumulate kernel is compiled for (register cap = 65536 / (128 * this))
-#endif
-#ifndef B2S_MADD_BYVALUE
-#define B2S_MADD_BYVALUE 1
-#endif
-
 namespace b2s {
 
 static constexpr int MSM_ACC_THREADS = 128;
-static constexpr int MSM_SEG = 16;          // buckets per thread in the bucket-sum kernel
 static constexpr int MSM_RED_THREADS = 128;
 
 struct MsmShape {
@@ -75,8 +67,7 @@ __device__ __forceinline__ void madd(XYZZ<F>& acc, const Affine<F>& q) {
     F r = q.y * acc.zzz - acc.y;
     if (p.is_zero()) {
         if (sizeof(F) > 64) madd_rare_ref(acc, q, r.is_zero());
-        else if (B2S_MADD_BYVALUE) acc = madd_rare<F>(q, r.is_zero());
-        else madd_rare_ref(acc, q, r.is_zero());
+        else acc = madd_rare<F>(q, r.is_zero());
         return;
     }
     F pp = p.sqr();
@@ -91,7 +82,7 @@ __device__ __forceinline__ void madd(XYZZ<F>& acc, const Affine<F>& q) {
 
 // One thread per task.  Task t belongs to bucket g = upper_bound(task_off, t) - 1.
 template <class F>
-__global__ void __launch_bounds__(MSM_ACC_THREADS, (sizeof(F) > 64 ? B2S_G2_MIN_BLOCKS : 1))
+__global__ void __launch_bounds__(MSM_ACC_THREADS, 1)
 msm_accumulate_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __restrict__ sorted,
                       const uint32_t* __restrict__ offsets, const uint32_t* __restrict__ task_off,
                       const uint32_t* __restrict__ perm, MsmShape sh, XYZZ<F>* __restrict__ bucket_acc,

@@ -39,10 +39,7 @@ enum : uint32_t { BA_F_VALID = 1u, BA_F_SINGLE = 2u };
 
 static constexpr uint32_t BA_KMIN = 16, BA_KMAX = 256;   // rows per unit (chosen on the device from the round's size)
 static constexpr uint32_t BA_K2 = 32;                     // lane totals per Fermat inversion
-#ifndef B2S_BA_P1_STAGES
-#define B2S_BA_P1_STAGES 3
-#endif
-static constexpr uint32_t BA_P1_STAGES = B2S_BA_P1_STAGES, BA_P2_STAGES = 2;
+static constexpr uint32_t BA_P1_STAGES = 3, BA_P2_STAGES = 2;
 
 __host__ __device__ constexpr uint32_t ba_slot_bytes(uint32_t n) { return ((((n + 15u) / 16u) | 1u)) * 16u; }
 
@@ -51,9 +48,6 @@ struct BaGeom {
     static constexpr uint32_t FE = sizeof(F), PT = sizeof(Affine<F>);
     static constexpr uint32_t THREADS_ = sizeof(F) > 64 ? 64 : 128;
     static constexpr uint32_t P1_META = 2 * FE, P1_SLOT = ba_slot_bytes(2 * FE + 16);
-    // staged first round (gathers are random): pass 1 fetches the whole points once and writes the pairs out in order
-    static constexpr uint32_t P1S_META = 2 * PT, P1S_SLOT = ba_slot_bytes(2 * PT + 16);
-    static constexpr uint32_t P1S_SMEM = THREADS_ * BA_P1_STAGES * P1S_SLOT;
     // pass 2 stages the two points only; the prefix product travels through registers (one row ahead) so that the slot
     // ring of 16 warps fits an SM: occupancy is what hides the dependent-issue latency of the carry chains
     static constexpr uint32_t P2_META = 2 * PT, P2_SLOT = ba_slot_bytes(2 * PT + 16);
@@ -191,12 +185,11 @@ __device__ __forceinline__ Affine<F> ba_output(const Affine<F>& p1, const Affine
 
 // descriptor of (row q, this lane): where its inputs are
 struct BaDesc { uint32_t in0, flags; };
-// dense: the inputs were written as one PAIR per output (staged first round), so output o reads positions 2 o, 2 o + 1
-__device__ __forceinline__ BaDesc ba_desc(uint32_t word, uint32_t wr, uint32_t q, uint32_t lane, uint32_t t_out, uint32_t dense = 0) {
+__device__ __forceinline__ BaDesc ba_desc(uint32_t word, uint32_t wr, uint32_t q, uint32_t lane, uint32_t t_out) {
     const uint32_t o = q * 32u + lane;
     BaDesc d;
     d.flags = (o < t_out ? BA_F_VALID : 0u) | (((word >> lane) & 1u) ? BA_F_SINGLE : 0u);
-    d.in0 = 2u * o - (dense ? 0u : wr + __popc(word & ((1u << lane) - 1u)));
+    d.in0 = 2u * o - (wr + __popc(word & ((1u << lane) - 1u)));
     return d;
 }
 
@@ -224,20 +217,13 @@ __device__ __noinline__ F ba_slow_denominator(const Affine<F>* __restrict__ base
 // Software pipeline per lane, time step t:  consume row t-S | issue the copies of row t into the slot just freed |
 // descriptor + sorted indices of row t+1 | bitmap word of row t+2.  A row's operands are in flight during the S-1
 // row computations before its own.
-// STAGE (first round only): the lane fetches both whole points (one random access each instead of one here and one in
-// pass 2), and writes the pair -- y already negated where the digit was negative -- to staged[2 o], staged[2 o + 1]; pass 2
-// then streams.
-template <class F, bool FIRST, bool STAGE = false>
+template <class F, bool FIRST>
 __global__ void __launch_bounds__(BaGeom<F>::THREADS)
 msm_ba_p1_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __restrict__ sorted, const Affine<F>* __restrict__ prev,
                  const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ wrank, const uint32_t* __restrict__ t_out_p,
-                 uint32_t target_units, uint32_t* __restrict__ unit_ctr, F* __restrict__ prefix, F* __restrict__ tot,
-                 Affine<F>* __restrict__ staged) {
+                 uint32_t target_units, uint32_t* __restrict__ unit_ctr, F* __restrict__ prefix, F* __restrict__ tot) {
     using Gm = BaGeom<F>;
-    constexpr uint32_t S = BA_P1_STAGES, FE = Gm::FE, PT = Gm::PT;
-    constexpr uint32_t SLOT = STAGE ? Gm::P1S_SLOT : Gm::P1_SLOT, META = STAGE ? Gm::P1S_META : Gm::P1_META;
-    constexpr uint32_t X2 = STAGE ? PT : FE;      // where the second point's x sits in the slot
-    static_assert(!STAGE || FIRST, "staging is for the gathered first round");
+    constexpr uint32_t S = BA_P1_STAGES, FE = Gm::FE, SLOT = Gm::P1_SLOT, META = Gm::P1_META;
     extern __shared__ uint4 ba_smem[];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(ba_smem) + (warp * S * 32u + lane) * SLOT;
@@ -263,20 +249,10 @@ msm_ba_p1_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __restrict
                     const uint32_t o = (q0 + i) * 32u + lane;
                     F d = F::one();                              // no partner: the output is a copy
                     if (!single) {
-                        const F x1 = lds_struct<F>(slot), x2 = lds_struct<F>(slot + X2);
+                        const F x1 = lds_struct<F>(slot), x2 = lds_struct<F>(slot + FE);
                         // x = 0 may be the (0,0) encoding of infinity, equal x means doubling or cancellation
                         if (!x1.is_zero() && !x2.is_zero() && x1 != x2) d = x2 - x1;
                         else d = ba_slow_denominator<F, FIRST>(bases, prev, meta.x, meta.y, meta.z, false);
-                    }
-                    if (STAGE) {
-                        Affine<F> p = lds_struct<Affine<F>>(slot);
-                        if (meta.x >> 31) p.y = p.y.neg();
-                        st_struct(staged + 2 * (size_t)o, p);
-                        if (!single) {
-                            p = lds_struct<Affine<F>>(slot + PT);
-                            if (meta.y >> 31) p.y = p.y.neg();
-                            st_struct(staged + 2 * (size_t)o + 1, p);
-                        }
                     }
                     st_struct(prefix + o, prod);
                     prod = prod * d;
@@ -287,10 +263,10 @@ msm_ba_p1_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __restrict
                 const uint32_t slot = smem0 + ((uint32_t)t % S) * 32u * SLOT;
                 if (b_d.flags & BA_F_VALID) {
                     const F* px1 = FIRST ? &bases[b_e1 & 0x7fffffffu].x : &prev[b_d.in0].x;
-                    cp_async_bytes<STAGE ? PT : FE>(slot, px1);
+                    cp_async_bytes<FE>(slot, px1);
                     if (!(b_d.flags & BA_F_SINGLE)) {
                         const F* px2 = FIRST ? &bases[b_e2 & 0x7fffffffu].x : &prev[b_d.in0 + 1].x;
-                        cp_async_bytes<STAGE ? PT : FE>(slot + X2, px2);
+                        cp_async_bytes<FE>(slot + FE, px2);
                     }
                 }
                 sts16(slot + META, make_uint4(b_e1, b_e2, b_d.in0, b_d.flags));
@@ -356,9 +332,9 @@ __global__ void __launch_bounds__(BaGeom<F>::THREADS, BaGeom<F>::P2_MIN_CTAS)
 msm_ba_p2_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __restrict__ sorted, const Affine<F>* __restrict__ prev,
                  const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ wrank, const uint32_t* __restrict__ t_out_p,
                  uint32_t target_units, uint32_t* __restrict__ unit_ctr, const F* __restrict__ prefix, const F* __restrict__ tot_inv,
-                 Affine<F>* __restrict__ out, uint32_t dense) {
+                 Affine<F>* __restrict__ out) {
     using Gm = BaGeom<F>;
-    constexpr uint32_t S = BA_P2_STAGES, FE = Gm::FE, PT = Gm::PT;
+    constexpr uint32_t S = BA_P2_STAGES, PT = Gm::PT;
     extern __shared__ uint4 ba_smem[];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     const uint32_t smem0 = (uint32_t)__cvta_generic_to_shared(ba_smem) + (warp * S * 32u + lane) * Gm::P2_SLOT;
@@ -417,7 +393,7 @@ msm_ba_p2_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __restrict
             }
             cp_async_commit();
             if (t + 1 >= 0 && (uint32_t)(t + 1) < nr) {
-                b_d = ba_desc(a_word, a_wr, q0 + nr - 1 - (uint32_t)(t + 1), lane, t_out, dense);
+                b_d = ba_desc(a_word, a_wr, q0 + nr - 1 - (uint32_t)(t + 1), lane, t_out);
                 if (FIRST && (b_d.flags & BA_F_VALID)) {
                     b_e1 = sorted[b_d.in0];
                     b_e2 = (b_d.flags & BA_F_SINGLE) ? 0u : sorted[b_d.in0 + 1];
@@ -440,7 +416,7 @@ template <class F>
 __global__ void __launch_bounds__(BaGeom<F>::THREADS, BaGeom<F>::P2_MIN_CTAS)
 msm_ba_p2_bulk_kernel(const Affine<F>* __restrict__ prev, const uint32_t* __restrict__ bitmap, const uint32_t* __restrict__ wrank,
                       const uint32_t* __restrict__ t_out_p, uint32_t target_units, uint32_t* __restrict__ unit_ctr, const F* __restrict__ prefix,
-                      const F* __restrict__ tot_inv, Affine<F>* __restrict__ out, uint32_t dense) {
+                      const F* __restrict__ tot_inv, Affine<F>* __restrict__ out) {
     using Gm = BaGeom<F>;
     constexpr uint32_t S = BA_P2_STAGES, PT = Gm::PT;
     static_assert(S == 2, "parity bookkeeping below is written for two stages");
@@ -504,7 +480,7 @@ msm_ba_p2_bulk_kernel(const Affine<F>* __restrict__ prev, const uint32_t* __rest
                     bulk_g2s(st, prev + first_in, bytes, st + Gm::P2B_MBAR);
                 }
             }
-            if (t + 1 >= 0 && (uint32_t)(t + 1) < nr) b_d = ba_desc(a_word, a_wr, q0 + nr - 1 - (uint32_t)(t + 1), lane, t_out, dense);
+            if (t + 1 >= 0 && (uint32_t)(t + 1) < nr) b_d = ba_desc(a_word, a_wr, q0 + nr - 1 - (uint32_t)(t + 1), lane, t_out);
             if ((uint32_t)(t + 2) < nr) {
                 a_word = bitmap[q0 + nr - 1 - (uint32_t)(t + 2)];
                 a_wr = wrank[q0 + nr - 1 - (uint32_t)(t + 2)];
@@ -616,7 +592,6 @@ struct BaRoundArgs {
     void* tot;                    // F[lane totals bound]
     void* inv_scratch;            // F[lane totals bound]
     void* out;                    // Affine<F>[t_out bound]
-    void* staged;                 // first round only, optional: Affine<F>[2 * t_out bound] -- gather once, then stream
 };
 int32_t msm_ba_round_g1(Ctx* c, const BaRoundArgs& a);
 int32_t msm_ba_round_g2(Ctx* c, const BaRoundArgs& a);
@@ -631,45 +606,31 @@ static int32_t msm_ba_round_launch(Ctx* c, const char* l1, const char* li, const
     // persistent grids: four CTAs per SM for pass 2 (16 warps; register- and shared-memory-bound there), up to five for pass 1
     const unsigned ctas = 4u * (unsigned)c->sm_count;
     auto fit = [&](uint32_t smem) { return (unsigned)c->sm_count * std::max(1u, std::min(5u, (224u * 1024u) / (smem + 1024u))); };
-    Affine<F>* staged = reinterpret_cast<Affine<F>*>(a.staged);
     Affine<F>* out = reinterpret_cast<Affine<F>*>(a.out);
-    const bool stage = a.first && staged != nullptr;
-    if (stage) {
-        B2S_SMEM_ATTR(c, (msm_ba_p1_kernel<F, true, true>), Gm::P1S_SMEM);
-        B2S_LAUNCH_N(c, l1, (msm_ba_p1_kernel<F, true, true>), fit(Gm::P1S_SMEM), Gm::THREADS, Gm::P1S_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank,
-                     a.t_out, a.target_units, a.unit_ctr, prefix, tot, staged);
-    } else if (a.first) {
-        B2S_SMEM_ATTR(c, (msm_ba_p1_kernel<F, true, false>), Gm::P1_SMEM);
-        B2S_LAUNCH_N(c, l1, (msm_ba_p1_kernel<F, true, false>), fit(Gm::P1_SMEM), Gm::THREADS, Gm::P1_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank,
-                     a.t_out, a.target_units, a.unit_ctr, prefix, tot, staged);
+    if (a.first) {
+        B2S_SMEM_ATTR(c, (msm_ba_p1_kernel<F, true>), Gm::P1_SMEM);
+        B2S_LAUNCH_N(c, l1, (msm_ba_p1_kernel<F, true>), fit(Gm::P1_SMEM), Gm::THREADS, Gm::P1_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank,
+                     a.t_out, a.target_units, a.unit_ctr, prefix, tot);
     } else {
-        B2S_SMEM_ATTR(c, (msm_ba_p1_kernel<F, false, false>), Gm::P1_SMEM);
-        B2S_LAUNCH_N(c, l1, (msm_ba_p1_kernel<F, false, false>), fit(Gm::P1_SMEM), Gm::THREADS, Gm::P1_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank,
-                     a.t_out, a.target_units, a.unit_ctr, prefix, tot, staged);
+        B2S_SMEM_ATTR(c, (msm_ba_p1_kernel<F, false>), Gm::P1_SMEM);
+        B2S_LAUNCH_N(c, l1, (msm_ba_p1_kernel<F, false>), fit(Gm::P1_SMEM), Gm::THREADS, Gm::P1_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank,
+                     a.t_out, a.target_units, a.unit_ctr, prefix, tot);
     }
     B2S_LAUNCH_N(c, li, msm_ba_inv_kernel<F>, 4 * c->sm_count, 128, 0, tot, a.t_out, a.target_units, reinterpret_cast<F*>(a.inv_scratch));
-    if (a.first && !stage) {
+    if (a.first) {
         B2S_SMEM_ATTR(c, (msm_ba_p2_kernel<F, true>), Gm::P2_SMEM);
         B2S_LAUNCH_N(c, l2, (msm_ba_p2_kernel<F, true>), ctas, Gm::THREADS, Gm::P2_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank, a.t_out,
-                     a.target_units, a.unit_ctr + 1, (const F*)prefix, (const F*)tot, out, 0u);
+                     a.target_units, a.unit_ctr + 1, (const F*)prefix, (const F*)tot, out);
+    } else if (sizeof(F) <= 64) {
+        // later rounds read the previous round's output, where a row's inputs are contiguous: bulk copies for G1, the per-lane
+        // cp.async ring for G2 (pass 2, 2^24 uniform points, H100 80GB HBM3 at 400 W: G1 67.0 vs 69.8 ms, G2 215.6 vs 217.0 ms)
+        B2S_SMEM_ATTR(c, msm_ba_p2_bulk_kernel<F>, Gm::P2B_SMEM);
+        B2S_LAUNCH_N(c, l2, msm_ba_p2_bulk_kernel<F>, ctas, Gm::THREADS, Gm::P2B_SMEM, prev, a.bitmap, a.wrank, a.t_out, a.target_units, a.unit_ctr + 1,
+                     (const F*)prefix, (const F*)tot, out);
     } else {
-        // later rounds read the previous round's output; a staged first round reads its own pairs, two per output.  Rows are
-        // contiguous there: bulk copies (B2S_MSM_BULK=0 falls back to the per-lane cp.async ring, same results)
-        const Affine<F>* src = stage ? (const Affine<F>*)staged : prev;
-        // measured with tools/msm_probe.py (2^24 uniform points, H100 80GB HBM3 at a 400 W limit): G1 pass 2 67.0 ms with bulk
-        // copies vs 69.8 ms with the cp.async ring; G2 pass 2 215.6 vs 217.0 ms, within noise (a lane's two 192-byte points at a
-        // 384-byte stride conflict in shared memory) -- default: bulk for G1, ring for G2
-        const char* bulk_env = getenv("B2S_MSM_BULK");
-        const bool use_bulk = bulk_env ? bulk_env[0] != '0' : sizeof(F) <= 64;
-        if (use_bulk) {
-            B2S_SMEM_ATTR(c, msm_ba_p2_bulk_kernel<F>, Gm::P2B_SMEM);
-            B2S_LAUNCH_N(c, l2, msm_ba_p2_bulk_kernel<F>, ctas, Gm::THREADS, Gm::P2B_SMEM, src, a.bitmap, a.wrank, a.t_out, a.target_units, a.unit_ctr + 1,
-                         (const F*)prefix, (const F*)tot, out, stage ? 1u : 0u);
-        } else {
-            B2S_SMEM_ATTR(c, (msm_ba_p2_kernel<F, false>), Gm::P2_SMEM);
-            B2S_LAUNCH_N(c, l2, (msm_ba_p2_kernel<F, false>), ctas, Gm::THREADS, Gm::P2_SMEM, bases, a.sorted, src, a.bitmap, a.wrank, a.t_out,
-                         a.target_units, a.unit_ctr + 1, (const F*)prefix, (const F*)tot, out, stage ? 1u : 0u);
-        }
+        B2S_SMEM_ATTR(c, (msm_ba_p2_kernel<F, false>), Gm::P2_SMEM);
+        B2S_LAUNCH_N(c, l2, (msm_ba_p2_kernel<F, false>), ctas, Gm::THREADS, Gm::P2_SMEM, bases, a.sorted, prev, a.bitmap, a.wrank, a.t_out,
+                     a.target_units, a.unit_ctr + 1, (const F*)prefix, (const F*)tot, out);
     }
     return B2S_OK;
 }
