@@ -299,13 +299,30 @@ int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
  *                    share `mem`; host batches go through bounded device scratch in chunks, so n_proofs is not limited by
  *                    device memory.  n_inputs + 1 != n_gamma_abc -> B2S_ERR_MALFORMED_VK (ark's prepare_inputs error);
  *                    n_proofs == 0 -> B2S_OK.  Points are assumed valid, as in ark: decode untrusted bytes with validate = 1.
- *   b2s_pairing      Pairing::pairing, element-wise: out[i] = e(P_i, Q_i), i < n; a pair with P or Q at infinity (all-zero)
+ *   b2s_groth16_verify_batch_rlc  one verdict for the whole batch (bellman's groth16::batch, Zcash's batch verifier): with
+ *                    caller-drawn 128-bit rho_i,
+ *                      prod_i e(rho_i A_i, B_i) * e(IC*, -gamma) * e(C*, -delta) == e(alpha, beta)^S,
+ *                    S = sum_i rho_i, C* = sum_i rho_i C_i, IC* = S gamma_abc[0] + sum_j (sum_i rho_i x_ij) gamma_abc[j+1]
+ *                    (mod r).  One Miller loop over one pair per proof, one G1 MSM for the C terms and one final
+ *                    exponentiation for the batch.  *ok = 1 when every proof is accepted.  If a proof is invalid, the batch
+ *                    is accepted with probability <= 2^-128, provided (1) the rho_i are unpredictable to whoever made the
+ *                    proofs: draw them from a CSPRNG for each call, and (2) every point lies in its prime-order subgroup:
+ *                    decode untrusted bytes with validate = 1.  rho: n_proofs x 16 bytes, little-endian 128-bit integers,
+ *                    in `mem` like inputs, a, b, c (same layouts as b2s_groth16_verify_batch); ok: one byte, always HOST,
+ *                    always written.  A zero rho_i would leave proof i unchecked: B2S_ERR_INVALID_ARG, b2s_last_error names
+ *                    the lowest such index.  Another curve's key or a null buffer -> B2S_ERR_INVALID_ARG;
+ *                    n_inputs + 1 != n_gamma_abc -> B2S_ERR_MALFORMED_VK; n_proofs == 0 -> B2S_OK with *ok = 1.  To learn
+ *                    which proofs of a rejected batch failed, run b2s_groth16_verify_batch on it.
+ *   b2s_pairing     Pairing::pairing, element-wise: out[i] = e(P_i, Q_i), i < n; a pair with P or Q at infinity (all-zero)
  *                    gives 1.  All buffers share `mem`. */
 int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,
                        const void* gamma_abc_g1, uint64_t n_gamma_abc, b2s_pvk** out);
 void b2s_pvk_free(b2s_ctx* ctx, b2s_pvk* pvk);
 int32_t b2s_groth16_verify_batch(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
                                  const void* a_g1, const void* b_g2, const void* c_g1, int32_t mem, uint8_t* ok);
+int32_t b2s_groth16_verify_batch_rlc(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                     const void* a_g1, const void* b_g2, const void* c_g1, const void* rho, int32_t mem,
+                                     uint8_t* ok);
 int32_t b2s_pairing(b2s_ctx* ctx, const void* p_g1, const void* q_g2, uint64_t n, int32_t mem, void* out_gt);
 
 /* ---- setup helper (SURVEY 8(f) row 2): fixed-base batch multiplication -------------------------

@@ -71,6 +71,9 @@ extern "C" {
     pub fn b2s_pvk_free(ctx: *mut B2sCtx, pvk: *mut B2sPvk);
     pub fn b2s_groth16_verify_batch(ctx: *mut B2sCtx, pvk: *const B2sPvk, n_proofs: u64, inputs: *const c_void, n_inputs: u64,
                                     a_g1: *const c_void, b_g2: *const c_void, c_g1: *const c_void, mem: i32, ok: *mut u8) -> i32;
+    pub fn b2s_groth16_verify_batch_rlc(ctx: *mut B2sCtx, pvk: *const B2sPvk, n_proofs: u64, inputs: *const c_void, n_inputs: u64,
+                                        a_g1: *const c_void, b_g2: *const c_void, c_g1: *const c_void, rho: *const c_void, mem: i32,
+                                        ok: *mut u8) -> i32;
     pub fn b2s_pairing(ctx: *mut B2sCtx, p_g1: *const c_void, q_g2: *const c_void, n: u64, mem: i32, out_gt: *mut c_void) -> i32;
     // universal-setup schemes (UniversalSetupSNARK, snark/src/lib.rs:107-133): the seams a polynomial-commitment /
     // evaluation-domain backend binds (INTEGRATION.md section 8).  mem: 0 host, 1 device; s, c, z: one Montgomery Fr on the host
@@ -240,6 +243,49 @@ impl<E: Pairing> Groth16B200<E> {
             unsafe { b2s_pvk_free(ctx, pvk) };
             check(ctx, st)?;
             Ok(ok.into_iter().map(|v| v != 0).collect())
+        };
+        let out = run();
+        unsafe { b2s_ctx_destroy(ctx) };
+        out
+    }
+
+    /// One verdict for the whole batch: `true` when every proof is accepted, by a random linear combination of the
+    /// proofs with nonzero 128-bit weights drawn from `rng` (bellman's `batch::Verifier::verify(rng, ..)`).  One Miller
+    /// loop over one pair per proof, one MSM for the C terms and one final exponentiation for the batch.  A batch with an
+    /// invalid proof passes with probability at most 2^-128 if `rng` is unpredictable to whoever made the proofs and
+    /// every point lies in its prime-order subgroup (decode untrusted proofs with validation).  On `false`,
+    /// `verify_batch` tells which proofs failed.
+    pub fn verify_all<R: RngCore + CryptoRng>(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>], proofs: &[Proof<E>], rng: &mut R)
+        -> Result<bool, B200Error> {
+        if inputs.len() != proofs.len() { return Err(SynthesisError::AssignmentMissing.into()); }
+        let ni = vk.gamma_abc_g1.len().saturating_sub(1);
+        if inputs.iter().any(|x| x.len() != ni) { return Err(SynthesisError::MalformedVerifyingKey.into()); }
+        let mut rho = vec![0u8; 16 * proofs.len()];
+        for w in rho.chunks_mut(16) {
+            while w.iter().all(|b| *b == 0) { rng.fill_bytes(w); }
+        }
+        let curve_id = if core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>() == 48 { 0 } else { 1 };
+        let mut ctx: *mut B2sCtx = core::ptr::null_mut();
+        check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
+        let run = || -> Result<bool, B200Error> {
+            let (alpha, beta, gamma, delta) = (pack_points(&[vk.alpha_g1]), pack_points(&[vk.beta_g2]), pack_points(&[vk.gamma_g2]),
+                                               pack_points(&[vk.delta_g2]));
+            let abc = pack_points(&vk.gamma_abc_g1);
+            let mut pvk: *mut B2sPvk = core::ptr::null_mut();
+            check(ctx, unsafe { b2s_vk_prepare(ctx, alpha.as_ptr().cast(), beta.as_ptr().cast(), gamma.as_ptr().cast(),
+                                               delta.as_ptr().cast(), abc.as_ptr().cast(), vk.gamma_abc_g1.len() as u64, &mut pvk) })?;
+            let x: Vec<E::ScalarField> = inputs.iter().flat_map(|v| v.iter().copied()).collect();
+            let a = pack_points(&proofs.iter().map(|p| p.a).collect::<Vec<_>>());
+            let b = pack_points(&proofs.iter().map(|p| p.b).collect::<Vec<_>>());
+            let c = pack_points(&proofs.iter().map(|p| p.c).collect::<Vec<_>>());
+            let mut ok = 0u8;
+            let st = unsafe { b2s_groth16_verify_batch_rlc(ctx, pvk, proofs.len() as u64,
+                                                           if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
+                                                           a.as_ptr().cast(), b.as_ptr().cast(), c.as_ptr().cast(), rho.as_ptr().cast(),
+                                                           0 /* B2S_MEM_HOST */, &mut ok) };
+            unsafe { b2s_pvk_free(ctx, pvk) };
+            check(ctx, st)?;
+            Ok(ok != 0)
         };
         let out = run();
         unsafe { b2s_ctx_destroy(ctx) };

@@ -41,6 +41,9 @@ void pvk_free(b2s_pvk* pvk);
 int32_t groth16_verify_batch(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const void* a, const void* b,
                              const void* cc, int32_t mem, uint8_t* ok);
 int32_t pairing_batch(Ctx* c, const void* p, const void* q, uint64_t n, int32_t mem, void* out);
+// verify_rlc.cu
+int32_t groth16_verify_batch_rlc(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const void* a, const void* b,
+                                 const void* cc, const void* rho, int32_t mem, uint8_t* ok);
 }  // namespace b2s
 
 #define LOCK(ctx)                                      \
@@ -610,6 +613,12 @@ int32_t b2s_groth16_verify_batch(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_pr
     LOCK(ctx);
     if (!pvk) return fail(ctx, B2S_ERR_INVALID_ARG, "verify_batch: null prepared key");
     return groth16_verify_batch(ctx, pvk, n_proofs, inputs, n_inputs, a_g1, b_g2, c_g1, mem, ok);
+}
+int32_t b2s_groth16_verify_batch_rlc(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                     const void* a_g1, const void* b_g2, const void* c_g1, const void* rho, int32_t mem, uint8_t* ok) {
+    LOCK(ctx);
+    if (!pvk) return fail(ctx, B2S_ERR_INVALID_ARG, "verify_batch_rlc: null prepared key");
+    return groth16_verify_batch_rlc(ctx, pvk, n_proofs, inputs, n_inputs, a_g1, b_g2, c_g1, rho, mem, ok);
 }
 int32_t b2s_pairing(b2s_ctx* ctx, const void* p_g1, const void* q_g2, uint64_t n, int32_t mem, void* out_gt) {
     LOCK(ctx);

@@ -208,6 +208,22 @@ B2S_PAIR_NOINLINE Fp12<P> cyclotomic_exp_x(const Fp12<P>& f) {
     }
     return P::X_NEG ? acc.conj() : acc;
 }
+// f^e in the cyclotomic subgroup, e = sum_i words[i] 2^(32 i) (little-endian, not Montgomery); e = 0 gives 1
+template <class P>
+B2S_PAIR_NOINLINE Fp12<P> cyclotomic_exp(const Fp12<P>& f, const uint32_t* words, int nwords) {
+    Fp12<P> acc = Fp12<P>::one();
+    bool started = false;
+    for (int w = nwords - 1; w >= 0; w--) {
+        for (int b = 31; b >= 0; b--) {
+            if (started) acc = fp12_cyclotomic_sqr(acc);
+            if ((words[w] >> b) & 1) {
+                acc = started ? fp12_mul(acc, f) : f;
+                started = true;
+            }
+        }
+    }
+    return acc;
+}
 
 // ---- lines ---------------------------------------------------------------------------------------------------------
 template <class P>
@@ -435,6 +451,34 @@ B2S_HD bool groth16_verdict(const Affine<Fp<typename Curve::FqP>>& a, const Affi
                             const G2Prepared<Curve>* neg_gamma, const G2Prepared<Curve>* neg_delta,
                             const Fp12<typename Curve::FqP>& alpha_beta) {
     return final_exponentiation(groth16_miller<Curve>(a, b, ic, c, neg_gamma, neg_delta)) == alpha_beta;
+}
+
+// The random-linear-combination check of many proofs under one key (verify_rlc.cu), with caller-drawn nonzero 128-bit
+// rho_i:
+//   prod_i e(rho_i A_i, B_i) * e(IC*, -gamma) * e(C*, -delta) == e(alpha, beta)^S,
+//   S = sum_i rho_i,  C* = sum_i rho_i C_i,  IC* = S gamma_abc[0] + sum_j (sum_i rho_i x_ij) gamma_abc[j+1]  (mod r).
+// It holds for valid proofs because every factor goes through the same final exponentiation.  If a proof is invalid, at
+// most one rho_i < 2^128 < r (the others fixed) passes, since GT has prime order r.
+//
+// One thread's share of the left side: prod_j f_{rho_j A_j, B_j}, NF proofs, rho as 4 little-endian words per proof.
+// rho_j A_j is made affine with one Fq inversion.  Pairs with A or B at infinity (the padding of a last partial group)
+// contribute 1.  Not yet final-exponentiated.
+template <class Curve, int NF>
+B2S_PAIR_NOINLINE Fp12<typename Curve::FqP> rlc_miller(const Affine<Fp<typename Curve::FqP>>* a,
+                                                      const Affine<Fp2<typename Curve::FqP>>* b, const uint32_t* rho) {
+    Affine<Fp<typename Curve::FqP>> p[NF];
+    for (int i = 0; i < NF; i++) p[i] = scalar_mul_words(Curve::G1::from_affine(a[i]), rho + 4 * i, 4).to_affine();
+    return multi_miller_loop<Curve, NF, 0>(p, b, nullptr, nullptr);
+}
+// The verdict: f = the product of every rlc_miller value, ic = IC*, c = C* (affine), s = S (8 canonical words)
+template <class Curve>
+B2S_PAIR_NOINLINE bool rlc_verdict(const Fp12<typename Curve::FqP>& f, const Affine<Fp<typename Curve::FqP>>& ic,
+                                   const Affine<Fp<typename Curve::FqP>>& c, const G2Prepared<Curve>* neg_gamma,
+                                   const G2Prepared<Curve>* neg_delta, const Fp12<typename Curve::FqP>& alpha_beta, const uint32_t* s) {
+    const Affine<Fp<typename Curve::FqP>> pp[2] = {ic, c};
+    const G2Prepared<Curve>* prep[2] = {neg_gamma, neg_delta};
+    const Fp12<typename Curve::FqP> g = fp12_mul(f, multi_miller_loop<Curve, 0, 2>(nullptr, nullptr, pp, prep));
+    return final_exponentiation(g) == cyclotomic_exp(alpha_beta, s, 8);
 }
 
 }  // namespace b2s

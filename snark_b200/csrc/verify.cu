@@ -11,23 +11,7 @@
 
 #include "common.cuh"
 #include "pairing.cuh"
-
-namespace b2s {
-
-// Public-input sum: per base g_j a table of [d 2^(8 w)] g_j, d = 1..255, w < 32 (affine), so a scalar costs at most 32
-// mixed additions.  Memory per public input: 32 * 255 affine G1 points = 765 KiB (BLS12-381) / 510 KiB (BN254).
-constexpr int IC_WBITS = 8, IC_WINDOWS = 32, IC_DIGITS = (1 << IC_WBITS) - 1;
-
-}  // namespace b2s
-
-struct b2s_pvk {
-    int curve = 0;
-    uint64_t n_abc = 0;
-    b2s::DevBuf prep;    // G2Prepared[2]: -gamma, -delta
-    b2s::DevBuf ab;      // e(alpha, beta) in GT
-    b2s::DevBuf abc0;    // gamma_abc[0]
-    b2s::DevBuf table;   // (n_abc - 1) x IC_WINDOWS x IC_DIGITS affine G1
-};
+#include "verify.cuh"
 
 namespace b2s {
 
@@ -96,8 +80,6 @@ __global__ void final_exp_kernel(const Fp12<typename Curve::FqP>* f, uint32_t n,
     else out[i] = r;
 }
 
-constexpr int VERIFY_THREADS = 128;
-
 int32_t vk_prepare(Ctx* c, const void* alpha, const void* beta, const void* gamma, const void* delta, const void* abc, uint64_t n_abc,
                    b2s_pvk** out) {
     if (n_abc == 0) return fail(c, B2S_ERR_MALFORMED_VK, "vk_prepare: gamma_abc_g1 is empty");
@@ -139,12 +121,6 @@ int32_t vk_prepare(Ctx* c, const void* alpha, const void* beta, const void* gamm
     if (st != B2S_OK) { delete pvk; return st; }
     *out = pvk;
     return B2S_OK;
-}
-
-// Device scratch for one chunk: host buffers are copied in, device buffers are used in place.
-static uint64_t chunk_size(uint64_t n, size_t per_proof) {
-    constexpr uint64_t MAX_CHUNK = 1u << 18, SCRATCH = 1ull << 30;
-    return std::max<uint64_t>(1, std::min<uint64_t>({n, MAX_CHUNK, SCRATCH / per_proof}));
 }
 
 int32_t groth16_verify_batch(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const void* a, const void* b,

@@ -2,6 +2,7 @@
 interfaces each entry point replaces)."""
 import ctypes
 import os
+import secrets
 from ctypes import POINTER, c_char_p, c_int32, c_uint32, c_uint64, c_void_p
 
 import numpy as np
@@ -93,6 +94,8 @@ SIGNATURES = {
     "b2s_pvk_free": (None, [c_void_p, c_void_p]),
     "b2s_groth16_verify_batch": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_int32,
                                            c_void_p]),
+    "b2s_groth16_verify_batch_rlc": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p,
+                                               c_void_p, c_int32, POINTER(ctypes.c_uint8)]),
     "b2s_pairing": (c_int32, [c_void_p, c_void_p, c_void_p, c_uint64, c_int32, c_void_p]),
     "b2s_fixed_base_g1": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
     "b2s_fixed_base_g2": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
@@ -126,6 +129,17 @@ def load_library():
             fn.argtypes = args
         _lib = lib
     return _lib
+
+
+def random_rho(n):
+    """n nonzero 128-bit integers from the OS CSPRNG, as n x 4 little-endian uint32 words (the rho of
+    b2s_groth16_verify_batch_rlc)"""
+    w = np.frombuffer(secrets.token_bytes(16 * n), dtype=np.uint32).reshape(n, 4).copy()
+    zero = ~w.any(axis=1)
+    while zero.any():
+        w[zero] = np.frombuffer(secrets.token_bytes(16 * int(zero.sum())), dtype=np.uint32).reshape(-1, 4)
+        zero = ~w.any(axis=1)
+    return w.reshape(-1)
 
 
 def _ptr(x):
@@ -425,6 +439,29 @@ class Backend:
         po, _ = _ptr(ok)
         self._ck(self.lib.b2s_groth16_verify_batch(self.h, pvk, n_proofs, px, n_inputs, pa, pb, pc, mem, po))
         return ok
+
+    def groth16_verify_all(self, pvk, inputs, n_inputs, a, b, c, rho=None, n_proofs=None):
+        """True when every proof is accepted, by one random linear combination of the batch (b2s_groth16_verify_batch_rlc).
+        Buffers as for groth16_verify_batch.  rho: n_proofs x 4 uint32 words (little-endian 128-bit, nonzero) in the same
+        memory as the proofs; None draws them with `secrets`.  On False, groth16_verify_batch tells which proofs failed."""
+        pa, mem = _ptr(a)
+        pb, mem_b = _ptr(b)
+        pc, mem_c = _ptr(c)
+        px, mem_x = _ptr(inputs)
+        assert mem == mem_b == mem_c and (inputs is None or mem_x == mem)
+        if n_proofs is None:
+            n_proofs = (a.nbytes if isinstance(a, np.ndarray) else a.numel() * a.element_size()) // self.g1_bytes
+        if rho is None:
+            rho = random_rho(n_proofs)
+            if mem == MEM_DEVICE:
+                import torch
+
+                rho = torch.from_numpy(rho.view(np.int32)).to(a.device)
+        pr, mem_r = _ptr(rho)
+        assert n_proofs == 0 or mem_r == mem
+        ok = ctypes.c_uint8(0)
+        self._ck(self.lib.b2s_groth16_verify_batch_rlc(self.h, pvk, n_proofs, px, n_inputs, pa, pb, pc, pr, mem, ctypes.byref(ok)))
+        return bool(ok.value)
 
     def pairing(self, p, q, n=None, out=None):
         """e(P_i, Q_i) element-wise.  p, q: affine G1 / G2 arrays (HOST numpy, or CUDA torch tensors with `out` a device

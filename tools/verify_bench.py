@@ -8,7 +8,11 @@ to 2^log_n: the work per proof does not depend on its values.  One proof in 64 o
 every verdict is checked.  Prints one JSON line: proofs/s over the timed calls, the per-kernel split from a separate profiled
 call, the time outside the kernels (host copies), the card and its power limit, and the algorithmic Fq-multiplication count
 per verification with that count times proofs/s as a fraction of the 2.6e10 Fq mul/s ceiling of DESIGN.md section 4 (that
-ceiling is the 381-bit one; for BN254 the fraction is against the same figure)."""
+ceiling is the 381-bit one; for BN254 the fraction is against the same figure).
+
+With --rlc the same batch, all valid, goes through groth16_verify_all (b2s_groth16_verify_batch_rlc, one verdict per
+batch) and groth16_verify_batch in alternation; the line reports both rates, their ratio, both kernel splits and the
+operation counts of both paths, and the batch with the broken proofs must be rejected."""
 import argparse
 import json
 import os
@@ -49,6 +53,29 @@ def fq_mul_count(curve, n_inputs):
     return int(miller + easy + hard + ic)
 
 
+def fq_mul_count_rlc(curve, nf=2, log_n=20):
+    """Fq multiplications per proof of the random-linear-combination check (b2s_groth16_verify_batch_rlc), the same
+    operation counts as fq_mul_count: a one-pair Miller loop with B's lines on the fly whose Fq12 squarings are shared by nf
+    proofs, rho A by 128-bit double-and-add in XYZZ (dbl 10, add 14) with one inversion, the share of the C MSM (signed
+    windows of c bits over the 255-bit scalar, one mixed XYZZ addition of 10 per point and window) and of the product of
+    the Miller values.  The per-batch terms (one final exponentiation, two prepared pairs, e(alpha, beta)^S, IC*) are
+    left out: they are shared by 2^log_n proofs.  The public-input sums cost Fr multiplications, not counted."""
+    bls = curve == "bls12_381"
+    bits = 381 if bls else 254
+    inv_fq = bits + bits // 2
+    digits = [int(b) for b in bin(gp.BLS_X_ABS)[2:]] if bls else gp.naf(6 * gp.BN_X + 2)
+    steps, adds = len(digits) - 1, sum(1 for d in digits[1:] if d)
+    sqr12, mul12, ell, dbl, add = 36, 54, 43, 28, 37
+    miller = (steps - 1) * sqr12 / nf + steps * (dbl + ell) + adds * (add + ell)
+    if not bls:
+        miller += 2 * (6 + add + ell)
+    scalar = 127 * 10 + 64 * 14 + inv_fq + 3
+    c = max(8, log_n - 4)
+    msm = (255 // c + 1) * 10
+    product = mul12 / nf
+    return int(miller + scalar + msm + product)
+
+
 def gpu_info():
     try:
         out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
@@ -66,7 +93,10 @@ def main():
     ap.add_argument("--n-inputs", type=int, default=1)
     ap.add_argument("--mem", choices=["host", "device"], default="host")
     ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--rlc", action="store_true", help="time groth16_verify_all (one verdict per batch) against the per-proof path")
     args = ap.parse_args()
+    if args.rlc:
+        return main_rlc(args)
 
     from snark_b200 import Backend
     from tests.test_gpu_verify import Sim
@@ -126,6 +156,80 @@ def main():
         "kernel_ms": kern, "outside_kernels_ms": round(prof_s * 1e3 - sum(kern.values()), 3),
         "fq_mul_per_verification": muls, "fq_mul_per_s": round(muls * pps, 1), "fraction_of_ceiling": round(muls * pps / CEILING, 4),
         "gpu": name, "power_limit": power, "invalid_checked": int((~want).sum()),
+    }))
+    be.pvk_free(sim.pvk)
+    be.close()
+
+
+def main_rlc(args):
+    """The same tiled batch, all valid, through groth16_verify_all and groth16_verify_batch in alternation; then the batch
+    with one proof in 64 broken must give False.  rho is drawn once per batch outside the timed calls."""
+    from snark_b200 import Backend
+    from snark_b200.lib import random_rho
+    from tests.test_gpu_verify import Sim
+
+    be = Backend(curve=0 if args.curve == "bls12_381" else 1)
+    rng = random.Random(20)
+    sim = Sim(be, rng, args.n_inputs)
+    base = 1 << min(12, args.log_n)
+    x, a, b = sim.scalars(rng, base)
+    c = sim.c_of(x, a, b)
+    broken = set(range(0, base, 64))
+    a_bad = [(v + 1) % sim.curve.r if i in broken else v for i, v in enumerate(a)]
+    n = 1 << args.log_n
+    reps = n // base
+    tile = lambda arrs: [np.tile(v, reps) if v is not None else None for v in arrs]
+    inputs, A, B, C = tile(sim.arrays(x, a, b, c))
+    A_bad = tile(sim.arrays(x, a_bad, b, c))[1]
+    if args.mem == "device":
+        import torch
+
+        dev = torch.device("cuda")
+        t = lambda arr: torch.from_numpy(arr.view(np.int32)).to(dev) if arr is not None else None
+        inputs, A, B, C, A_bad = t(inputs), t(A), t(B), t(C), t(A_bad)
+        rho = t(random_rho(n))
+        okd = torch.zeros(n, dtype=torch.uint8, device=dev)
+
+        def per_proof():
+            be.groth16_verify_batch(sim.pvk, inputs, args.n_inputs, A, B, C, n_proofs=n, ok=okd)
+            be.sync()
+            return bool(okd.all().item())
+    else:
+        rho = random_rho(n)
+
+        def per_proof():
+            return bool(be.groth16_verify_batch(sim.pvk, inputs, args.n_inputs, A, B, C).all())
+
+    rlc = lambda a_: be.groth16_verify_all(sim.pvk, inputs, args.n_inputs, a_, B, C, rho=rho, n_proofs=n)
+    assert rlc(A) and per_proof(), "an all-valid batch must be accepted"     # warm-up, and the checks
+    assert not rlc(A_bad), "a batch with broken proofs must be rejected"
+    t_rlc, t_pp = [], []
+    for _ in range(args.steps):
+        t0 = time.perf_counter()
+        assert rlc(A)
+        t_rlc.append(time.perf_counter() - t0)
+        t0 = time.perf_counter()
+        assert per_proof()
+        t_pp.append(time.perf_counter() - t0)
+    split = {}
+    for name, fn in (("rlc", lambda: rlc(A)), ("per_proof", per_proof)):
+        be.profile(True)
+        t0 = time.perf_counter()
+        fn()
+        prof_s = time.perf_counter() - t0
+        rep = be.profile_report()
+        be.profile(False)
+        kern = {k: round(v[1], 3) for k, v in rep.items()}
+        split[name] = {"kernel_ms": kern, "outside_kernels_ms": round(prof_s * 1e3 - sum(kern.values()), 3)}
+    pps_rlc, pps_pp = n / min(t_rlc), n / min(t_pp)
+    muls_rlc, muls_pp = fq_mul_count_rlc(args.curve, log_n=args.log_n), fq_mul_count(args.curve, args.n_inputs)
+    name, power = gpu_info()
+    print(json.dumps({
+        "curve": args.curve, "n_proofs": n, "n_inputs": args.n_inputs, "mem": args.mem,
+        "rlc_seconds": [round(s, 4) for s in t_rlc], "per_proof_seconds": [round(s, 4) for s in t_pp],
+        "rlc_proofs_per_s": round(pps_rlc, 1), "per_proof_proofs_per_s": round(pps_pp, 1), "ratio": round(pps_rlc / pps_pp, 3),
+        "split": split, "fq_mul_per_proof_rlc": muls_rlc, "fq_mul_per_proof": muls_pp,
+        "count_ratio": round(muls_pp / muls_rlc, 3), "gpu": name, "power_limit": power, "invalid_rejected": len(broken) * reps,
     }))
     be.pvk_free(sim.pvk)
     be.close()
