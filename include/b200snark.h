@@ -298,7 +298,7 @@ int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
  *                    (NULL when n_inputs == 0); a, b, c: affine arrays; ok: n_proofs bytes (1 = accepted).  All buffers
  *                    share `mem`; host batches go through bounded device scratch in chunks, so n_proofs is not limited by
  *                    device memory.  n_inputs + 1 != n_gamma_abc -> B2S_ERR_MALFORMED_VK (ark's prepare_inputs error);
- *                    n_proofs == 0 -> B2S_OK.  Points are assumed valid, as in ark: decode untrusted bytes with validate = 1.
+ *                    n_proofs == 0 -> B2S_OK.  Points are assumed valid, as in ark: untrusted bytes go to the _bytes form below.
  *   b2s_groth16_verify_batch_rlc  one verdict for the whole batch (bellman's groth16::batch, Zcash's batch verifier): with
  *                    caller-drawn 128-bit rho_i,
  *                      prod_i e(rho_i A_i, B_i) * e(IC*, -gamma) * e(C*, -delta) == e(alpha, beta)^S,
@@ -313,6 +313,20 @@ int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
  *                    the lowest such index.  Another curve's key or a null buffer -> B2S_ERR_INVALID_ARG;
  *                    n_inputs + 1 != n_gamma_abc -> B2S_ERR_MALFORMED_VK; n_proofs == 0 -> B2S_OK with *ok = 1.  To learn
  *                    which proofs of a rejected batch failed, run b2s_groth16_verify_batch on it.
+ *   b2s_groth16_verify_batch_bytes / b2s_groth16_verify_batch_rlc_bytes  the same two checks on ark-serialized proofs as
+ *                    received from untrusted parties: `proofs` is n_proofs Proofs back to back (a || b || c, as
+ *                    b2s_proof_serialize_* writes them, 192 / 128 B compressed on BLS12-381 / BN254), exactly `len` bytes,
+ *                    else B2S_ERR_INVALID_DATA.  compressed = 1 / 0 as for the deserializers.  Every point is decoded ON THE
+ *                    DEVICE with validation always on (flags, canonical coordinates, curve equation, prime-order subgroup),
+ *                    so the RLC bound above holds without a separate decoding step; the decoded points never leave the
+ *                    device.  A proof that fails to decode is rejected on its own: the call does not fail for it.
+ *                      ok[i]      (per proof) 1 = proof i decoded and satisfies the verification equation, else 0
+ *                      *ok        (RLC, HOST, always written) 1 = every proof decoded and the combination holds
+ *                      reason[i]  may be NULL; 0 = proof i decoded, else 16 * (1 + e) + r with e = 0 / 1 / 2 for a / b / c (the
+ *                                 first failing element) and r the decode reason: 1 bad flags, 2 coordinate >= p, 3 not on
+ *                                 the curve (or no square root), 4 not in the prime-order subgroup
+ *                    `mem` covers inputs, proofs, rho, the per-proof ok and reason.  Argument errors are those of the points
+ *                    entry points above; n_proofs == 0 (with len == 0) -> B2S_OK, RLC *ok = 1.
  *   b2s_pairing     Pairing::pairing, element-wise: out[i] = e(P_i, Q_i), i < n; a pair with P or Q at infinity (all-zero)
  *                    gives 1.  All buffers share `mem`. */
 int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,
@@ -323,6 +337,12 @@ int32_t b2s_groth16_verify_batch(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_pr
 int32_t b2s_groth16_verify_batch_rlc(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
                                      const void* a_g1, const void* b_g2, const void* c_g1, const void* rho, int32_t mem,
                                      uint8_t* ok);
+int32_t b2s_groth16_verify_batch_bytes(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                       const uint8_t* proofs, uint64_t len, int32_t compressed, int32_t mem, uint8_t* ok,
+                                       uint8_t* reason);
+int32_t b2s_groth16_verify_batch_rlc_bytes(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                           const uint8_t* proofs, uint64_t len, int32_t compressed, const void* rho, int32_t mem,
+                                           uint8_t* ok, uint8_t* reason);
 int32_t b2s_pairing(b2s_ctx* ctx, const void* p_g1, const void* q_g2, uint64_t n, int32_t mem, void* out_gt);
 
 /* ---- setup helper (SURVEY 8(f) row 2): fixed-base batch multiplication -------------------------

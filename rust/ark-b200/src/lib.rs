@@ -74,6 +74,11 @@ extern "C" {
     pub fn b2s_groth16_verify_batch_rlc(ctx: *mut B2sCtx, pvk: *const B2sPvk, n_proofs: u64, inputs: *const c_void, n_inputs: u64,
                                         a_g1: *const c_void, b_g2: *const c_void, c_g1: *const c_void, rho: *const c_void, mem: i32,
                                         ok: *mut u8) -> i32;
+    pub fn b2s_groth16_verify_batch_bytes(ctx: *mut B2sCtx, pvk: *const B2sPvk, n_proofs: u64, inputs: *const c_void, n_inputs: u64,
+                                          proofs: *const u8, len: u64, compressed: i32, mem: i32, ok: *mut u8, reason: *mut u8) -> i32;
+    pub fn b2s_groth16_verify_batch_rlc_bytes(ctx: *mut B2sCtx, pvk: *const B2sPvk, n_proofs: u64, inputs: *const c_void,
+                                              n_inputs: u64, proofs: *const u8, len: u64, compressed: i32, rho: *const c_void,
+                                              mem: i32, ok: *mut u8, reason: *mut u8) -> i32;
     pub fn b2s_pairing(ctx: *mut B2sCtx, p_g1: *const c_void, q_g2: *const c_void, n: u64, mem: i32, out_gt: *mut c_void) -> i32;
     // universal-setup schemes (UniversalSetupSNARK, snark/src/lib.rs:107-133): the seams a polynomial-commitment /
     // evaluation-domain backend binds (INTEGRATION.md section 8).  mem: 0 host, 1 device; s, c, z: one Montgomery Fr on the host
@@ -218,35 +223,18 @@ impl<E: Pairing> Groth16B200<E> {
     /// as in ark: proofs from untrusted bytes are decoded with validation first.
     pub fn verify_batch(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>], proofs: &[Proof<E>]) -> Result<Vec<bool>, B200Error> {
         if inputs.len() != proofs.len() { return Err(SynthesisError::AssignmentMissing.into()); }
-        let ni = vk.gamma_abc_g1.len().saturating_sub(1);
-        if inputs.iter().any(|x| x.len() != ni) { return Err(SynthesisError::MalformedVerifyingKey.into()); }
-        // the curve from the base field width: 48-byte Fq is BLS12-381, 32-byte Fq BN254
-        let curve_id = if core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>() == 48 { 0 } else { 1 };
-        let mut ctx: *mut B2sCtx = core::ptr::null_mut();
-        check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
-        let run = || -> Result<Vec<bool>, B200Error> {
-            let (alpha, beta, gamma, delta) = (pack_points(&[vk.alpha_g1]), pack_points(&[vk.beta_g2]), pack_points(&[vk.gamma_g2]),
-                                               pack_points(&[vk.delta_g2]));
-            let abc = pack_points(&vk.gamma_abc_g1);
-            let mut pvk: *mut B2sPvk = core::ptr::null_mut();
-            check(ctx, unsafe { b2s_vk_prepare(ctx, alpha.as_ptr().cast(), beta.as_ptr().cast(), gamma.as_ptr().cast(),
-                                               delta.as_ptr().cast(), abc.as_ptr().cast(), vk.gamma_abc_g1.len() as u64, &mut pvk) })?;
-            let x: Vec<E::ScalarField> = inputs.iter().flat_map(|v| v.iter().copied()).collect();
+        let (ni, x) = Self::flat_inputs(vk, inputs)?;
+        Self::with_prepared(vk, |ctx, pvk| {
             let a = pack_points(&proofs.iter().map(|p| p.a).collect::<Vec<_>>());
             let b = pack_points(&proofs.iter().map(|p| p.b).collect::<Vec<_>>());
             let c = pack_points(&proofs.iter().map(|p| p.c).collect::<Vec<_>>());
             let mut ok = vec![0u8; proofs.len()];
-            let st = unsafe { b2s_groth16_verify_batch(ctx, pvk, proofs.len() as u64,
-                                                       if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
-                                                       a.as_ptr().cast(), b.as_ptr().cast(), c.as_ptr().cast(), 0 /* B2S_MEM_HOST */,
-                                                       ok.as_mut_ptr()) };
-            unsafe { b2s_pvk_free(ctx, pvk) };
-            check(ctx, st)?;
+            check(ctx, unsafe { b2s_groth16_verify_batch(ctx, pvk, proofs.len() as u64,
+                                                         if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
+                                                         a.as_ptr().cast(), b.as_ptr().cast(), c.as_ptr().cast(), 0 /* B2S_MEM_HOST */,
+                                                         ok.as_mut_ptr()) })?;
             Ok(ok.into_iter().map(|v| v != 0).collect())
-        };
-        let out = run();
-        unsafe { b2s_ctx_destroy(ctx) };
-        out
+        })
     }
 
     /// One verdict for the whole batch: `true` when every proof is accepted, by a random linear combination of the
@@ -258,34 +246,90 @@ impl<E: Pairing> Groth16B200<E> {
     pub fn verify_all<R: RngCore + CryptoRng>(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>], proofs: &[Proof<E>], rng: &mut R)
         -> Result<bool, B200Error> {
         if inputs.len() != proofs.len() { return Err(SynthesisError::AssignmentMissing.into()); }
-        let ni = vk.gamma_abc_g1.len().saturating_sub(1);
-        if inputs.iter().any(|x| x.len() != ni) { return Err(SynthesisError::MalformedVerifyingKey.into()); }
-        let mut rho = vec![0u8; 16 * proofs.len()];
+        let (ni, x) = Self::flat_inputs(vk, inputs)?;
+        let rho = Self::draw_rho(proofs.len(), rng);
+        Self::with_prepared(vk, |ctx, pvk| {
+            let a = pack_points(&proofs.iter().map(|p| p.a).collect::<Vec<_>>());
+            let b = pack_points(&proofs.iter().map(|p| p.b).collect::<Vec<_>>());
+            let c = pack_points(&proofs.iter().map(|p| p.c).collect::<Vec<_>>());
+            let mut ok = 0u8;
+            check(ctx, unsafe { b2s_groth16_verify_batch_rlc(ctx, pvk, proofs.len() as u64,
+                                                             if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
+                                                             a.as_ptr().cast(), b.as_ptr().cast(), c.as_ptr().cast(), rho.as_ptr().cast(),
+                                                             0 /* B2S_MEM_HOST */, &mut ok) })?;
+            Ok(ok != 0)
+        })
+    }
+
+    /// `verify_batch` on serialized proofs as received from untrusted parties: `proofs` is `inputs.len()` ark `Proof`s
+    /// back to back (`serialize_compressed` / `serialize_uncompressed` of each, a || b || c).  Every point is decoded and
+    /// validated (curve equation, prime-order subgroup) on the GPU, where it stays.  A proof that fails to decode is
+    /// rejected on its own: the verdict is `false` and `reasons[i]` is 16 * (1 + e) + r for its first bad element e
+    /// (0 a, 1 b, 2 c) and decode reason r (1 flags, 2 coordinate >= p, 3 not on the curve, 4 not in the subgroup);
+    /// 0 when the proof decoded.  A wrong byte length is `InvalidData`.
+    pub fn verify_batch_bytes(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>], proofs: &[u8], compressed: bool)
+        -> Result<(Vec<bool>, Vec<u8>), B200Error> {
+        let (ni, x) = Self::flat_inputs(vk, inputs)?;
+        Self::with_prepared(vk, |ctx, pvk| {
+            let (mut ok, mut reason) = (vec![0u8; inputs.len()], vec![0u8; inputs.len()]);
+            check(ctx, unsafe { b2s_groth16_verify_batch_bytes(ctx, pvk, inputs.len() as u64,
+                                                               if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
+                                                               proofs.as_ptr(), proofs.len() as u64, compressed as i32,
+                                                               0 /* B2S_MEM_HOST */, ok.as_mut_ptr(), reason.as_mut_ptr()) })?;
+            Ok((ok.into_iter().map(|v| v != 0).collect(), reason))
+        })
+    }
+
+    /// `verify_all` on serialized proofs (layout and reasons as for `verify_batch_bytes`): `true` only when every proof
+    /// decodes and the random linear combination holds.  Validation is always on, so the 2^-128 bound of `verify_all`
+    /// needs no separate decoding step.
+    pub fn verify_all_bytes<R: RngCore + CryptoRng>(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>], proofs: &[u8],
+                                                   compressed: bool, rng: &mut R) -> Result<(bool, Vec<u8>), B200Error> {
+        let (ni, x) = Self::flat_inputs(vk, inputs)?;
+        let rho = Self::draw_rho(inputs.len(), rng);
+        Self::with_prepared(vk, |ctx, pvk| {
+            let (mut ok, mut reason) = (0u8, vec![0u8; inputs.len()]);
+            check(ctx, unsafe { b2s_groth16_verify_batch_rlc_bytes(ctx, pvk, inputs.len() as u64,
+                                                                   if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() },
+                                                                   ni as u64, proofs.as_ptr(), proofs.len() as u64, compressed as i32,
+                                                                   rho.as_ptr().cast(), 0 /* B2S_MEM_HOST */, &mut ok,
+                                                                   reason.as_mut_ptr()) })?;
+            Ok((ok != 0, reason))
+        })
+    }
+
+    /// n nonzero 128-bit weights from `rng`, 16 little-endian bytes each
+    fn draw_rho<R: RngCore + CryptoRng>(n: usize, rng: &mut R) -> Vec<u8> {
+        let mut rho = vec![0u8; 16 * n];
         for w in rho.chunks_mut(16) {
             while w.iter().all(|b| *b == 0) { rng.fill_bytes(w); }
         }
+        rho
+    }
+
+    /// the public inputs row-major, after the input-count check (`MalformedVerifyingKey`, as in ark)
+    fn flat_inputs(vk: &VerifyingKey<E>, inputs: &[Vec<E::ScalarField>]) -> Result<(usize, Vec<E::ScalarField>), B200Error> {
+        let ni = vk.gamma_abc_g1.len().saturating_sub(1);
+        if inputs.iter().any(|x| x.len() != ni) { return Err(SynthesisError::MalformedVerifyingKey.into()); }
+        Ok((ni, inputs.iter().flat_map(|v| v.iter().copied()).collect()))
+    }
+
+    /// runs `f` with a ctx and the key prepared on it, and frees both whatever `f` returns
+    fn with_prepared<T>(vk: &VerifyingKey<E>, f: impl FnOnce(*mut B2sCtx, *mut B2sPvk) -> Result<T, B200Error>) -> Result<T, B200Error> {
+        // the curve from the base field width: 48-byte Fq is BLS12-381, 32-byte Fq BN254
         let curve_id = if core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>() == 48 { 0 } else { 1 };
         let mut ctx: *mut B2sCtx = core::ptr::null_mut();
         check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
-        let run = || -> Result<bool, B200Error> {
+        let run = || -> Result<T, B200Error> {
             let (alpha, beta, gamma, delta) = (pack_points(&[vk.alpha_g1]), pack_points(&[vk.beta_g2]), pack_points(&[vk.gamma_g2]),
                                                pack_points(&[vk.delta_g2]));
             let abc = pack_points(&vk.gamma_abc_g1);
             let mut pvk: *mut B2sPvk = core::ptr::null_mut();
             check(ctx, unsafe { b2s_vk_prepare(ctx, alpha.as_ptr().cast(), beta.as_ptr().cast(), gamma.as_ptr().cast(),
                                                delta.as_ptr().cast(), abc.as_ptr().cast(), vk.gamma_abc_g1.len() as u64, &mut pvk) })?;
-            let x: Vec<E::ScalarField> = inputs.iter().flat_map(|v| v.iter().copied()).collect();
-            let a = pack_points(&proofs.iter().map(|p| p.a).collect::<Vec<_>>());
-            let b = pack_points(&proofs.iter().map(|p| p.b).collect::<Vec<_>>());
-            let c = pack_points(&proofs.iter().map(|p| p.c).collect::<Vec<_>>());
-            let mut ok = 0u8;
-            let st = unsafe { b2s_groth16_verify_batch_rlc(ctx, pvk, proofs.len() as u64,
-                                                           if ni == 0 { core::ptr::null() } else { x.as_ptr().cast() }, ni as u64,
-                                                           a.as_ptr().cast(), b.as_ptr().cast(), c.as_ptr().cast(), rho.as_ptr().cast(),
-                                                           0 /* B2S_MEM_HOST */, &mut ok) };
+            let out = f(ctx, pvk);
             unsafe { b2s_pvk_free(ctx, pvk) };
-            check(ctx, st)?;
-            Ok(ok != 0)
+            out
         };
         let out = run();
         unsafe { b2s_ctx_destroy(ctx) };

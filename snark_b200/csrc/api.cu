@@ -44,6 +44,11 @@ int32_t pairing_batch(Ctx* c, const void* p, const void* q, uint64_t n, int32_t 
 // verify_rlc.cu
 int32_t groth16_verify_batch_rlc(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const void* a, const void* b,
                                  const void* cc, const void* rho, int32_t mem, uint8_t* ok);
+// verify_bytes.cu
+int32_t groth16_verify_batch_bytes(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const uint8_t* proofs,
+                                   uint64_t len, bool compressed, int32_t mem, uint8_t* ok, uint8_t* reason);
+int32_t groth16_verify_batch_rlc_bytes(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const uint8_t* proofs,
+                                       uint64_t len, bool compressed, const void* rho, int32_t mem, uint8_t* ok, uint8_t* reason);
 }  // namespace b2s
 
 #define LOCK(ctx)                                      \
@@ -619,6 +624,20 @@ int32_t b2s_groth16_verify_batch_rlc(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t 
     LOCK(ctx);
     if (!pvk) return fail(ctx, B2S_ERR_INVALID_ARG, "verify_batch_rlc: null prepared key");
     return groth16_verify_batch_rlc(ctx, pvk, n_proofs, inputs, n_inputs, a_g1, b_g2, c_g1, rho, mem, ok);
+}
+int32_t b2s_groth16_verify_batch_bytes(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                       const uint8_t* proofs, uint64_t len, int32_t compressed, int32_t mem, uint8_t* ok,
+                                       uint8_t* reason) {
+    LOCK(ctx);
+    if (!pvk) return fail(ctx, B2S_ERR_INVALID_ARG, "verify_batch_bytes: null prepared key");
+    return groth16_verify_batch_bytes(ctx, pvk, n_proofs, inputs, n_inputs, proofs, len, compressed != 0, mem, ok, reason);
+}
+int32_t b2s_groth16_verify_batch_rlc_bytes(b2s_ctx* ctx, const b2s_pvk* pvk, uint64_t n_proofs, const void* inputs, uint64_t n_inputs,
+                                           const uint8_t* proofs, uint64_t len, int32_t compressed, const void* rho, int32_t mem,
+                                           uint8_t* ok, uint8_t* reason) {
+    LOCK(ctx);
+    if (!pvk) return fail(ctx, B2S_ERR_INVALID_ARG, "verify_batch_rlc_bytes: null prepared key");
+    return groth16_verify_batch_rlc_bytes(ctx, pvk, n_proofs, inputs, n_inputs, proofs, len, compressed != 0, rho, mem, ok, reason);
 }
 int32_t b2s_pairing(b2s_ctx* ctx, const void* p_g1, const void* q_g2, uint64_t n, int32_t mem, void* out_gt) {
     LOCK(ctx);

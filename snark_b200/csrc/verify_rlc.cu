@@ -4,13 +4,14 @@
 // through one final exponentiation.
 //
 // Host batches are processed in chunks through bounded scratch, as in verify.cu.  Across chunks four running values stay
-// on the device: the Fq12 Miller product, C* (XYZZ), S and t_j = sum_i rho_i x_ij (canonical Fr).  Per chunk:
+// on the device: the Fq12 Miller product, C* (XYZZ), S and t_j = sum_i rho_i x_ij (canonical Fr).  The host side is cut
+// into the steps of RlcRun (verify.cuh), which verify_bytes.cu shares.  Per chunk (rlc_chunk):
 //   verify_rlc_miller   one thread per RLC_NF proofs: rho_i A_i, then the Miller loop with B_i's lines on the fly; also
 //                       widens rho to Fr words for the MSM and records the lowest zero rho
 //   verify_rlc_product  the chunk's Fq12 values multiplied together, in place, into the running product
 //   msm_*               C*_chunk = sum_i rho_i C_i (canonical scalars)
 //   verify_rlc_inputs   S and t_j: per-block partial sums, then one block adds them and C*_chunk to the running values
-// and once at the end verify_rlc_final (one thread): IC* from S gamma_abc[0] and the public-input window tables applied to
+// and after the last chunk verify_rlc_final (one thread): IC* from S gamma_abc[0] and the public-input window tables applied to
 // t_j, C* affine, the two prepared pairs, the final exponentiation, and the comparison with e(alpha, beta)^S.
 #include <algorithm>
 
@@ -121,6 +122,100 @@ __global__ void verify_rlc_final_kernel(const Fp12<typename Curve::FqP>* f, cons
     *ok = rlc_verdict<Curve>(*f, ic.to_affine(), c_acc->to_affine(), &prep[0], &prep[1], *ab, s.v) ? 1 : 0;
 }
 
+size_t rlc_per_proof(Ctx* c) {
+    size_t out = 0;
+    dispatch_curve(c, [&](auto curve) {
+        using C = decltype(curve);
+        out = sizeof(Fp12<typename C::FqP>) / RLC_NF + sizeof(typename C::Fr);   // its share of the Miller values, rho widened
+        return (int32_t)B2S_OK;
+    });
+    return out;
+}
+
+int32_t rlc_begin(Ctx* c, const b2s_pvk* pvk, uint64_t ni, uint64_t ch, const char* name, RlcRun& r) {
+    r.c = c; r.pvk = pvk; r.name = name; r.ni = ni; r.ch = ch;
+    return dispatch_curve(c, [&](auto curve) -> int32_t {
+        using C = decltype(curve);
+        using F12 = Fp12<typename C::FqP>;
+        using Fr = typename C::Fr;
+        const size_t fr = sizeof(Fr), f12 = sizeof(F12);
+        const uint64_t groups = cdiv(ch, RLC_NF), blocks = cdiv(ch, RLC_ROWS);
+        B2S_TRY(r.scratch.alloc(c, groups * f12 + ch * fr + blocks * (ni + 1) * fr));
+        char* sp = r.scratch.as<char>();
+        r.f = sp;
+        r.rho_fr = sp + groups * f12;
+        r.part = sp + groups * f12 + ch * fr;
+        // running values: the Miller product, C*, this chunk's C*, S and t_j, the lowest zero rho, the verdict
+        const size_t xyzz = sizeof(typename C::G1);
+        B2S_TRY(r.state.alloc(c, f12 + 2 * xyzz + (ni + 1) * fr + 8 + 8));
+        char* q = r.state.as<char>();
+        r.prod = q;
+        r.c_acc = q + f12;
+        r.c_chunk = q + f12 + xyzz;
+        r.st = q + f12 + 2 * xyzz;
+        r.zero_at = reinterpret_cast<unsigned long long*>(q + f12 + 2 * xyzz + (ni + 1) * fr);
+        r.ok_dev = reinterpret_cast<uint8_t*>(r.zero_at + 1);
+        const F12 one = F12::one();
+        B2S_CUDA(c, cudaMemcpyAsync(r.prod, &one, f12, cudaMemcpyHostToDevice, c->stream));
+        B2S_CUDA(c, cudaMemsetAsync(r.c_acc, 0, xyzz + xyzz + (ni + 1) * fr, c->stream));   // identity, zeros
+        B2S_CUDA(c, cudaMemsetAsync(r.zero_at, 0xFF, 8, c->stream));
+        return (int32_t)B2S_OK;
+    });
+}
+
+int32_t rlc_chunk(RlcRun& r, const void* xi, const void* ai, const void* bi, const void* ci, const void* ri, uint32_t m, uint64_t base,
+                  bool last) {
+    Ctx* c = r.c;
+    const uint64_t ni = r.ni;
+    return dispatch_curve(c, [&](auto curve) -> int32_t {
+        using C = decltype(curve);
+        using P = typename C::FqP;
+        using F12 = Fp12<P>;
+        using Fr = typename C::Fr;
+        using G1A = typename C::G1Affine;
+        auto* f = static_cast<F12*>(r.f);
+        auto* rho_fr = static_cast<Fr*>(r.rho_fr);
+        auto* part = static_cast<Fr*>(r.part);
+        auto* c_chunk = static_cast<typename C::G1*>(r.c_chunk);
+        const uint32_t* rw = static_cast<const uint32_t*>(ri);
+        const uint32_t g = cdiv(m, RLC_NF);
+        B2S_LAUNCH_N(c, "verify_rlc_miller", (verify_rlc_miller_kernel<C, RLC_NF>), cdiv(g, VERIFY_THREADS), VERIFY_THREADS, 0,
+                     static_cast<const G1A*>(ai), static_cast<const typename C::G2Affine*>(bi), rw, m, base, rho_fr, r.zero_at, f);
+        uint32_t cnt = g;
+        while (cnt > RLC_PER) {
+            const uint32_t stride = cdiv(cnt, RLC_PER);
+            B2S_LAUNCH_N(c, "verify_rlc_product", verify_rlc_product_kernel<P>, cdiv(stride, VERIFY_THREADS), VERIFY_THREADS, 0, f,
+                         cnt, stride, (F12*)nullptr);
+            cnt = stride;
+        }
+        B2S_LAUNCH_N(c, "verify_rlc_product", verify_rlc_product_kernel<P>, 1, 1, 0, f, cnt, 1u, static_cast<F12*>(r.prod));
+        B2S_TRY(msm_run(c, 1, ci, rho_fr, m, false, c_chunk));
+        const uint32_t nb = cdiv(m, RLC_ROWS);
+        const unsigned cols = (unsigned)std::min<uint64_t>(VERIFY_THREADS, 32 * cdiv(ni + 1, 32));
+        B2S_LAUNCH_N(c, "verify_rlc_inputs", verify_rlc_inputs_kernel<Fr>, nb, cols, 0, static_cast<const Fr*>(xi), rw, m,
+                     (uint32_t)ni, part);
+        B2S_LAUNCH_N(c, "verify_rlc_inputs", verify_rlc_fold_kernel<C>, 1, cols, 0, (const Fr*)part, nb, (uint32_t)ni,
+                     static_cast<Fr*>(r.st), (const typename C::G1*)c_chunk, static_cast<typename C::G1*>(r.c_acc));
+        if (last)
+            B2S_LAUNCH_N(c, "verify_rlc_final", verify_rlc_final_kernel<C>, 1, 1, 0, static_cast<const F12*>(r.prod),
+                         static_cast<const Fr*>(r.st), (uint32_t)ni, r.pvk->abc0.as<G1A>(), r.pvk->table.as<G1A>(),
+                         static_cast<const typename C::G1*>(r.c_acc), r.pvk->prep.as<G2Prepared<C>>(), r.pvk->ab.as<F12>(), r.ok_dev);
+        return (int32_t)B2S_OK;
+    });
+}
+
+int32_t rlc_read(RlcRun& r, uint8_t* ok) {
+    Ctx* c = r.c;
+    unsigned long long zero_host = 0;
+    uint8_t ok_host = 0;
+    B2S_CUDA(c, cudaMemcpyAsync(&zero_host, r.zero_at, 8, cudaMemcpyDeviceToHost, c->stream));
+    B2S_CUDA(c, cudaMemcpyAsync(&ok_host, r.ok_dev, 1, cudaMemcpyDeviceToHost, c->stream));
+    B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (zero_host != ~0ull) return fail(c, B2S_ERR_INVALID_ARG, "%s: rho[%llu] is zero", r.name, zero_host);
+    *ok = ok_host;
+    return B2S_OK;
+}
+
 int32_t groth16_verify_batch_rlc(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void* inputs, uint64_t ni, const void* a, const void* b,
                                  const void* cc, const void* rho, int32_t mem, uint8_t* ok) {
     if (pvk->curve != c->curve) return fail(c, B2S_ERR_INVALID_ARG, "verify_batch_rlc: the prepared key belongs to another curve");
@@ -132,95 +227,40 @@ int32_t groth16_verify_batch_rlc(Ctx* c, const b2s_pvk* pvk, uint64_t n, const v
     if (n == 0) { *ok = 1; return B2S_OK; }
     if (!a || !b || !cc || !rho || (ni && !inputs)) return fail(c, B2S_ERR_INVALID_ARG, "verify_batch_rlc: null buffer");
     const bool host = mem != B2S_MEM_DEVICE;
-    return dispatch_curve(c, [&](auto curve) -> int32_t {
-        using C = decltype(curve);
-        using P = typename C::FqP;
-        using F12 = Fp12<P>;
-        using Fr = typename C::Fr;
-        using G1A = typename C::G1Affine;
-        constexpr size_t RHO = 16;
-        const size_t g1 = sizeof(G1A), g2 = sizeof(typename C::G2Affine), fr = sizeof(Fr), f12 = sizeof(F12);
-        const size_t in_row = ni * fr;
-        // per proof: its share of the Miller values, rho widened, and the staged inputs of host batches
-        const size_t per_proof = f12 / RLC_NF + fr + (host ? in_row + 2 * g1 + g2 + RHO : 0);
-        const uint64_t ch = chunk_size(n, per_proof);
-        const uint64_t groups = cdiv(ch, RLC_NF), blocks = cdiv(ch, RLC_ROWS);
-        DevBuf scratch, state;
-        B2S_TRY(scratch.alloc(c, groups * f12 + ch * fr + blocks * (ni + 1) * fr + (host ? ch * (in_row + 2 * g1 + g2 + RHO) : 0)));
-        char* sp = scratch.as<char>();
-        auto* f = reinterpret_cast<F12*>(sp);
-        auto* rho_fr = reinterpret_cast<Fr*>(sp + groups * f12);
-        auto* part = reinterpret_cast<Fr*>(sp + groups * f12 + ch * fr);
-        char* stage = sp + groups * f12 + ch * fr + blocks * (ni + 1) * fr;   // host mode: inputs, a, b, c, rho
-        // running values: the Miller product, C*, this chunk's C*, S and t_j, the lowest zero rho, the verdict
-        const size_t xyzz = sizeof(typename C::G1);
-        B2S_TRY(state.alloc(c, f12 + 2 * xyzz + (ni + 1) * fr + 8 + 8));
-        char* q = state.as<char>();
-        auto* prod = reinterpret_cast<F12*>(q);
-        auto* c_acc = reinterpret_cast<typename C::G1*>(q + f12);
-        auto* c_chunk = reinterpret_cast<typename C::G1*>(q + f12 + xyzz);
-        auto* st = reinterpret_cast<Fr*>(q + f12 + 2 * xyzz);
-        auto* zero_at = reinterpret_cast<unsigned long long*>(q + f12 + 2 * xyzz + (ni + 1) * fr);
-        auto* ok_dev = reinterpret_cast<uint8_t*>(zero_at + 1);
-        const F12 one = F12::one();
-        B2S_CUDA(c, cudaMemcpyAsync(prod, &one, f12, cudaMemcpyHostToDevice, c->stream));
-        B2S_CUDA(c, cudaMemsetAsync(c_acc, 0, xyzz + xyzz + (ni + 1) * fr, c->stream));   // identity, zeros
-        B2S_CUDA(c, cudaMemsetAsync(zero_at, 0xFF, 8, c->stream));
-        for (uint64_t base = 0; base < n; base += ch) {
-            const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
-            const char *xi, *ai, *bi, *ci, *ri;
-            if (host) {
-                char* s = stage;
-                xi = s; s += ch * in_row;
-                ai = s; s += ch * g1;
-                bi = s; s += ch * g2;
-                ci = s; s += ch * g1;
-                ri = s;
-                if (ni) B2S_CUDA(c, cudaMemcpyAsync((void*)xi, static_cast<const char*>(inputs) + base * in_row, m * in_row, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)ai, static_cast<const char*>(a) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)bi, static_cast<const char*>(b) + base * g2, m * g2, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)ci, static_cast<const char*>(cc) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)ri, static_cast<const char*>(rho) + base * RHO, m * RHO, cudaMemcpyHostToDevice, c->stream));
-            } else {
-                xi = ni ? static_cast<const char*>(inputs) + base * in_row : nullptr;
-                ai = static_cast<const char*>(a) + base * g1;
-                bi = static_cast<const char*>(b) + base * g2;
-                ci = static_cast<const char*>(cc) + base * g1;
-                ri = static_cast<const char*>(rho) + base * RHO;
-            }
-            const uint32_t* rw = reinterpret_cast<const uint32_t*>(ri);
-            const uint32_t g = cdiv(m, RLC_NF);
-            B2S_LAUNCH_N(c, "verify_rlc_miller", (verify_rlc_miller_kernel<C, RLC_NF>), cdiv(g, VERIFY_THREADS), VERIFY_THREADS, 0,
-                         reinterpret_cast<const G1A*>(ai), reinterpret_cast<const typename C::G2Affine*>(bi), rw, m, base, rho_fr,
-                         zero_at, f);
-            uint32_t cnt = g;
-            while (cnt > RLC_PER) {
-                const uint32_t stride = cdiv(cnt, RLC_PER);
-                B2S_LAUNCH_N(c, "verify_rlc_product", verify_rlc_product_kernel<P>, cdiv(stride, VERIFY_THREADS), VERIFY_THREADS, 0, f,
-                             cnt, stride, (F12*)nullptr);
-                cnt = stride;
-            }
-            B2S_LAUNCH_N(c, "verify_rlc_product", verify_rlc_product_kernel<P>, 1, 1, 0, f, cnt, 1u, prod);
-            B2S_TRY(msm_run(c, 1, ci, rho_fr, m, false, c_chunk));
-            const uint32_t nb = cdiv(m, RLC_ROWS);
-            const unsigned cols = (unsigned)std::min<uint64_t>(VERIFY_THREADS, 32 * cdiv(ni + 1, 32));
-            B2S_LAUNCH_N(c, "verify_rlc_inputs", verify_rlc_inputs_kernel<Fr>, nb, cols, 0, reinterpret_cast<const Fr*>(xi), rw, m,
-                         (uint32_t)ni, part);
-            B2S_LAUNCH_N(c, "verify_rlc_inputs", verify_rlc_fold_kernel<C>, 1, cols, 0, (const Fr*)part, nb, (uint32_t)ni, st,
-                         (const typename C::G1*)c_chunk, c_acc);
+    const Sizes z = sizes(c);
+    const size_t g1 = z.g1, g2 = z.g2, in_row = ni * z.fr;
+    // per proof: the check's own scratch, and the staged inputs of host batches
+    const size_t stage_row = host ? in_row + 2 * g1 + g2 + RLC_RHO : 0;
+    const uint64_t ch = chunk_size(n, rlc_per_proof(c) + stage_row);
+    RlcRun r;
+    B2S_TRY(rlc_begin(c, pvk, ni, ch, "verify_batch_rlc", r));
+    DevBuf stage;   // host mode: inputs, a, b, c, rho
+    B2S_TRY(stage.alloc(c, ch * stage_row));
+    for (uint64_t base = 0; base < n; base += ch) {
+        const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
+        const char *xi, *ai, *bi, *ci, *ri;
+        if (host) {
+            char* s = stage.as<char>();
+            xi = s; s += ch * in_row;
+            ai = s; s += ch * g1;
+            bi = s; s += ch * g2;
+            ci = s; s += ch * g1;
+            ri = s;
+            if (ni) B2S_CUDA(c, cudaMemcpyAsync((void*)xi, static_cast<const char*>(inputs) + base * in_row, m * in_row, cudaMemcpyHostToDevice, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync((void*)ai, static_cast<const char*>(a) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync((void*)bi, static_cast<const char*>(b) + base * g2, m * g2, cudaMemcpyHostToDevice, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync((void*)ci, static_cast<const char*>(cc) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync((void*)ri, static_cast<const char*>(rho) + base * RLC_RHO, m * RLC_RHO, cudaMemcpyHostToDevice, c->stream));
+        } else {
+            xi = ni ? static_cast<const char*>(inputs) + base * in_row : nullptr;
+            ai = static_cast<const char*>(a) + base * g1;
+            bi = static_cast<const char*>(b) + base * g2;
+            ci = static_cast<const char*>(cc) + base * g1;
+            ri = static_cast<const char*>(rho) + base * RLC_RHO;
         }
-        B2S_LAUNCH_N(c, "verify_rlc_final", verify_rlc_final_kernel<C>, 1, 1, 0, (const F12*)prod, (const Fr*)st, (uint32_t)ni,
-                     pvk->abc0.as<G1A>(), pvk->table.as<G1A>(), (const typename C::G1*)c_acc, pvk->prep.as<G2Prepared<C>>(),
-                     pvk->ab.as<F12>(), ok_dev);
-        unsigned long long zero_host = 0;
-        uint8_t ok_host = 0;
-        B2S_CUDA(c, cudaMemcpyAsync(&zero_host, zero_at, 8, cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaMemcpyAsync(&ok_host, ok_dev, 1, cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        if (zero_host != ~0ull) return fail(c, B2S_ERR_INVALID_ARG, "verify_batch_rlc: rho[%llu] is zero", zero_host);
-        *ok = ok_host;
-        return (int32_t)B2S_OK;
-    });
+        B2S_TRY(rlc_chunk(r, xi, ai, bi, ci, ri, m, base, base + m == n));
+    }
+    return rlc_read(r, ok);
 }
 
 }  // namespace b2s

@@ -96,6 +96,10 @@ SIGNATURES = {
                                            c_void_p]),
     "b2s_groth16_verify_batch_rlc": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p,
                                                c_void_p, c_int32, POINTER(ctypes.c_uint8)]),
+    "b2s_groth16_verify_batch_bytes": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_uint64, c_int32, c_int32,
+                                                 c_void_p, c_void_p]),
+    "b2s_groth16_verify_batch_rlc_bytes": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_uint64, c_int32,
+                                                     c_void_p, c_int32, POINTER(ctypes.c_uint8), c_void_p]),
     "b2s_pairing": (c_int32, [c_void_p, c_void_p, c_void_p, c_uint64, c_int32, c_void_p]),
     "b2s_fixed_base_g1": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
     "b2s_fixed_base_g2": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_void_p]),
@@ -462,6 +466,58 @@ class Backend:
         ok = ctypes.c_uint8(0)
         self._ck(self.lib.b2s_groth16_verify_batch_rlc(self.h, pvk, n_proofs, px, n_inputs, pa, pb, pc, pr, mem, ctypes.byref(ok)))
         return bool(ok.value)
+
+    def _proof_buf(self, proofs, compressed, n_proofs):
+        """serialized proofs (bytes / numpy uint8 on the HOST, or a CUDA torch uint8 tensor) -> (address, mem, len, n_proofs)"""
+        if isinstance(proofs, (bytes, bytearray, memoryview)):
+            proofs = np.frombuffer(bytes(proofs), dtype=np.uint8)
+        ln = proofs.nbytes if isinstance(proofs, np.ndarray) else proofs.numel() * proofs.element_size()
+        pp, mem = _ptr(proofs)
+        if n_proofs is None:
+            n_proofs = ln // (4 * self.fq_bytes * (1 if compressed else 2))
+        return proofs, pp, mem, ln, n_proofs
+
+    def groth16_verify_batch_bytes(self, pvk, inputs, n_inputs, proofs, compressed=True, n_proofs=None, ok=None, reason=None):
+        """One verdict per ark-serialized proof (b2s_groth16_verify_batch_bytes): `proofs` is a || b || c per proof, back to
+        back, decoded and validated on the GPU.  inputs as for groth16_verify_batch, in the same memory as `proofs`.  Returns
+        (ok, reason): a bool and a uint8 numpy array for HOST buffers (reason[i] = 0 when proof i decoded, else
+        16 (1 + element) + decode reason); for device buffers fills the uint8 tensors `ok` and `reason` (may be None)."""
+        proofs, pp, mem, ln, n_proofs = self._proof_buf(proofs, compressed, n_proofs)
+        px, mem_x = _ptr(inputs)
+        assert inputs is None or mem_x == mem
+        if mem == MEM_HOST:
+            out, rs = np.zeros(max(n_proofs, 1), dtype=np.uint8), np.zeros(max(n_proofs, 1), dtype=np.uint8)
+            self._ck(self.lib.b2s_groth16_verify_batch_bytes(self.h, pvk, n_proofs, px, n_inputs, pp, ln, int(compressed), mem,
+                                                             out.ctypes.data, rs.ctypes.data))
+            return out[:n_proofs].astype(bool), rs[:n_proofs]
+        po, _ = _ptr(ok)
+        pr, _ = _ptr(reason)
+        self._ck(self.lib.b2s_groth16_verify_batch_bytes(self.h, pvk, n_proofs, px, n_inputs, pp, ln, int(compressed), mem, po, pr))
+        return ok, reason
+
+    def groth16_verify_all_bytes(self, pvk, inputs, n_inputs, proofs, compressed=True, rho=None, n_proofs=None, reason=None):
+        """True when every ark-serialized proof decodes and the batch passes the random linear combination
+        (b2s_groth16_verify_batch_rlc_bytes).  Buffers as for groth16_verify_batch_bytes; rho as for groth16_verify_all (None
+        draws it with `secrets`).  Returns (verdict, reason): reason is a uint8 numpy array for HOST buffers, else the
+        device tensor `reason` passed in (may be None)."""
+        proofs, pp, mem, ln, n_proofs = self._proof_buf(proofs, compressed, n_proofs)
+        px, mem_x = _ptr(inputs)
+        assert inputs is None or mem_x == mem
+        if rho is None:
+            rho = random_rho(n_proofs)
+            if mem == MEM_DEVICE:
+                import torch
+
+                rho = torch.from_numpy(rho.view(np.int32)).to(proofs.device)
+        pr, mem_r = _ptr(rho)
+        assert n_proofs == 0 or mem_r == mem
+        if mem == MEM_HOST:
+            reason = np.zeros(max(n_proofs, 1), dtype=np.uint8)
+        prs, _ = _ptr(reason)
+        ok = ctypes.c_uint8(0)
+        self._ck(self.lib.b2s_groth16_verify_batch_rlc_bytes(self.h, pvk, n_proofs, px, n_inputs, pp, ln, int(compressed), pr, mem,
+                                                             ctypes.byref(ok), prs))
+        return bool(ok.value), (reason[:n_proofs] if mem == MEM_HOST else reason)
 
     def pairing(self, p, q, n=None, out=None):
         """e(P_i, Q_i) element-wise.  p, q: affine G1 / G2 arrays (HOST numpy, or CUDA torch tensors with `out` a device

@@ -12,7 +12,14 @@ ceiling is the 381-bit one; for BN254 the fraction is against the same figure).
 
 With --rlc the same batch, all valid, goes through groth16_verify_all (b2s_groth16_verify_batch_rlc, one verdict per
 batch) and groth16_verify_batch in alternation; the line reports both rates, their ratio, both kernel splits and the
-operation counts of both paths, and the batch with the broken proofs must be rejected."""
+operation counts of both paths, and the batch with the broken proofs must be rejected.
+
+With --bytes the batch is serialized (compressed ark Proofs, a || b || c) and goes through groth16_verify_batch_bytes
+(with --rlc: groth16_verify_all_bytes) in alternation with two alternatives on the same proofs: the points path on
+already-decoded points, and what a caller without the bytes path does -- split the bytes into three arrays, three validated
+deserialize_points calls, then the points path.  The line reports the three rates, the bytes path's kernel split with the
+decode kernels' share, and the decode operation count; a batch with malformed and invalid proofs must get the expected
+verdicts and reasons."""
 import argparse
 import json
 import os
@@ -76,6 +83,23 @@ def fq_mul_count_rlc(curve, nf=2, log_n=20):
     return int(miller + scalar + msm + product)
 
 
+def fq_mul_count_decode(curve):
+    """Fq multiplications of decoding one compressed proof with validation (verify_decode_g1 / _g2): the square roots are
+    powers to (p - 3) / 4 (bits - 1 squarings and popcount - 1 multiplications; the Fq2 root by the norm method takes one
+    for the norm and on average 1.5 for delta), the subgroup criteria are scalar multiplications by the endomorphism scalar
+    in XYZZ (dbl 10, add 14; x3 over Fq2): [|x|] twice per BLS12-381 G1 point, [|x|] / [6 x^2] once per G2 point, none for
+    BN254 G1 (cofactor 1).  Montgomery conversions and comparisons are left out."""
+    bls = curve == "bls12_381"
+    p = gp.BLS_P if bls else gp.BN_P
+    e = (p - 3) // 4
+    pw = (e.bit_length() - 1) + (bin(e).count("1") - 1)
+    k = gp.BLS_X_ABS if bls else 6 * gp.BN_X * gp.BN_X
+    smul = (k.bit_length() - 1) * 10 + (bin(k).count("1") - 1) * 14
+    g1 = pw + 4 + (2 * smul if bls else 0)
+    g2 = 2.5 * pw + 3 * 8 + 3 * smul
+    return int(2 * g1 + g2)
+
+
 def gpu_info():
     try:
         out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
@@ -94,7 +118,10 @@ def main():
     ap.add_argument("--mem", choices=["host", "device"], default="host")
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--rlc", action="store_true", help="time groth16_verify_all (one verdict per batch) against the per-proof path")
+    ap.add_argument("--bytes", action="store_true", help="time the serialized-proof path against decoded points and decode-to-host")
     args = ap.parse_args()
+    if args.bytes:
+        return main_bytes(args)
     if args.rlc:
         return main_rlc(args)
 
@@ -230,6 +257,108 @@ def main_rlc(args):
         "rlc_proofs_per_s": round(pps_rlc, 1), "per_proof_proofs_per_s": round(pps_pp, 1), "ratio": round(pps_rlc / pps_pp, 3),
         "split": split, "fq_mul_per_proof_rlc": muls_rlc, "fq_mul_per_proof": muls_pp,
         "count_ratio": round(muls_pp / muls_rlc, 3), "gpu": name, "power_limit": power, "invalid_rejected": len(broken) * reps,
+    }))
+    be.pvk_free(sim.pvk)
+    be.close()
+
+
+def main_bytes(args):
+    """One tiled batch of compressed proofs, all valid, through the bytes path, the points path on the decoded points and the
+    decode-to-host workflow in alternation (per proof, or with --rlc one verdict per batch); then a batch with one proof in
+    64 algebraically broken (A + G1) and one in 64 malformed (C's flag bit) must get the expected verdicts and reasons."""
+    from snark_b200 import Backend
+    from snark_b200.lib import random_rho
+    from tests.test_gpu_verify import Sim
+
+    if args.mem != "host":
+        raise SystemExit("--bytes times host batches")
+    be = Backend(curve=0 if args.curve == "bls12_381" else 1)
+    rng = random.Random(20)
+    sim = Sim(be, rng, args.n_inputs)
+    ni = args.n_inputs
+    base = 1 << min(12, args.log_n)
+    x, a, b = sim.scalars(rng, base)
+    c = sim.c_of(x, a, b)
+    n = 1 << args.log_n
+    reps = n // base
+    g1e, g2e = be.fq_bytes, 2 * be.fq_bytes   # compressed encodings
+
+    def encode(A_, B_, C_):
+        parts = [np.frombuffer(be.serialize_points(g, arr, base, True), dtype=np.uint8).reshape(base, -1)
+                 for g, arr in ((1, A_), (2, B_), (1, C_))]
+        return np.concatenate(parts, axis=1)
+
+    inputs, A0, B0, C0 = sim.arrays(x, a, b, c)
+    blob = np.tile(encode(A0, B0, C0), (reps, 1)).reshape(-1)
+    inputs = np.tile(inputs, reps) if inputs is not None else None
+    A, B, C = np.tile(A0, reps), np.tile(B0, reps), np.tile(C0, reps)
+    # the check batch: A + G1 at i = 0 mod 64, C's flag bit flipped at i = 32 mod 64
+    broken, malformed = set(range(0, base, 64)), set(range(32, base, 64))
+    A_bad = sim.arrays(x, [(v + 1) % sim.curve.r if i in broken else v for i, v in enumerate(a)], b, c)[1]
+    bad = encode(A_bad, B0, C0)
+    flag = (g1e + g2e) + (0 if be.curve == 0 else g1e - 1)
+    for i in malformed:
+        bad[i, flag] ^= 0x80 if be.curve == 0 else 0x40
+    bad = np.tile(bad, (reps, 1)).reshape(-1)
+    want_ok = np.tile(np.array([i not in broken and i not in malformed for i in range(base)]), reps)
+    want_reason = np.tile(np.array([48 + 1 if i in malformed else 0 for i in range(base)], dtype=np.uint8), reps)
+    rho = random_rho(n)
+
+    def split(data):   # what a caller does first without the bytes path: three contiguous arrays of encodings
+        rows = data.reshape(n, -1)
+        return rows[:, :g1e].copy(), rows[:, g1e:g1e + g2e].copy(), rows[:, g1e + g2e:].copy()
+
+    def decode_host(data):
+        ea, eb, ec = split(data)
+        return (be.deserialize_points(1, ea, n, True, True), be.deserialize_points(2, eb, n, True, True),
+                be.deserialize_points(1, ec, n, True, True))
+
+    if args.rlc:
+        paths = {
+            "bytes": lambda: be.groth16_verify_all_bytes(sim.pvk, inputs, ni, blob, rho=rho)[0],
+            "points": lambda: be.groth16_verify_all(sim.pvk, inputs, ni, A, B, C, rho=rho),
+            "decode_host": lambda: be.groth16_verify_all(sim.pvk, inputs, ni, *decode_host(blob), rho=rho),
+        }
+        verdict, reason = be.groth16_verify_all_bytes(sim.pvk, inputs, ni, bad, rho=rho)
+        assert not verdict and np.array_equal(reason, want_reason), "the batch with broken proofs must be rejected"
+    else:
+        paths = {
+            "bytes": lambda: bool(be.groth16_verify_batch_bytes(sim.pvk, inputs, ni, blob)[0].all()),
+            "points": lambda: bool(be.groth16_verify_batch(sim.pvk, inputs, ni, A, B, C).all()),
+            "decode_host": lambda: bool(be.groth16_verify_batch(sim.pvk, inputs, ni, *decode_host(blob)).all()),
+        }
+        ok, reason = be.groth16_verify_batch_bytes(sim.pvk, inputs, ni, bad)
+        assert np.array_equal(ok, want_ok) and np.array_equal(reason, want_reason), "verdicts differ from the expected ones"
+    for name, fn in paths.items():
+        assert fn(), name   # warm-up, and the all-valid check
+    times = {name: [] for name in paths}
+    for _ in range(args.steps):
+        for name, fn in paths.items():
+            t0 = time.perf_counter()
+            assert fn(), name
+            times[name].append(time.perf_counter() - t0)
+    be.profile(True)
+    t0 = time.perf_counter()
+    paths["bytes"]()
+    prof_s = time.perf_counter() - t0
+    rep = be.profile_report()
+    be.profile(False)
+    kern = {k: round(v[1], 3) for k, v in rep.items()}
+    decode_ms = sum(v for k, v in kern.items() if k.startswith("verify_decode"))
+    pps = {name: n / min(t) for name, t in times.items()}
+    muls_dec = fq_mul_count_decode(args.curve)
+    muls_ver = fq_mul_count_rlc(args.curve, log_n=args.log_n) if args.rlc else fq_mul_count(args.curve, ni)
+    name, power = gpu_info()
+    print(json.dumps({
+        "curve": args.curve, "n_proofs": n, "n_inputs": ni, "mem": "host", "mode": "rlc" if args.rlc else "per_proof",
+        "seconds": {k: [round(s, 4) for s in v] for k, v in times.items()},
+        "proofs_per_s": {k: round(v, 1) for k, v in pps.items()},
+        "bytes_vs_points": round(pps["bytes"] / pps["points"], 3), "bytes_vs_decode_host": round(pps["bytes"] / pps["decode_host"], 3),
+        "kernel_ms": kern, "decode_kernel_ms": round(decode_ms, 3), "decode_share": round(decode_ms / sum(kern.values()), 4),
+        "outside_kernels_ms": round(prof_s * 1e3 - sum(kern.values()), 3),
+        "fq_mul_per_proof_decode": muls_dec, "fq_mul_per_proof_verify": muls_ver,
+        "count_ratio": round(muls_ver / (muls_ver + muls_dec), 3), "gpu": name, "power_limit": power,
+        "invalid_checked": int((~want_ok).sum()),
     }))
     be.pvk_free(sim.pvk)
     be.close()
