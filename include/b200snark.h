@@ -189,6 +189,21 @@ int32_t b2s_groth16_prove(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, con
 /* Same, with z = instance || witness already resident on the GPU (n_instance + n_witness elements). */
 int32_t b2s_groth16_prove_resident(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void* r,
                                    const void* s, void* out_a_g1, void* out_b_g2, void* out_c_g1);
+/* n_proofs proofs under one full key in one call.  z: n_proofs rows of n_instance + n_witness Montgomery Fr, row i =
+ * proof i's instance || witness with z[0] = 1 (as b2s_groth16_prove_resident takes one); r, s: n_proofs Montgomery Fr each.
+ * Outputs: n_proofs affine A (G1), B (G2) and C (G1).  Every buffer is in `mem` (B2S_MEM_HOST or B2S_MEM_DEVICE).
+ * Proof i is bit-identical to b2s_groth16_prove on (z_i, r_i, s_i).  Errors as b2s_groth16_prove; n_proofs == 0 returns
+ * B2S_OK and writes nothing.  Host batches go through bounded device scratch in chunks, so n_proofs is not limited by device
+ * memory.  Within a chunk the witness maps and each of the five MSMs run batched, with the launches of one proof.  The batch
+ * MSMs do not use the multiplicity-aware front end of the single-proof path (repeated witness values, e.g. 0 / 1 heavy
+ * witnesses, cost the batch full Pippenger price).
+ * When to use which (H100 80GB HBM3, 400 W, DESIGN.md section 4): for 16 or more proofs at domains up to 2^16 the batch
+ * wins, 2.9x to 25x over a loop of b2s_groth16_prove_resident; at 2^20 it wins 1.1x (BLS12-381) / 1.5x (BN254) on uniform
+ * witnesses and LOSES (0.5x to 0.7x) on witnesses made of a few repeated values, where the loop's front end pays off; a
+ * single proof (n_proofs == 1) is 7 % to 17 % slower than b2s_groth16_prove_resident.  Large single proofs (2^20 and up with
+ * repeated witness values, 2^24) belong to the single-proof entry points. */
+int32_t b2s_groth16_prove_batch(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, uint64_t n_proofs, const void* z,
+                                const void* r, const void* s, int32_t mem, void* out_a_g1, void* out_b_g2, void* out_c_g1);
 /* Shard step for multi-GPU: computes this shard's five MSM partial sums
  *   out_partials = [ h_acc, l_acc, a_acc, b1_acc ] (4 G1 XYZZ) and out_b2_partial (1 G2 XYZZ), HOST.
  * r, s are needed here too: the shard that owns the end of a query range folds r*delta / s*delta into its MSMs. */

@@ -46,6 +46,9 @@ extern "C" {
     pub fn b2s_groth16_prove_group(group: *mut B2sGroup, pk_shard: *const B2sPk, m: *const B2sR1cs, z_inst: *const c_void,
                                    z_wit: *const c_void, r: *const c_void, s: *const c_void, out_a: *mut c_void,
                                    out_b: *mut c_void, out_c: *mut c_void) -> i32;
+    pub fn b2s_groth16_prove_batch(ctx: *mut B2sCtx, pk: *const B2sPk, m: *const B2sR1cs, n_proofs: u64, z: *const c_void,
+                                   r: *const c_void, s: *const c_void, mem: i32, out_a: *mut c_void, out_b: *mut c_void,
+                                   out_c: *mut c_void) -> i32;
     // CanonicalSerialize of the key types (snark/src/lib.rs:25-31)
     pub fn b2s_vk_serialized_size(ctx: *const B2sCtx, n_gamma_abc: u64, compressed: i32) -> u64;
     pub fn b2s_vk_serialize(ctx: *mut B2sCtx, alpha_g1: *const c_void, beta_g2: *const c_void, gamma_g2: *const c_void,
@@ -214,6 +217,37 @@ impl<E: Pairing> Groth16B200<E> {
         let mut pkh: *mut B2sPk = core::ptr::null_mut();
         check(ctx, unsafe { b2s_pk_deserialize(ctx, pk_bytes.as_ptr(), pk_bytes.len() as u64, compressed as i32, validate as i32, &mut pkh) })?;
         Ok(Resident { ctx, pk: pkh, mat })
+    }
+
+    /// `prove` for many circuits of one shape under one resident key, in one GPU call (b2s_groth16_prove_batch): each
+    /// circuit is synthesised on the host, r and s are drawn per proof in ark's order (r, then s, then synthesis), and
+    /// the witness maps and MSMs of the whole batch run batched on the GPU.  Proof i is the proof `prove` would give
+    /// with the same r and s.  Every circuit must have the matrices `res` was made for.
+    pub fn prove_batch<C: ConstraintSynthesizer<E::ScalarField>, R: RngCore + CryptoRng>(res: &Resident, circuits: Vec<C>, rng: &mut R)
+        -> Result<Vec<Proof<E>>, B200Error> {
+        let n = circuits.len();
+        let (mut z, mut r, mut s) = (Vec::new(), Vec::with_capacity(n), Vec::with_capacity(n));
+        let mut row = None;
+        for circuit in circuits {
+            r.push(E::ScalarField::rand(rng));
+            s.push(E::ScalarField::rand(rng));
+            let cs = ConstraintSystem::new_ref();
+            cs.set_optimization_goal(OptimizationGoal::Constraints);
+            circuit.generate_constraints(cs.clone())?;
+            cs.finalize();
+            let (zi, zw) = (cs.instance_assignment()?, cs.witness_assignment()?);
+            if *row.get_or_insert(zi.len() + zw.len()) != zi.len() + zw.len() { return Err(SynthesisError::AssignmentMissing.into()); }
+            z.extend_from_slice(&zi);
+            z.extend_from_slice(&zw);
+        }
+        let g1 = 2 * core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>();
+        let (mut a, mut b, mut c) = (vec![0u8; n * g1], vec![0u8; n * 2 * g1], vec![0u8; n * g1]);
+        check(res.ctx, unsafe {
+            b2s_groth16_prove_batch(res.ctx, res.pk, res.mat, n as u64, z.as_ptr().cast(), r.as_ptr().cast(), s.as_ptr().cast(),
+                                    0 /* B2S_MEM_HOST */, a.as_mut_ptr().cast(), b.as_mut_ptr().cast(), c.as_mut_ptr().cast())
+        })?;
+        Ok((0..n).map(|i| Proof { a: unpack_point::<E::G1Affine>(&a[i * g1..(i + 1) * g1]), b: unpack_point::<E::G2Affine>(&b[i * 2 * g1..(i + 1) * 2 * g1]),
+                                  c: unpack_point::<E::G1Affine>(&c[i * g1..(i + 1) * g1]) }).collect())
     }
 
     /// `verify_with_processed_vk` for many proofs under one key, one verdict per proof (`inputs[i]` belongs to

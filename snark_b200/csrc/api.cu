@@ -444,6 +444,16 @@ int32_t b2s_groth16_prove_resident(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1c
     return prove_full(ctx, pk, m, nullptr, nullptr, z_dev, r, s, out_a_g1, out_b_g2, out_c_g1);
 }
 
+int32_t b2s_groth16_prove_batch(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, uint64_t n_proofs, const void* z, const void* r,
+                                const void* s, int32_t mem, void* out_a_g1, void* out_b_g2, void* out_c_g1) {
+    LOCK(ctx);
+    if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove_batch: null key or matrices");
+    if (!z || !r || !s) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove_batch: null assignment");
+    if (!out_a_g1 || !out_b_g2 || !out_c_g1) return fail(ctx, B2S_ERR_INVALID_ARG, "prove_batch: null output");
+    if (!pk_is_full(pk)) return fail(ctx, B2S_ERR_MALFORMED_VK, "prove_batch: needs a full (unsharded) proving key");
+    return groth16_prove_batch(ctx, pk, m, n_proofs, z, r, s, mem, out_a_g1, out_b_g2, out_c_g1);
+}
+
 int32_t b2s_groth16_prove_shard_resident(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void* r,
                                          const void* s, void* out_g1_partials, void* out_g2_partial) {
     LOCK(ctx);

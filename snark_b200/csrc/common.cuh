@@ -209,6 +209,12 @@ void ntt_free_plans(Ctx* c);
 struct MsmPre { uint32_t c, nwin; uint32_t stride; };
 int32_t msm_run(Ctx* c, int group, const void* bases_dev, const void* scalars_dev, uint64_t n, bool scalars_mont,
                 void* out_xyzz_dev, void* wins_ext = nullptr, const MsmPre* pre = nullptr);
+// K scalar vectors over the same n bases (vector k at scalars_dev + k * stride scalars): out_xyzz_dev[k] = MSM of vector k.
+// One Pippenger problem on c->stream, so the launches do not grow with K; no multiplicity-aware front end.
+int32_t msm_run_batch(Ctx* c, int group, const void* bases_dev, const void* scalars_dev, uint64_t n, uint64_t stride, uint32_t K,
+                      bool scalars_mont, void* out_xyzz_dev, const MsmPre* pre = nullptr);
+// device bytes per vector of msm_run_batch over n points; *max_k = the most vectors its u32 indices allow
+uint64_t msm_batch_bytes(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint64_t* max_k);
 // table[w * n + i] = 2^(c w) bases[i] (affine), w < nwin; picks c / nwin for n points itself and reports them in *pre
 int32_t msm_precompute(Ctx* c, int group, const void* bases_dev, uint64_t n, void* table_dev, MsmPre* pre);
 uint32_t msm_precompute_windows(Ctx* c, uint64_t n, uint32_t* c_out);

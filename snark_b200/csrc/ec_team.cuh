@@ -5,8 +5,9 @@
 // a doubling is 3 multiplication latencies deep instead of 9, a general addition 4 instead of 14.  Same formulas as
 // ec.cuh (EFD xyzz dbl-2008-s-1 / add-2008-s, a = 0), same special cases, bit-identical results.
 //
-// Every lane of the warp must call these functions with the SAME operands (full-mask shuffles, warp-uniform branches);
-// teams are lanes {4k .. 4k+3}, the eight teams of a warp compute the same thing.
+// Teams are lanes {4k .. 4k+3}.  Every lane of a team must call these functions with the SAME operands (team-uniform
+// branches, shuffles masked to the team), so the eight teams of a warp may work on eight different points (the batched
+// Horner tail) or all compute the same thing.  team_scalar_mul fills its table from lane 0: there all teams of the warp agree.
 #pragma once
 #include "ec.cuh"
 
@@ -18,9 +19,10 @@ __device__ __forceinline__ F team_bcast(const F& v, uint32_t src) {
     F r;
     const uint32_t* s = reinterpret_cast<const uint32_t*>(&v);
     uint32_t* d = reinterpret_cast<uint32_t*>(&r);
-    const int from = (int)((threadIdx.x & 31u & ~3u) | src);
+    const uint32_t first = threadIdx.x & 31u & ~3u;
+    const unsigned team = 0xfu << first;
 #pragma unroll
-    for (uint32_t i = 0; i < sizeof(F) / 4; i++) d[i] = __shfl_sync(0xffffffffu, s[i], from);
+    for (uint32_t i = 0; i < sizeof(F) / 4; i++) d[i] = __shfl_sync(team, s[i], (int)(first | src));
     return r;
 }
 template <class F>

@@ -27,10 +27,11 @@ namespace b2s {
 
 // Warps 0, 1, 2 run the three remaining scalar multiplications side by side (4-bit windows, four-lane teams of
 // ec_team.cuh: a doubling costs 3 multiplication latencies instead of 9); warp 3 normalises A meanwhile.
+// One CTA per proof k = blockIdx.x: its sums are sums[j * gridDim.x + k] (j = h, l, a, b1), its r and s rs[k * rs_stride + 0 / 1].
 template <class Curve>
 __global__ void __launch_bounds__(128)
 groth16_epilogue_g1_kernel(const Affine<typename Curve::Fq>* consts /*alpha,beta,delta*/, const XYZZ<typename Curve::Fq>* sums /*h,l,a,b1*/,
-                           const typename Curve::Fr* rs, Affine<typename Curve::Fq>* out_a, Affine<typename Curve::Fq>* out_c) {
+                           const typename Curve::Fr* rs, uint64_t rs_stride, Affine<typename Curve::Fq>* out_a, Affine<typename Curve::Fq>* out_c) {
     using Fq = typename Curve::Fq;
     using Fr = typename Curve::Fr;
     using P = XYZZ<Fq>;
@@ -38,14 +39,19 @@ groth16_epilogue_g1_kernel(const Affine<typename Curve::Fq>* consts /*alpha,beta
     __shared__ P table[3][16];
     const int role = threadIdx.x >> 5;
     const bool lead = (threadIdx.x & 31) == 0;
+    sums += blockIdx.x;
+    const uint32_t K = gridDim.x;
+    rs += blockIdx.x * rs_stride;
+    out_a += blockIdx.x;
+    out_c += blockIdx.x;
     if (role == 0) {   // s * A,  A = alpha + a_acc
-        P a = sums[2];
+        P a = sums[2 * K];
         a.add_affine(consts[0]);
         Fr s = rs[1].from_mont();
         P v = team_scalar_mul(a, s.v, Fr::N, table[0]);
         if (lead) sh[0] = v;
     } else if (role == 1) {   // r * B1,  B1 = beta + b1_acc
-        P b = sums[3];
+        P b = sums[3 * K];
         b.add_affine(consts[1]);
         Fr r = rs[0].from_mont();
         P v = team_scalar_mul(b, r.v, Fr::N, table[1]);
@@ -55,7 +61,7 @@ groth16_epilogue_g1_kernel(const Affine<typename Curve::Fq>* consts /*alpha,beta
         P v = team_scalar_mul(P::from_affine(consts[2]), rsp.v, Fr::N, table[2]);
         if (lead) sh[2] = v;
     } else {   // A itself, normalised (one inversion) while the others multiply
-        P a = sums[2];
+        P a = sums[2 * K];
         a.add_affine(consts[0]);
         if (lead) *out_a = a.to_affine();
     }
@@ -64,19 +70,20 @@ groth16_epilogue_g1_kernel(const Affine<typename Curve::Fq>* consts /*alpha,beta
         P c = sh[0];
         team_add(c, sh[1]);
         team_add(c, sh[2].neg());
-        team_add(c, sums[1]);
+        team_add(c, sums[K]);
         team_add(c, sums[0]);
         if (lead) *out_c = c.to_affine();
     }
 }
 
+// one thread per proof: B = beta_2 + b2_acc[k], k = blockIdx.x
 template <class Curve>
 __global__ void groth16_epilogue_g2_kernel(const Affine<typename Curve::Fq2>* consts /*beta,delta*/,
                                            const XYZZ<typename Curve::Fq2>* b2_sum, Affine<typename Curve::Fq2>* out_b) {
     if (threadIdx.x != 0) return;
-    XYZZ<typename Curve::Fq2> acc = b2_sum[0];
+    XYZZ<typename Curve::Fq2> acc = b2_sum[blockIdx.x];
     acc.add_affine(consts[0]);
-    *out_b = acc.to_affine();
+    out_b[blockIdx.x] = acc.to_affine();
 }
 
 // sums[j] = sum over shards of partials[shard * stride + j], j < count
@@ -179,17 +186,22 @@ struct ReplicatedH : HSource {
     }
 };
 
+static int32_t pk_matches(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m) {
+    const uint64_t N = 1ull << m->log_domain;
+    if (pk->n_instance != m->n_instance || pk->n_witness != m->n_witness || pk->domain_size != N)
+        return fail(c, B2S_ERR_ASSIGNMENT_MISSING, "prove: key (%llu,%llu,%llu) does not match matrices (%llu,%llu,%llu)",
+                    (unsigned long long)pk->n_instance, (unsigned long long)pk->n_witness, (unsigned long long)pk->domain_size,
+                    (unsigned long long)m->n_instance, (unsigned long long)m->n_witness, (unsigned long long)N);
+    return B2S_OK;
+}
+
 template <class Curve>
 static int32_t shard_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* z_inst, const void* z_wit, const void* z_dev,
                        const void* r_host, const void* s_host, void* g1_out, void* g2_out, HSource* hs) {
     using Fr = typename Curve::Fr;
     using P1 = XYZZ<typename Curve::Fq>;
     using P2 = XYZZ<typename Curve::Fq2>;
-    const uint64_t N = 1ull << m->log_domain;
-    if (pk->n_instance != m->n_instance || pk->n_witness != m->n_witness || pk->domain_size != N)
-        return fail(c, B2S_ERR_ASSIGNMENT_MISSING, "prove: key (%llu,%llu,%llu) does not match matrices (%llu,%llu,%llu)",
-                    (unsigned long long)pk->n_instance, (unsigned long long)pk->n_witness, (unsigned long long)pk->domain_size,
-                    (unsigned long long)m->n_instance, (unsigned long long)m->n_witness, (unsigned long long)N);
+    B2S_TRY(pk_matches(c, pk, m));
     const uint64_t n_vars = m->n_instance + m->n_witness;
     // z_ext = z ++ [r, s]
     DevBuf z, tails;
@@ -257,6 +269,96 @@ int32_t groth16_shard(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* z
     });
 }
 
+// ---- many proofs under one key -----------------------------------------------------------------------------------------
+// Proofs per chunk at most (DESIGN.md section 4): at domain 2^12 proofs/s still grow from 64 to 256 proofs (799 -> 991 on
+// BLS12-381), at 2^16 they are flat from 16 on.  Free memory and the u32 entry limits of the MSM lower it at larger domains.
+static constexpr uint64_t PROVE_BATCH_CAP = 256;
+
+// The chunk's K assignments sit on the device as rows z_k ++ [r_k, s_k] of n_vars + 2 scalars, so that each MSM of shard_t
+// becomes one batched MSM over the same bases (scalar stride n_vars + 2; h at stride N), the witness map runs once for all K,
+// and the epilogue runs one CTA per proof.  No multiplicity-aware front end: the batched MSMs see every scalar.
+template <class Curve>
+static int32_t prove_batch_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, uint64_t n_proofs, const void* z, const void* r, const void* s,
+                             int32_t mem, void* out_a, void* out_b, void* out_c) {
+    using Fr = typename Curve::Fr;
+    using Fq = typename Curve::Fq;
+    using Fq2 = typename Curve::Fq2;
+    using P1 = XYZZ<Fq>;
+    using P2 = XYZZ<Fq2>;
+    using A1 = Affine<Fq>;
+    using A2 = Affine<Fq2>;
+    B2S_TRY(pk_matches(c, pk, m));
+    if (n_proofs == 0) return B2S_OK;
+    const uint64_t N = 1ull << m->log_domain;
+    const uint64_t n_vars = m->n_instance + m->n_witness, row = n_vars + 2;
+    const MsmPre* h_pre = pk->h_table.p ? &pk->h_pre : nullptr;
+    // per proof: its row, the witness map (h, two more vectors, transform scratch), sums and outputs, the largest MSM
+    uint64_t max_k = PROVE_BATCH_CAP, msm_bytes = 0;
+    for (int w = 0; w < PK_QUERIES; w++) {
+        uint64_t mk = 0;
+        msm_bytes = std::max(msm_bytes, msm_batch_bytes(c, PK_QUERY[w].group, pk->q[w].len + pk->q[w].ext, w == Q_H ? h_pre : nullptr, &mk));
+        max_k = std::min(max_k, mk);
+    }
+    const uint64_t per_proof = row * sizeof(Fr) + 4 * N * sizeof(Fr) + msm_bytes + 4 * sizeof(P1) + sizeof(P2) + 2 * sizeof(A1) + sizeof(A2);
+    size_t free_b = 0, total_b = 0;
+    B2S_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
+    max_k = std::max<uint64_t>(1, std::min<uint64_t>(max_k, free_b / 2 / per_proof));
+    const uint32_t ch = (uint32_t)std::min<uint64_t>(max_k, n_proofs);
+    const bool host = mem != B2S_MEM_DEVICE;
+    const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    DevBuf zb, h, sums1, sums2, outs;
+    B2S_TRY(zb.alloc(c, (size_t)ch * row * sizeof(Fr)));
+    B2S_TRY(sums1.alloc(c, (size_t)4 * ch * sizeof(P1)));
+    B2S_TRY(sums2.alloc(c, (size_t)ch * sizeof(P2)));
+    if (host) B2S_TRY(outs.alloc(c, (size_t)ch * (2 * sizeof(A1) + sizeof(A2))));
+    Fr* zd = zb.as<Fr>();
+    const size_t fr = sizeof(Fr);
+    for (uint64_t p0 = 0; p0 < n_proofs; p0 += ch) {
+        const uint32_t K = (uint32_t)std::min<uint64_t>(ch, n_proofs - p0);
+        B2S_CUDA(c, cudaMemcpy2DAsync(zd, row * fr, static_cast<const char*>(z) + p0 * n_vars * fr, n_vars * fr, n_vars * fr, K, kind, c->stream));
+        B2S_CUDA(c, cudaMemcpy2DAsync(zd + n_vars, row * fr, static_cast<const char*>(r) + p0 * fr, fr, fr, K, kind, c->stream));
+        B2S_CUDA(c, cudaMemcpy2DAsync(zd + n_vars + 1, row * fr, static_cast<const char*>(s) + p0 * fr, fr, fr, K, kind, c->stream));
+        P1* g1 = sums1.as<P1>();   // [h | l | a | b1] x K, the layout the epilogue reads
+        auto msm = [&](int w, void* out, const void* scalars, uint64_t stride, const void* bases = nullptr, const MsmPre* pre = nullptr) {
+            const PkQuery& q = pk->q[w];
+            return msm_run_batch(c, PK_QUERY[w].group, bases ? bases : q.pts.p, scalars, q.len + q.ext, stride, K, true, out, pre);
+        };
+        auto from_z = [&](int w) { return zd + (PK_QUERY[w].scalars == FROM_WITNESS ? m->n_instance : 0) + pk->q[w].off; };
+        B2S_TRY(msm(Q_B_G2, sums2.p, from_z(Q_B_G2), row));
+        B2S_TRY(msm(Q_A, g1 + 2 * K, from_z(Q_A), row));
+        B2S_TRY(msm(Q_B_G1, g1 + 3 * K, from_z(Q_B_G1), row));
+        B2S_TRY(msm(Q_L, g1 + 1 * K, from_z(Q_L), row));
+        {
+            B2S_TRY(h.alloc(c, (size_t)K * N * fr));
+            B2S_TRY(witness_map_run(c, m, zd, h.p, K, row));
+            const Fr* hs = h.as<Fr>() + pk->q[Q_H].off;
+            if (h_pre) B2S_TRY(msm(Q_H, g1, hs, N, pk->h_table.p, h_pre));
+            else B2S_TRY(msm(Q_H, g1, hs, N));
+            h.release();
+        }
+        char* oa = host ? outs.as<char>() : static_cast<char*>(out_a) + p0 * sizeof(A1);
+        char* oc = host ? outs.as<char>() + (size_t)K * sizeof(A1) : static_cast<char*>(out_c) + p0 * sizeof(A1);
+        char* ob = host ? outs.as<char>() + (size_t)2 * K * sizeof(A1) : static_cast<char*>(out_b) + p0 * sizeof(A2);
+        B2S_LAUNCH(c, groth16_epilogue_g1_kernel<Curve>, K, 128, 0, pk->consts_g1.as<A1>(), (const P1*)g1, (const Fr*)(zd + n_vars), row,
+                   reinterpret_cast<A1*>(oa), reinterpret_cast<A1*>(oc));
+        B2S_LAUNCH(c, groth16_epilogue_g2_kernel<Curve>, K, 32, 0, pk->consts_g2.as<A2>(), sums2.as<P2>(), reinterpret_cast<A2*>(ob));
+        if (host) {
+            B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(out_a) + p0 * sizeof(A1), oa, K * sizeof(A1), cudaMemcpyDeviceToHost, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(out_c) + p0 * sizeof(A1), oc, K * sizeof(A1), cudaMemcpyDeviceToHost, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(out_b) + p0 * sizeof(A2), ob, K * sizeof(A2), cudaMemcpyDeviceToHost, c->stream));
+        }
+    }
+    B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+    return B2S_OK;
+}
+
+int32_t groth16_prove_batch(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, uint64_t n_proofs, const void* z, const void* r, const void* s,
+                            int32_t mem, void* out_a, void* out_b, void* out_c) {
+    return dispatch_curve(c, [&](auto curve) {
+        return prove_batch_t<decltype(curve)>(c, pk, m, n_proofs, z, r, s, mem, out_a, out_b, out_c);
+    });
+}
+
 // g1_partials: shard i's four G1 sums start at element i * g1_stride (XYZZ<Fq> units); g2_partials likewise (XYZZ<Fq2>)
 template <class Curve>
 static int32_t finish_t(Ctx* c, const b2s_pk* pk, const void* g1_partials, uint32_t g1_stride, const void* g2_partials, uint32_t g2_stride,
@@ -275,7 +377,7 @@ static int32_t finish_t(Ctx* c, const b2s_pk* pk, const void* g1_partials, uint3
     const size_t g1 = sizeof(Affine<Fq>), g2 = sizeof(Affine<Fq2>);
     B2S_TRY(outs.alloc(c, 2 * g1 + g2));
     char* o = outs.as<char>();
-    B2S_LAUNCH(c, groth16_epilogue_g1_kernel<Curve>, 1, 128, 0, pk->consts_g1.as<Affine<Fq>>(), sums1.as<XYZZ<Fq>>(), rs.as<Fr>(),
+    B2S_LAUNCH(c, groth16_epilogue_g1_kernel<Curve>, 1, 128, 0, pk->consts_g1.as<Affine<Fq>>(), sums1.as<XYZZ<Fq>>(), rs.as<Fr>(), (uint64_t)2,
                reinterpret_cast<Affine<Fq>*>(o), reinterpret_cast<Affine<Fq>*>(o + g1));
     B2S_LAUNCH(c, groth16_epilogue_g2_kernel<Curve>, 1, 32, 0, pk->consts_g2.as<Affine<Fq2>>(), sums2.as<XYZZ<Fq2>>(),
                reinterpret_cast<Affine<Fq2>*>(o + 2 * g1));

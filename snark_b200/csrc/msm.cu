@@ -81,18 +81,21 @@ __device__ __forceinline__ void load_scalar(DigitIter& it, const Fr* scalars, ui
 // Histogram of (window, |digit|).  Lanes of a warp that hit the same bucket are combined with
 // match.any so that skewed scalar distributions (all-equal witnesses, many 0/1 values) issue one
 // atomic per distinct bucket per warp instead of 32 to the same address.
+// Batch: blockIdx.y is the scalar vector k (at scalars + k * stride); its windows are the super-windows k * nwin + w
+// (k alone with a precomputed table) of B buckets each.
 template <class Fr>
-__global__ void msm_count_kernel(const Fr* __restrict__ scalars, uint64_t n, bool mont, MsmShape sh,
+__global__ void msm_count_kernel(const Fr* __restrict__ scalars, uint64_t n, uint64_t stride, bool mont, MsmShape sh,
                                  uint32_t* __restrict__ counts) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const unsigned active = __activemask();
     const unsigned lane = threadIdx.x & 31;
+    const uint32_t win0 = blockIdx.y * (sh.pre_stride ? 1u : sh.nwin);
     DigitIter it;
-    load_scalar(it, scalars, i, mont);
+    load_scalar(it, scalars + blockIdx.y * stride, i, mont);
     for (uint32_t w = 0; w < sh.nwin; w++) {
         const int32_t d = it.next(w, sh.c, sh.nwin);
-        const uint32_t key = d != 0 ? (sh.pre_stride ? 0u : w * sh.B) + (uint32_t)(d < 0 ? -d : d) - 1 : 0xffffffffu;
+        const uint32_t key = d != 0 ? (sh.pre_stride ? win0 : win0 + w) * sh.B + (uint32_t)(d < 0 ? -d : d) - 1 : 0xffffffffu;
         const unsigned peers = __match_any_sync(active, key);
         if (key != 0xffffffffu && lane == (unsigned)(__ffs(peers) - 1)) atomicAdd(&counts[key], (uint32_t)__popc(peers));
     }
@@ -311,11 +314,12 @@ __device__ void block_excl_scan(const uint32_t* in, uint32_t* out, uint32_t n) {
 }
 
 // Pass 1.  Scalars are kept canonical in shared memory, word-major, so that each window reads its two words without bank
-// conflicts and the recoding carry walks the windows in order.
+// conflicts and the recoding carry walks the windows in order.  Batch: blockIdx.y is the scalar vector k, as in the count
+// kernel; a tile never straddles two vectors, and its entries keep the base index because the vectors share the bases.
 template <class Fr>
 __global__ void __launch_bounds__(SORT_THREADS, 1)
-msm_partition_kernel(const Fr* __restrict__ scalars, const uint32_t* __restrict__ index_map, uint64_t n, bool mont, MsmShape sh, uint32_t F,
-                     const uint32_t* __restrict__ offsets, uint32_t* __restrict__ bin_cursor, uint32_t* __restrict__ part_val,
+msm_partition_kernel(const Fr* __restrict__ scalars, const uint32_t* __restrict__ index_map, uint64_t n, uint64_t stride, bool mont, MsmShape sh,
+                     uint32_t F, const uint32_t* __restrict__ offsets, uint32_t* __restrict__ bin_cursor, uint32_t* __restrict__ part_val,
                      uint16_t* __restrict__ part_fine) {
     extern __shared__ uint4 sort_smem[];
     const uint32_t nbw = sh.B >> F;                          // coarse bins per window
@@ -333,7 +337,7 @@ msm_partition_kernel(const Fr* __restrict__ scalars, const uint32_t* __restrict_
         const uint32_t s = threadIdx.x + j * SORT_THREADS;
         if (s < cnt) {
             DigitIter it;
-            load_scalar(it, scalars, tile + s, mont);
+            load_scalar(it, scalars + blockIdx.y * stride, tile + s, mont);
 #pragma unroll
             for (int q = 0; q < 8; q++) sc[q * SORT_TILE + s] = it.k[q];
             base[j] = index_map ? index_map[tile + s] : (uint32_t)(tile + s);
@@ -365,7 +369,7 @@ msm_partition_kernel(const Fr* __restrict__ scalars, const uint32_t* __restrict_
         }
         __syncthreads();
         block_excl_scan(hist, start, nbw);
-        const uint32_t bin0 = sh.pre_stride ? 0u : w * nbw;
+        const uint32_t bin0 = (sh.pre_stride ? blockIdx.y : blockIdx.y * sh.nwin + w) * nbw;
         for (uint32_t b = threadIdx.x; b < nbw; b += SORT_THREADS) {
             const uint32_t k = hist[b];
             if (k) dest[b] = offsets[(bin0 + b) << F] + atomicAdd(&bin_cursor[bin0 + b], k) - start[b];
@@ -565,12 +569,13 @@ static uint32_t env_u32(const char* name, uint32_t dflt) {
 
 // Window size: minimise  n * nwin  (bucket accumulation, mixed additions)  +  nwin * 2^(c-1) * 4.7
 // (bucket reduction: two general additions per bucket at ~1.4x the cost of a mixed one, plus the
-// per-segment double-and-add), subject to the bucket array staying under 4 GiB.
-static MsmShape msm_shape(uint64_t n, uint32_t scalar_bits, size_t point_bytes, const MsmPre* pre = nullptr) {
+// per-segment double-and-add), subject to the bucket array staying under 4 GiB.  A batch of K scalar vectors keeps the
+// window size of one (the cost per vector is the same) and has K times the buckets and entries.
+static MsmShape msm_shape(uint64_t n, uint32_t scalar_bits, size_t point_bytes, const MsmPre* pre = nullptr, uint32_t K = 1) {
     MsmShape sh{};
     if (pre) {      // the table fixes c; all windows share one bucket set
-        sh.c = pre->c; sh.nwin = pre->nwin; sh.B = 1u << (pre->c - 1); sh.G = sh.B; sh.pre_stride = pre->stride;
-        const uint64_t t_upper = (uint64_t)sh.nwin * n;
+        sh.c = pre->c; sh.nwin = pre->nwin; sh.B = 1u << (pre->c - 1); sh.G = K * sh.B; sh.pre_stride = pre->stride;
+        const uint64_t t_upper = (uint64_t)K * sh.nwin * n;
         sh.L = (uint32_t)std::max<uint64_t>(64, t_upper >> 18);
         sh.max_tasks = t_upper / sh.L + sh.G + 1;
         return sh;
@@ -596,8 +601,8 @@ static MsmShape msm_shape(uint64_t n, uint32_t scalar_bits, size_t point_bytes, 
     sh.c = c;
     sh.nwin = nwin_of(c);
     sh.B = 1u << (c - 1);
-    sh.G = sh.nwin * sh.B;
-    const uint64_t t_upper = (uint64_t)sh.nwin * n;
+    sh.G = K * sh.nwin * sh.B;
+    const uint64_t t_upper = (uint64_t)K * sh.nwin * n;
     uint64_t L = t_upper >> 18;
     if (L < 64) L = 64;
     L = env_u32("B2S_MSM_L", (uint32_t)L);
@@ -779,20 +784,23 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
 // ---- the Pippenger pipeline proper ---------------------------------------------------------------------------------
 // index_map (optional): scalar i belongs to base index_map[i] (the multiplicity-aware front end hands over a compacted
 // scalar array); nullptr: base i.
+// K > 1: K scalar vectors (vector k at scalars + k * stride) over the same n bases, out[k] = MSM of vector k.  They run as one
+// Pippenger problem whose bucket key is (vector, window, digit): K * nwin super-windows of B buckets (K with a table).
 template <class Curve, class F>
 static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::Fr* scalars, const uint32_t* index_map, uint64_t n, bool mont,
-                          XYZZ<F>* out, void* wins_ext, bool* used_aux = nullptr, const MsmPre* pre = nullptr) {
+                          XYZZ<F>* out, void* wins_ext, bool* used_aux = nullptr, const MsmPre* pre = nullptr, uint32_t K = 1, uint64_t stride = 0) {
     using Fr = typename Curve::Fr;
     using Pt = XYZZ<F>;
     constexpr bool is_g1 = sizeof(F) == sizeof(typename Curve::Fq);
     if (n == 0) {
-        B2S_CUDA(c, cudaMemsetAsync(out, 0, sizeof(Pt), c->stream));
+        B2S_CUDA(c, cudaMemsetAsync(out, 0, K * sizeof(Pt), c->stream));
         return B2S_OK;
     }
-    MsmShape sh = msm_shape(n, Curve::FrP::BITS, sizeof(Pt), pre);
-    if ((uint64_t)sh.nwin * n >= (1ull << 32)) return fail(c, B2S_ERR_INVALID_ARG, "msm: n * windows exceeds 2^32");
+    MsmShape sh = msm_shape(n, Curve::FrP::BITS, sizeof(Pt), pre, K);
+    if ((uint64_t)K * sh.nwin * n >= (1ull << 32) || (uint64_t)K * sh.nwin * sh.B >= (1ull << 32))
+        return fail(c, B2S_ERR_INVALID_ARG, "msm: vectors * n * windows exceeds 2^32");
     if (pre && (uint64_t)pre->nwin * pre->stride >= (1ull << 31)) return fail(c, B2S_ERR_INVALID_ARG, "msm: precomputed table exceeds 2^31 points");
-    const RoundPlan rp = plan_rounds<F>(c, (uint64_t)sh.nwin * n, sh.G, is_g1, sh.L);
+    const RoundPlan rp = plan_rounds<F>(c, (uint64_t)K * sh.nwin * n, sh.G, is_g1, sh.L);
     sh.L = rp.L; sh.max_tasks = rp.max_tasks;
     const uint32_t MSM_SEG = sh.B >= (1u << 16) ? 32u : 16u;
     const uint32_t ntiles = (sh.G + SCAN_TILE - 1) / SCAN_TILE;
@@ -807,19 +815,20 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
     uint32_t* task_off = offsets + sh.G + 1;
     uint32_t* heavy = task_off + sh.G + 1;
     B2S_CUDA(c, cudaMemsetAsync(counts, 0, (size_t)2 * sh.G * sizeof(uint32_t), c->stream));
-    B2S_TRY(sorted.alloc(c, (size_t)sh.nwin * n * sizeof(uint32_t)));
+    const uint64_t T = (uint64_t)K * sh.nwin * n;
+    B2S_TRY(sorted.alloc(c, (size_t)T * sizeof(uint32_t)));
     B2S_TRY(bucket_acc.alloc(c, (size_t)sh.G * sizeof(Pt)));
     B2S_CUDA(c, cudaMemsetAsync(bucket_acc.p, 0, (size_t)sh.G * sizeof(Pt), c->stream));  // identity = zeros
     const uint32_t segs_per_win = (sh.B + MSM_SEG - 1) / MSM_SEG;
-    // what the bucket reduction and the Horner tail see: nwin windows of B buckets, or ONE with a precomputed table
+    // what the bucket reduction and the Horner tail see: K * nwin windows of B buckets, or K with a precomputed table
     MsmShape sh_red = sh;
-    if (pre) sh_red.nwin = 1;
+    sh_red.nwin = K * (pre ? 1u : sh.nwin);
     B2S_TRY(segs.alloc(c, (size_t)segs_per_win * sh_red.nwin * sizeof(Pt)));
-    if (sh.nwin > 64) wins_ext = nullptr;   // caller scratch holds 64 window sums; tiny windows take the in-stream path
-    if (!wins_ext) B2S_TRY(wins.alloc(c, (size_t)sh.nwin * sizeof(Pt)));
+    if (sh.nwin > 64 || K > 1) wins_ext = nullptr;   // caller scratch holds 64 window sums; tiny windows take the in-stream path
+    if (!wins_ext) B2S_TRY(wins.alloc(c, (size_t)std::max(sh.nwin, sh_red.nwin) * sizeof(Pt)));
     Pt* wins_p = wins_ext ? reinterpret_cast<Pt*>(wins_ext) : wins.as<Pt>();
 
-    B2S_LAUNCH(c, msm_count_kernel<Fr>, cdiv(n, 256), 256, 0, scalars, n, mont, sh, counts);
+    B2S_LAUNCH(c, msm_count_kernel<Fr>, dim3(cdiv(n, 256), K), 256, 0, scalars, n, stride, mont, sh, counts);
     const uint32_t* no_perm = nullptr;
     B2S_LAUNCH(c, msm_scan_tiles_kernel, ntiles, SCAN_THREADS, 0, counts, no_perm, sh, tiles.as<Scan3>());
     B2S_LAUNCH(c, msm_scan_spine_kernel, 1, 1024, 0, tiles.as<Scan3>(), ntiles, sh, offsets, task_off, heavy);
@@ -827,7 +836,6 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
     {
         // the partitioned entries (u32 value + u16 fine key) go back to the pool before bucket_sums_t allocates its rounds
         const uint32_t fine_bits = sort_fine_bits(sh.c), nbins = sh.G >> fine_bits, nbw = sh.B >> fine_bits;
-        const uint64_t T = (uint64_t)sh.nwin * n;
         DevBuf part;
         B2S_TRY(part.alloc(c, (size_t)T * (sizeof(uint32_t) + sizeof(uint16_t)) + (size_t)nbins * sizeof(uint32_t)));
         uint32_t* part_val = part.as<uint32_t>();
@@ -836,22 +844,22 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
         B2S_CUDA(c, cudaMemsetAsync(bin_cursor, 0, (size_t)nbins * sizeof(uint32_t), c->stream));
         B2S_SMEM_ATTR(c, msm_partition_kernel<Fr>, partition_smem(nbw));
         B2S_SMEM_ATTR(c, msm_place_kernel, place_smem(fine_bits));
-        B2S_LAUNCH(c, msm_partition_kernel<Fr>, cdiv(n, SORT_TILE), SORT_THREADS, partition_smem(nbw), scalars, index_map, n, mont, sh, fine_bits,
-                   (const uint32_t*)offsets, bin_cursor, part_val, part_fine);
+        B2S_LAUNCH(c, msm_partition_kernel<Fr>, dim3(cdiv(n, SORT_TILE), K), SORT_THREADS, partition_smem(nbw), scalars, index_map, n, stride, mont, sh,
+                   fine_bits, (const uint32_t*)offsets, bin_cursor, part_val, part_fine);
         B2S_LAUNCH(c, msm_place_kernel, nbins + c->sm_count, SORT_THREADS, place_smem(fine_bits), (const uint32_t*)offsets, nbins, fine_bits,
                    (const uint32_t*)part_val, (const uint16_t*)part_fine, cursor, sorted.as<uint32_t>());
     }
-    B2S_TRY((bucket_sums_t<Curve, F>(c, bases, sorted.as<uint32_t>(), counts, offsets, (uint64_t)sh.nwin * n, sh.G, rp, bucket_acc.as<Pt>())));
+    B2S_TRY((bucket_sums_t<Curve, F>(c, bases, sorted.as<uint32_t>(), counts, offsets, T, sh.G, rp, bucket_acc.as<Pt>())));
     // bucket reduction: compiled with the multiplication inlined (msm_acc_g1.cu), 2 general additions per bucket
     if (is_g1) B2S_TRY(msm_bucket_reduce_g1(c, bucket_acc.p, sh_red, MSM_SEG, segs.p, segs_per_win, wins_p));
     else B2S_TRY(msm_bucket_reduce_g2(c, bucket_acc.p, sh_red, MSM_SEG, segs.p, segs_per_win, wins_p));
     if (!wins_ext) {
-        B2S_TRY(msm_horner(c, c->stream, is_g1 ? 1 : 2, wins_p, sh_red, out));
+        B2S_TRY(msm_horner(c, c->stream, is_g1 ? 1 : 2, wins_p, sh_red, K, out));
     } else {
         // tail on the aux stream: it only needs the window sums, the main stream goes on with the next MSM
         B2S_CUDA(c, cudaEventRecord(c->ev_tail, c->stream));
         B2S_CUDA(c, cudaStreamWaitEvent(c->aux, c->ev_tail, 0));
-        B2S_TRY(msm_horner(c, c->aux, is_g1 ? 1 : 2, wins_p, sh_red, out));
+        B2S_TRY(msm_horner(c, c->aux, is_g1 ? 1 : 2, wins_p, sh_red, K, out));
         c->aux_pending = true;
         if (used_aux) *used_aux = true;
     }
@@ -1157,6 +1165,37 @@ int32_t msm_run(Ctx* c, int group, const void* bases_dev, const void* scalars_de
         if (group == 1) return msm_run_t<C, typename C::Fq>(c, bases_dev, scalars_dev, n, scalars_mont, out_xyzz_dev, wins_ext, pre);
         return msm_run_t<C, typename C::Fq2>(c, bases_dev, scalars_dev, n, scalars_mont, out_xyzz_dev, wins_ext, pre);
     });
+}
+
+int32_t msm_run_batch(Ctx* c, int group, const void* bases_dev, const void* scalars_dev, uint64_t n, uint64_t stride, uint32_t K,
+                      bool scalars_mont, void* out_xyzz_dev, const MsmPre* pre) {
+    if (n >= (1ull << 31)) return fail(c, B2S_ERR_INVALID_ARG, "msm: n = %llu exceeds 2^31 - 1", (unsigned long long)n);
+    return dispatch_curve(c, [&](auto curve) {
+        using C = decltype(curve);
+        const auto* s = reinterpret_cast<const typename C::Fr*>(scalars_dev);
+        if (group == 1) {
+            using F = typename C::Fq;
+            return msm_core_t<C, F>(c, reinterpret_cast<const Affine<F>*>(bases_dev), s, nullptr, n, scalars_mont, reinterpret_cast<XYZZ<F>*>(out_xyzz_dev),
+                                    nullptr, nullptr, pre, K, stride);
+        }
+        using F = typename C::Fq2;
+        return msm_core_t<C, F>(c, reinterpret_cast<const Affine<F>*>(bases_dev), s, nullptr, n, scalars_mont, reinterpret_cast<XYZZ<F>*>(out_xyzz_dev),
+                                nullptr, nullptr, pre, K, stride);
+    });
+}
+
+// Per vector of a batch: device bytes of an MSM over n points, and how many vectors the u32 entry and bucket indices allow.
+uint64_t msm_batch_bytes(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint64_t* max_k) {
+    const Sizes z = sizes(c);
+    const uint32_t bits = c->curve == B2S_CURVE_BLS12_381 ? 255 : 254;
+    const size_t pt = z.xyzz(group);
+    const MsmShape sh = msm_shape(std::max<uint64_t>(n, 1), bits, pt, pre);
+    const uint64_t T = (uint64_t)sh.nwin * n, G = sh.G;
+    *max_k = std::max<uint64_t>(1, std::min(((1ull << 32) - 1) / std::max<uint64_t>(T, 1), ((1ull << 32) - 1) / G));
+    // buckets with their five u32 arrays and segment sums; per entry the sorted index, the partitioned entry, the task
+    // partials, and the scratch of the batched-affine rounds (half the entries: 1.5 affine points and one field element each)
+    const uint64_t fe = z.aff(group) / 2;
+    return G * (pt + 5 * sizeof(uint32_t)) + T * (sizeof(uint32_t) * 2 + sizeof(uint16_t)) + (T / 16 + G) * pt + T * (3 * fe + fe) / 2;
 }
 
 // ---- fixed-base window precomputation for a resident key ----------------------------------------------------------------

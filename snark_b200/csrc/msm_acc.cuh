@@ -118,16 +118,21 @@ msm_accumulate_kernel(const Affine<F>* __restrict__ bases, const uint32_t* __res
 
 
 // result = sum_w 2^(c w) S_w  (Horner from the top window): ~250 dependent doublings, the longest serial chain of an MSM.
-// One warp; the four-lane teams of ec_team.cuh cut a doubling from 9 multiplication latencies to 3.
+// The four-lane teams of ec_team.cuh cut a doubling from 9 multiplication latencies to 3.  A batch of K MSMs has
+// sh.nwin = K * (windows per MSM); team k of the grid (eight per warp) folds MSM k's windows into out[k].
 template <class F>
-__global__ void __launch_bounds__(32) msm_horner_kernel(const XYZZ<F>* __restrict__ win, MsmShape sh, XYZZ<F>* __restrict__ out) {
-    XYZZ<F> acc = ld_struct(win + (sh.nwin - 1));
-    for (uint32_t w = sh.nwin - 1; w-- > 0;) {
+__global__ void __launch_bounds__(32) msm_horner_kernel(const XYZZ<F>* __restrict__ win, MsmShape sh, uint32_t K, XYZZ<F>* __restrict__ out) {
+    const uint32_t k = (blockIdx.x * blockDim.x + threadIdx.x) >> 2;
+    if (k >= K) return;
+    const uint32_t nw = sh.nwin / K;
+    win += (size_t)k * nw;
+    XYZZ<F> acc = ld_struct(win + (nw - 1));
+    for (uint32_t w = nw - 1; w-- > 0;) {
         for (uint32_t i = 0; i < sh.c; i++) team_dbl(acc);
         XYZZ<F> v = ld_struct(win + w);
         team_add(acc, v);
     }
-    if (threadIdx.x == 0) st_struct(out, acc);
+    if ((threadIdx.x & 3) == 0) st_struct(out + k, acc);
 }
 
 // Sum `count` XYZZ points with one CTA; result in out[0] (also used by the join of shard partials).
@@ -214,10 +219,10 @@ int32_t msm_bucket_reduce_g2(Ctx* c, const void* bucket_acc, MsmShape sh, uint32
 // launches compiled with the multiplication inlined: msm_acc_g1.cu (G1) and msm_acc_g2.cu (G2)
 int32_t msm_accumulate_g2(Ctx* c, const void* bases, const uint32_t* sorted, const uint32_t* offsets,
                           const uint32_t* task_off, const uint32_t* perm, MsmShape sh, void* bucket_acc, void* partials);
-int32_t msm_horner_g1(Ctx* c, cudaStream_t st, const void* wins, MsmShape sh, void* out);
-int32_t msm_horner_g2(Ctx* c, cudaStream_t st, const void* wins, MsmShape sh, void* out);
-inline int32_t msm_horner(Ctx* c, cudaStream_t st, int group, const void* wins, MsmShape sh, void* out) {
-    return group == 1 ? msm_horner_g1(c, st, wins, sh, out) : msm_horner_g2(c, st, wins, sh, out);
+int32_t msm_horner_g1(Ctx* c, cudaStream_t st, const void* wins, MsmShape sh, uint32_t K, void* out);
+int32_t msm_horner_g2(Ctx* c, cudaStream_t st, const void* wins, MsmShape sh, uint32_t K, void* out);
+inline int32_t msm_horner(Ctx* c, cudaStream_t st, int group, const void* wins, MsmShape sh, uint32_t K, void* out) {
+    return group == 1 ? msm_horner_g1(c, st, wins, sh, K, out) : msm_horner_g2(c, st, wins, sh, K, out);
 }
 // G1 accumulate for the ctx's curve (msm_acc_g1.cu)
 int32_t msm_accumulate_g1(Ctx* c, const void* bases, const uint32_t* sorted, const uint32_t* offsets,

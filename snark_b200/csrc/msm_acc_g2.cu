@@ -18,10 +18,11 @@ int32_t msm_accumulate_g2(Ctx* c, const void* bases, const uint32_t* sorted, con
     });
 }
 
-int32_t msm_horner_g2(Ctx* c, cudaStream_t st, const void* wins, MsmShape sh, void* out) {
+int32_t msm_horner_g2(Ctx* c, cudaStream_t st, const void* wins, MsmShape sh, uint32_t K, void* out) {
     return dispatch_curve(c, [&](auto curve) {
         using F = typename decltype(curve)::Fq2;
-        B2S_LAUNCH_SN(c, st, "msm_horner_g2", msm_horner_kernel<F>, 1, 32, 0, reinterpret_cast<const XYZZ<F>*>(wins), sh, reinterpret_cast<XYZZ<F>*>(out));
+        B2S_LAUNCH_SN(c, st, "msm_horner_g2", msm_horner_kernel<F>, cdiv(K, 8), 32, 0, reinterpret_cast<const XYZZ<F>*>(wins), sh, K,
+                      reinterpret_cast<XYZZ<F>*>(out));
         return (int32_t)B2S_OK;
     });
 }

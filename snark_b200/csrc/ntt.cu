@@ -44,6 +44,7 @@ struct PassArgs {
     const void* bnd;         // strided pass: inter-pass twiddle of output (k, m) at entry k * 2^log_m + m
     const void* pre_full;    // input scaling, entry = global input index (takes the place of pre)
     const void* post_full;   // final pass: output scaling, entry = output index (takes the place of post / post_const)
+    uint64_t bstride;        // batch: transform blockIdx.y works on src / dst + blockIdx.y * bstride (the factors are shared)
 };
 
 // Non-final pass: sub-NTTs over a strided middle index, in-place positions.
@@ -53,6 +54,8 @@ __global__ void __launch_bounds__(NTT_THREADS) ntt_pass_strided(const Fr* __rest
     const uint32_t R = 1u << a.log_r, C = 1u << a.log_c;
     const uint32_t pitch = 2 * C + 1;
     uint4* tile = smem;
+    src += blockIdx.y * a.bstride;
+    dst += blockIdx.y * a.bstride;
     Fr* wtab = reinterpret_cast<Fr*>(smem + (size_t)R * pitch + 1);   // twiddles w_R^e behind the tile (16-byte aligned)
     const uint32_t tiles_per_p = 1u << (a.log_m - a.log_c);
     const uint64_t p = blockIdx.x / tiles_per_p;
@@ -91,6 +94,8 @@ __global__ void __launch_bounds__(NTT_THREADS) ntt_pass_final(const Fr* __restri
     const uint32_t R = 1u << a.log_r, C = 1u << a.log_c;
     const uint32_t pitch = 2 * C + 1;
     uint4* tile = smem;
+    src += blockIdx.y * a.bstride;
+    dst += blockIdx.y * a.bstride;
     Fr* wtab = reinterpret_cast<Fr*>(smem + (size_t)R * pitch + 1);
     const uint64_t PP = 1ull << a.log_pp;
     const uint64_t pp = blockIdx.x & (PP - 1);
@@ -290,7 +295,7 @@ int32_t ntt_get_full(Ctx* c, uint32_t log_n, NttPlan** out) {
 }
 
 template <class Curve>
-static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode) {
+static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode, uint32_t K) {
     using Fr = typename Curve::Fr;
     const bool inverse = (mode & NTT_M_INVERSE) != 0, coset = (mode & NTT_M_COSET) != 0, wm = (mode & NTT_M_WM) != 0;
     if (log_n == 0 && !wm) return B2S_OK;  // size-1 transform is the identity (coset scaling g^0 = 1, 1/N = 1)
@@ -301,7 +306,7 @@ static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode) 
     if (wm && !fu) return fail(c, B2S_ERR_INVALID_ARG, "ntt: witness-map transform modes need the full-size tables");
     Fr* data = reinterpret_cast<Fr*>(data_dev);
     DevBuf scratch;
-    if (pl->npass > 1) B2S_TRY(scratch.alloc(c, sizeof(Fr) << log_n));
+    if (pl->npass > 1) B2S_TRY(scratch.alloc(c, (sizeof(Fr) << log_n) * K));
     Fr* tmp = scratch.as<Fr>();
 
     PowTab none;
@@ -332,12 +337,13 @@ static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode) 
         a.post_full = nullptr;
         a.wr = fu ? fu->wr[inverse ? 1 : 0][i] : nullptr;
         a.bnd = nullptr;
+        a.bstride = 1ull << log_n;
         if (!last) {
             a.log_c = min((uint32_t)NTT_TILE_LOG - log_r, a.log_m);
             a.bnd = fu ? fu->bnd[inverse ? 1 : 0][i] : nullptr;
             Fr* dst = tmp;
             const unsigned grid = 1u << (log_n - log_r - a.log_c);
-            B2S_LAUNCH(c, ntt_pass_strided<Fr>, grid, NTT_THREADS, smem_bytes, src, dst, a);
+            B2S_LAUNCH(c, ntt_pass_strided<Fr>, dim3(grid, K), NTT_THREADS, smem_bytes, src, dst, a);
             src = tmp;
         } else {
             a.log_r1 = (pl->npass == 1) ? 0 : pl->radix[0];
@@ -347,15 +353,15 @@ static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode) 
             a.post_const = post_const;
             a.post_full = post_full;
             const unsigned grid = 1u << (log_n - log_r - a.log_c);
-            B2S_LAUNCH(c, ntt_pass_final<Fr>, grid, NTT_THREADS, smem_bytes, src, data, a);
+            B2S_LAUNCH(c, ntt_pass_final<Fr>, dim3(grid, K), NTT_THREADS, smem_bytes, src, data, a);
         }
         log_p += log_r;
     }
     return B2S_OK;
 }
 
-int32_t ntt_run_mode(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode) {
-    return dispatch_curve(c, [&](auto curve) { return ntt_run_t<decltype(curve)>(c, data_dev, log_n, mode); });
+int32_t ntt_run_mode(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode, uint32_t K) {
+    return dispatch_curve(c, [&](auto curve) { return ntt_run_t<decltype(curve)>(c, data_dev, log_n, mode, K); });
 }
 
 int32_t ntt_run(Ctx* c, void* data_dev, uint32_t log_n, bool inverse, bool coset) {

@@ -128,7 +128,8 @@ int32_t ntt_get_plan(Ctx* c, uint32_t log_n, NttPlan** out);
 //   WM | COSET             forward coset transform whose input scaling is g^j / N   (makes up for the line above)
 //   WM | INVERSE | COSET   inverse coset transform whose output scaling is g^-j * Zinv / N
 enum : uint32_t { NTT_M_INVERSE = 1, NTT_M_COSET = 2, NTT_M_WM = 4 };
-int32_t ntt_run_mode(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode);
+// K > 1: K transforms of the vectors data_dev + k * 2^log_n, one launch per pass for all of them
+int32_t ntt_run_mode(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode, uint32_t K = 1);
 // plan with full-size tables, or *out = nullptr when they are switched off (B2S_NTT_FULL=0) or would not fit
 int32_t ntt_get_full(Ctx* c, uint32_t log_n, NttPlan** out);
 // dynamic shared memory of one pass CTA (tile of 1024 elements at pitch 2C+1, butterfly twiddles behind it)

@@ -44,12 +44,15 @@ struct SpmvMat {
     void* out;
 };
 
-// One thread per (matrix, row).
+// One thread per (matrix, row).  Batch: blockIdx.y is the assignment k, read at z + k * z_stride, its rows written at
+// out + k * out_stride.
 template <class Fr>
 __global__ void __launch_bounds__(256)
-spmv_kernel(SpmvMat m0, SpmvMat m1, SpmvMat m2, const Fr* __restrict__ pool, const Fr* __restrict__ z, uint64_t n_rows) {
+spmv_kernel(SpmvMat m0, SpmvMat m1, SpmvMat m2, const Fr* __restrict__ pool, const Fr* __restrict__ z, uint64_t n_rows, uint64_t z_stride,
+            uint64_t out_stride) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= 3 * n_rows) return;
+    z += blockIdx.y * z_stride;
     const uint32_t k = (uint32_t)(t / n_rows);
     const uint64_t row = t - (uint64_t)k * n_rows;
     const SpmvMat m = k == 0 ? m0 : (k == 1 ? m1 : m2);
@@ -61,14 +64,14 @@ spmv_kernel(SpmvMat m0, SpmvMat m1, SpmvMat m2, const Fr* __restrict__ pool, con
         if (cid != 0) v = v * fr_ld(pool + cid);
         acc = acc + v;
     }
-    fr_st(reinterpret_cast<Fr*>(m.out) + row, acc);
+    fr_st(reinterpret_cast<Fr*>(m.out) + blockIdx.y * out_stride + row, acc);
 }
 
-// a[n_rows + i] = z[i], i < n_instance   (input-consistency rows of the LibsnarkReduction)
+// a[n_rows + i] = z[i], i < n_instance   (input-consistency rows of the LibsnarkReduction); blockIdx.y: assignment, as in spmv
 template <class Fr>
-__global__ void copy_instance_kernel(Fr* a, const Fr* z, uint64_t n_rows, uint64_t n_instance) {
+__global__ void copy_instance_kernel(Fr* a, const Fr* z, uint64_t n_rows, uint64_t n_instance, uint64_t z_stride, uint64_t a_stride) {
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n_instance) fr_st(a + n_rows + i, fr_ld(z + i));
+    if (i < n_instance) fr_st(a + blockIdx.y * a_stride + n_rows + i, fr_ld(z + blockIdx.y * z_stride + i));
 }
 
 // K3, first half: a[i] *= b[i]   (evaluations of A B on the coset g H)
@@ -181,15 +184,16 @@ int32_t r1cs_upload(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_wit
 }
 
 template <class Curve>
-static int32_t spmv_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* oa, void* ob, void* oc) {
+static int32_t spmv_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* oa, void* ob, void* oc, uint32_t K = 1, uint64_t z_stride = 0,
+                      uint64_t out_stride = 0) {
     using Fr = typename Curve::Fr;
     if (m->n_rows == 0) return B2S_OK;
     SpmvMat mm[3];
     void* outs[3] = {oa, ob, oc};
     for (int k = 0; k < 3; k++)
         mm[k] = SpmvMat{m->row_ptr[k].as<uint64_t>(), m->col[k].as<uint32_t>(), m->coeff_id[k].as<uint32_t>(), outs[k]};
-    B2S_LAUNCH(c, spmv_kernel<Fr>, cdiv(3 * m->n_rows, 256), 256, 0, mm[0], mm[1], mm[2], m->pool.as<Fr>(),
-               reinterpret_cast<const Fr*>(z_dev), m->n_rows);
+    B2S_LAUNCH(c, spmv_kernel<Fr>, dim3(cdiv(3 * m->n_rows, 256), K), 256, 0, mm[0], mm[1], mm[2], m->pool.as<Fr>(),
+               reinterpret_cast<const Fr*>(z_dev), m->n_rows, z_stride, out_stride);
     return B2S_OK;
 }
 
@@ -203,42 +207,45 @@ int32_t spmv_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* oa, void* o
 // for every assignment (satisfying or not) -- 6 transforms, the same field elements.  With the plan's full-size tables the
 // scalings are merged as well: the three inverse transforms run unscaled, the 1/N goes into the coset input scaling of a and
 // b (g^j / N), Zinv into the output scaling of the closing transform, and c's 1/N * Zinv into the (HBM-bound) last kernel.
+// A batch of K assignments (z_dev + k * z_stride) gives h_dev + k * N with the same launches: every kernel takes the
+// assignment from blockIdx.y, and the pointwise ones simply run over K * N elements.
 template <class Curve>
-static int32_t witness_map_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev) {
+static int32_t witness_map_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, uint32_t K, uint64_t z_stride) {
     using Fr = typename Curve::Fr;
     const uint64_t N = 1ull << m->log_domain;
     Fr* a = reinterpret_cast<Fr*>(h_dev);
     DevBuf bb, cb;
-    B2S_TRY(bb.alloc(c, N * sizeof(Fr)));
-    B2S_TRY(cb.alloc(c, N * sizeof(Fr)));
+    B2S_TRY(bb.alloc(c, K * N * sizeof(Fr)));
+    B2S_TRY(cb.alloc(c, K * N * sizeof(Fr)));
     Fr* b = bb.as<Fr>();
     Fr* cc = cb.as<Fr>();
-    // zero the padding [n_rows, N)
-    B2S_CUDA(c, cudaMemsetAsync(a + m->n_rows, 0, (N - m->n_rows) * sizeof(Fr), c->stream));
-    B2S_CUDA(c, cudaMemsetAsync(b + m->n_rows, 0, (N - m->n_rows) * sizeof(Fr), c->stream));
-    B2S_CUDA(c, cudaMemsetAsync(cc + m->n_rows, 0, (N - m->n_rows) * sizeof(Fr), c->stream));
-    B2S_TRY(spmv_t<Curve>(c, m, z_dev, a, b, cc));
-    B2S_LAUNCH(c, copy_instance_kernel<Fr>, cdiv(m->n_instance, 256), 256, 0, a, reinterpret_cast<const Fr*>(z_dev),
-               m->n_rows, m->n_instance);
+    // zero the padding [n_rows, N) of every vector
+    const size_t pitch = N * sizeof(Fr), pad = (N - m->n_rows) * sizeof(Fr);
+    B2S_CUDA(c, cudaMemset2DAsync(a + m->n_rows, pitch, 0, pad, K, c->stream));
+    B2S_CUDA(c, cudaMemset2DAsync(b + m->n_rows, pitch, 0, pad, K, c->stream));
+    B2S_CUDA(c, cudaMemset2DAsync(cc + m->n_rows, pitch, 0, pad, K, c->stream));
+    B2S_TRY(spmv_t<Curve>(c, m, z_dev, a, b, cc, K, z_stride, N));
+    B2S_LAUNCH(c, copy_instance_kernel<Fr>, dim3(cdiv(m->n_instance, 256), K), 256, 0, a, reinterpret_cast<const Fr*>(z_dev),
+               m->n_rows, m->n_instance, z_stride, N);
     NttPlan* pl = nullptr;
     B2S_TRY(ntt_get_full(c, m->log_domain, &pl));
     const uint32_t wm = pl ? NTT_M_WM : 0u;
     if (!pl) B2S_TRY(ntt_get_plan(c, m->log_domain, &pl));
     Fr* bufs[3] = {a, b, cc};
-    for (Fr* v : bufs) B2S_TRY(ntt_run_mode(c, v, m->log_domain, NTT_M_INVERSE | wm));
-    B2S_TRY(ntt_run_mode(c, a, m->log_domain, NTT_M_COSET | wm));
-    B2S_TRY(ntt_run_mode(c, b, m->log_domain, NTT_M_COSET | wm));
-    B2S_LAUNCH(c, qap_mul_kernel<Fr>, cdiv(N, 256), 256, 0, a, (const Fr*)b, N);
-    B2S_TRY(ntt_run_mode(c, a, m->log_domain, NTT_M_INVERSE | NTT_M_COSET | wm));
+    for (Fr* v : bufs) B2S_TRY(ntt_run_mode(c, v, m->log_domain, NTT_M_INVERSE | wm, K));
+    B2S_TRY(ntt_run_mode(c, a, m->log_domain, NTT_M_COSET | wm, K));
+    B2S_TRY(ntt_run_mode(c, b, m->log_domain, NTT_M_COSET | wm, K));
+    B2S_LAUNCH(c, qap_mul_kernel<Fr>, cdiv(K * N, 256), 256, 0, a, (const Fr*)b, K * N);
+    B2S_TRY(ntt_run_mode(c, a, m->log_domain, NTT_M_INVERSE | NTT_M_COSET | wm, K));
     // composed scalings: q and c both still lack Zinv;  merged: q is finished, c lacks Zinv / N
     const Fr* alpha = reinterpret_cast<const Fr*>(wm ? pl->one : pl->zinv);
     const Fr* beta = reinterpret_cast<const Fr*>(wm ? pl->full->wm_beta : pl->zinv);
-    B2S_LAUNCH(c, qap_quotient_kernel<Fr>, cdiv(N, 256), 256, 0, a, (const Fr*)cc, alpha, beta, N);
+    B2S_LAUNCH(c, qap_quotient_kernel<Fr>, cdiv(K * N, 256), 256, 0, a, (const Fr*)cc, alpha, beta, K * N);
     return B2S_OK;
 }
 
-int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev) {
-    return dispatch_curve(c, [&](auto curve) { return witness_map_t<decltype(curve)>(c, m, z_dev, h_dev); });
+int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, uint32_t K, uint64_t z_stride) {
+    return dispatch_curve(c, [&](auto curve) { return witness_map_t<decltype(curve)>(c, m, z_dev, h_dev, K, z_stride); });
 }
 
 }  // namespace b2s

@@ -68,8 +68,9 @@ int32_t r1cs_upload_lcmap(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t
                           const void* pool, uint32_t pool_len, b2s_r1cs** out);
 // out_k: device arrays with at least n_rows elements each
 int32_t spmv_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* out_a, void* out_b, void* out_c);
-// h_dev: device array of domain elements (output); z_dev: n_instance + n_witness elements
-int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev);
+// h_dev: device array of domain elements (output); z_dev: n_instance + n_witness elements.  K > 1: K assignments at
+// z_dev + k * z_stride (elements) give K vectors h_dev + k * domain, with the launches of one
+int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, uint32_t K = 1, uint64_t z_stride = 0);
 int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out);
 int32_t groth16_setup(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
                       void* o_gamma_g2, void* o_delta_g2, void* o_gamma_abc);
@@ -86,6 +87,10 @@ struct HSource {
 int32_t groth16_shard(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* z_inst_host, const void* z_wit_host,
                       const void* z_dev, const void* r_host, const void* s_host, void* g1_partials_dev /*4 xyzz*/,
                       void* g2_partial_dev /*1 xyzz*/, HSource* hs = nullptr);
+// n_proofs proofs under one full key: z holds n_proofs rows of n_instance + n_witness scalars, r and s one scalar per proof,
+// out_a / out_b / out_c n_proofs affine points; all in host memory, or all on the device (mem == B2S_MEM_DEVICE)
+int32_t groth16_prove_batch(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, uint64_t n_proofs, const void* z, const void* r, const void* s,
+                            int32_t mem, void* out_a, void* out_b, void* out_c);
 int32_t groth16_finish(Ctx* c, const b2s_pk* pk, const void* g1_partials_dev, const void* g2_partials_dev, uint32_t n_shards,
                        const void* r_host, const void* s_host, void* out_a, void* out_b, void* out_c);
 }  // namespace b2s

@@ -70,6 +70,8 @@ SIGNATURES = {
     "b2s_groth16_prove_shard": (c_int32, [c_void_p] * 9),
     "b2s_groth16_prove_resident": (c_int32, [c_void_p] * 9),
     "b2s_groth16_prove_shard_resident": (c_int32, [c_void_p] * 8),
+    "b2s_groth16_prove_batch": (c_int32, [c_void_p, c_void_p, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p,
+                                          c_void_p]),
     "b2s_profile_enable": (c_int32, [c_void_p, c_int32]),
     "b2s_profile_report": (c_int32, [c_void_p, c_char_p, c_uint64]),
     "b2s_groth16_finish": (c_int32, [c_void_p, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p, c_void_p,
@@ -549,6 +551,27 @@ class Backend:
         a, b, c = self._proof_bufs()
         self._ck(self.lib.b2s_groth16_prove_resident(self.h, pk, m, _ptr(z_dev)[0], r.ctypes.data, s.ctypes.data,
                                                      a.ctypes.data, b.ctypes.data, c.ctypes.data))
+        return a, b, c
+
+    def groth16_prove_batch(self, pk, m, z, r, s):
+        """n_proofs proofs under one key in one call (b2s_groth16_prove_batch).  z: n_proofs rows of n_instance + n_witness
+        Montgomery Fr (row i = proof i's instance || witness); r, s: n_proofs Montgomery Fr each; all HOST numpy arrays or all
+        CUDA torch tensors.  Returns (a, b, c): n_proofs x (G1 / G2 / G1 affine) uint32 numpy arrays, or int32 tensors on the
+        device of the inputs (the library's stream is synchronised before return)."""
+        pz, mem = _ptr(z)
+        pr, mem_r = _ptr(r)
+        ps, mem_s = _ptr(s)
+        assert mem == mem_r == mem_s
+        n = (r.nbytes if isinstance(r, np.ndarray) else r.numel() * r.element_size()) // self.fr_bytes
+        w1, w2 = self.g1_bytes // 4, self.g2_bytes // 4
+        if mem == MEM_HOST:
+            a, b, c = (np.zeros((n, w), dtype=np.uint32) for w in (w1, w2, w1))
+        else:
+            import torch
+
+            a, b, c = (torch.zeros((n, w), dtype=torch.int32, device=r.device) for w in (w1, w2, w1))
+            torch.cuda.current_stream(r.device).synchronize()
+        self._ck(self.lib.b2s_groth16_prove_batch(self.h, pk, m, n, pz, pr, ps, mem, _ptr(a)[0], _ptr(b)[0], _ptr(c)[0]))
         return a, b, c
 
     def groth16_prove_shard_resident(self, pk, m, z_dev, r, s):
