@@ -51,6 +51,22 @@ extern "C" {
 #define B2S_MEM_HOST 0
 #define B2S_MEM_DEVICE 1
 
+/* QAP reduction of a Groth16 key (ark-groth16's R1CSToQAP): fixed when the device-resident key is created, it selects the
+ * witness map of every proof under the key and the form of its h query.
+ *   B2S_QAP_LIBSNARK  ark-groth16's LibsnarkReduction (Groth16<E>): h = coefficients of (A B - C) / Z, |h_query| = N - 1,
+ *                     h_query[i] = tau^i Z(tau) / delta.  What every entry point without a `qap` argument uses.
+ *   B2S_QAP_CIRCOM    ark-circom's CircomReduction (Groth16<E, CircomReduction>, snarkjs keys): with w2 a primitive 2N-th
+ *                     root (w2^2 = w) and x_j = w2 w^j the odd coset, h_j = a_j b_j - c_j where a, b are A z and B z (instance
+ *                     rows in a) and c = (A z) o (B z) on H, all three moved to x_j; C is never read.  |h_query| = N,
+ *                     h_query[j] = L^(2N)_{2j+1}(tau) / delta (the odd-indexed Lagrange basis of the size-2N domain, as snarkjs
+ *                     writes it).  The rest of the key and the proof are unchanged; the verifiers below take circom proofs as
+ *                     they are.  Not provided: the distributed witness map (b2s_groth16_prove_group* refuse circom keys with
+ *                     B2S_ERR_INVALID_ARG; b2s_groth16_prove_shard + b2s_groth16_finish work), and readers of snarkjs
+ *                     .zkey / .wtns files (ark-circom turns a zkey into an ark ProvingKey: b2s_pk_deserialize_qap).
+ * Any other value is B2S_ERR_INVALID_ARG. */
+#define B2S_QAP_LIBSNARK 0
+#define B2S_QAP_CIRCOM 1
+
 /* status codes; 1..7 mirror SynthesisError (relations/src/utils/error.rs:5-21) */
 #define B2S_OK 0
 #define B2S_ERR_MISSING_CS 1
@@ -142,8 +158,12 @@ int32_t b2s_spmv(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, vo
  * field elements for every assignment.
  * out_h receives domain_size elements (the top one is 0); domain_size = next_pow2(n_rows + n_instance). */
 int32_t b2s_witness_map(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, void* out_h);
+/* The witness map of either reduction (B2S_QAP_*): B2S_QAP_LIBSNARK is b2s_witness_map; B2S_QAP_CIRCOM writes the domain_size
+ * odd-coset evaluations h_j = a_j b_j - c_j (CircomReduction::witness_map_from_matrices), six transforms, C not read.
+ * out_h receives domain_size elements under either reduction. */
+int32_t b2s_witness_map_qap(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, int32_t qap, void* out_h);
 uint64_t b2s_r1cs_domain_size(const b2s_r1cs* m);
-/* The same h computed by the DISTRIBUTED schedule of b2s_groth16_prove_group (four-step transforms, SpMV and quotient on
+/* The same (libsnark) h computed by the DISTRIBUTED schedule of b2s_groth16_prove_group (four-step transforms, SpMV and quotient on
  * column slabs, SURVEY 8(e)) with 2^log_ranks virtual ranks on this one GPU, the all-to-all replaced by device copies.
  * Exists so that the index algebra of the multi-GPU path is checked bit for bit on a one-GPU box; B2S_ERR_INVALID_ARG
  * when the domain cannot be cut that way (log2(domain) odd, or too few rows per rank). */
@@ -152,8 +172,9 @@ int32_t b2s_witness_map_sim(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int3
 /* ---- Groth16 (ark-groth16 ProvingKey / create_proof_with_reduction, SURVEY App. A.1) ------------
  * Query vectors are affine point arrays in HOST or DEVICE memory (`mem`); they are copied to the GPU.
  *   a_query, b_g1_query, b_g2_query: n_vars = n_instance + n_witness points
- *   h_query: domain_size - 1 points;  l_query: n_witness points
- * For a base-range shard (multi-GPU) pass the sub-ranges and their offsets; a full key has offsets 0.
+ *   h_query: domain_size - 1 points (B2S_QAP_LIBSNARK) or domain_size points (B2S_QAP_CIRCOM);  l_query: n_witness points
+ * For a base-range shard (multi-GPU) pass the sub-ranges and their offsets; a full key has offsets 0.  Every h range lies in
+ * [0, domain_size); a shard of a circom key holds a slice of the odd-coset points.
  */
 typedef struct b2s_pk_desc {
     uint64_t n_instance, n_witness, domain_size;
@@ -169,6 +190,9 @@ typedef struct b2s_pk_desc {
     const void* l_query;    uint64_t l_off, l_len;
 } b2s_pk_desc;
 int32_t b2s_pk_upload(b2s_ctx* ctx, const b2s_pk_desc* desc, int32_t mem, b2s_pk** out);
+/* The same for a key of either reduction; b2s_pk_upload is the B2S_QAP_LIBSNARK case.  Under B2S_QAP_CIRCOM a full key has
+ * h_len == domain_size; a full-looking key with h_len == domain_size - 1 is B2S_ERR_MALFORMED_VK. */
+int32_t b2s_pk_upload_qap(b2s_ctx* ctx, const b2s_pk_desc* desc, int32_t mem, int32_t qap, b2s_pk** out);
 void b2s_pk_free(b2s_ctx* ctx, b2s_pk* pk);
 
 /* CircuitSpecificSetupSNARK::setup (snark/src/lib.rs:84-93) on the GPU for uploaded matrices.  `trapdoor` = 5 Montgomery
@@ -177,12 +201,20 @@ void b2s_pk_free(b2s_ctx* ctx, b2s_pk* pk);
  * beta_g2, gamma_g2, delta_g2 (G2), gamma_abc_g1 (n_instance G1 points). */
 int32_t b2s_groth16_setup(b2s_ctx* ctx, const b2s_r1cs* m, const void* trapdoor, b2s_pk** out_pk, void* out_alpha_g1,
                           void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1);
+/* The same for either reduction; b2s_groth16_setup is the B2S_QAP_LIBSNARK case.  B2S_QAP_CIRCOM builds the N-point circom
+ * h query (see B2S_QAP_CIRCOM) and rejects tau with tau^(2N) = 1 (B2S_ERR_DIVISION_BY_ZERO).  Every other element of the key
+ * and the verifying key is the same as under libsnark for the same trapdoor, and so are the proofs of a satisfying
+ * assignment with the same r, s. */
+int32_t b2s_groth16_setup_qap(b2s_ctx* ctx, const b2s_r1cs* m, const void* trapdoor, int32_t qap, b2s_pk** out_pk,
+                              void* out_alpha_g1, void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2,
+                              void* out_gamma_abc_g1);
 /* Copy one vector of a device-resident key to the HOST (to serialise a ProvingKey):
  * which = 0 a_query, 1 b_g1_query, 2 b_g2_query, 3 h_query, 4 l_query, 5 [alpha,beta,delta]_g1, 6 [beta,delta]_g2. */
 int32_t b2s_pk_query(b2s_ctx* ctx, const b2s_pk* pk, int32_t which, void* out, uint64_t cap_bytes);
 
 /* One proof on one GPU (full key).  z_instance (n_instance, z[0] = 1), z_witness, r, s: Montgomery Fr, HOST.
- * Outputs (HOST): A (G1 affine), B (G2 affine), C (G1 affine) -- `Proof { a, b, c }`. */
+ * Outputs (HOST): A (G1 affine), B (G2 affine), C (G1 affine) -- `Proof { a, b, c }`.
+ * This and every prove / shard / serialize entry point below run under the key's own reduction (B2S_QAP_*). */
 int32_t b2s_groth16_prove(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_instance,
                           const void* z_witness, const void* r, const void* s, void* out_a_g1, void* out_b_g2,
                           void* out_c_g1);
@@ -284,6 +316,8 @@ int32_t b2s_pk_serialize(b2s_ctx* ctx, const b2s_pk* pk, const uint8_t* vk_bytes
  *                          handle b2s_pk_upload returns for the same points.  The dimensions follow from the bytes:
  *                          n_instance = |gamma_abc_g1|, n_witness = |l_query|, domain_size = |h_query| + 1 (a power of two),
  *                          |a_query| = |b_g1_query| = |b_g2_query| = n_instance + n_witness, else B2S_ERR_MALFORMED_VK.
+ *   b2s_pk_deserialize_qap the same for either reduction (b2s_pk_deserialize is B2S_QAP_LIBSNARK); under B2S_QAP_CIRCOM
+ *                          domain_size = |h_query| (a power of two): the bytes of a Groth16<Bn254, CircomReduction> key
  * Every Vec length prefix is checked against the bytes that remain before anything is allocated. */
 int32_t b2s_deserialize_g1(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t count, int32_t compressed, int32_t validate,
                            void* out_affine);
@@ -295,6 +329,8 @@ int32_t b2s_vk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
                            void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1, uint64_t cap_gamma_abc,
                            uint64_t* n_gamma_abc, uint64_t* consumed);
 int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, b2s_pk** out);
+int32_t b2s_pk_deserialize_qap(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, int32_t qap,
+                               b2s_pk** out);
 
 /* ---- verification: pairings and batched Groth16 verify ----------------------------------------------------------------
  * The optimal ate pairing in CUDA (snark_b200/csrc/pairing.cuh): BLS12-381 loops over |x| and conjugates, BN254 over the

@@ -68,6 +68,14 @@ extern "C" {
                               out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void, out_delta_g2: *mut c_void,
                               out_gamma_abc_g1: *mut c_void, cap_gamma_abc: u64, n_gamma_abc: *mut u64, consumed: *mut u64) -> i32;
     pub fn b2s_pk_deserialize(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, out: *mut *mut B2sPk) -> i32;
+    // the QAP reduction of a key (B2S_QAP_LIBSNARK = 0, B2S_QAP_CIRCOM = 1): see QAP_LIBSNARK / QAP_CIRCOM below
+    pub fn b2s_pk_deserialize_qap(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, qap: i32,
+                                  out: *mut *mut B2sPk) -> i32;
+    pub fn b2s_pk_upload_qap(ctx: *mut B2sCtx, desc: *const B2sPkDesc, mem: i32, qap: i32, out: *mut *mut B2sPk) -> i32;
+    pub fn b2s_groth16_setup_qap(ctx: *mut B2sCtx, m: *const B2sR1cs, trapdoor: *const c_void, qap: i32, out_pk: *mut *mut B2sPk,
+                                 out_alpha_g1: *mut c_void, out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void,
+                                 out_delta_g2: *mut c_void, out_gamma_abc_g1: *mut c_void) -> i32;
+    pub fn b2s_witness_map_qap(ctx: *mut B2sCtx, m: *const B2sR1cs, z: *const c_void, mem: i32, qap: i32, out_h: *mut c_void) -> i32;
     // verification (SNARK::process_vk / verify_with_processed_vk for many proofs; pairings in CUDA)
     pub fn b2s_vk_prepare(ctx: *mut B2sCtx, alpha_g1: *const c_void, beta_g2: *const c_void, gamma_g2: *const c_void,
                           delta_g2: *const c_void, gamma_abc_g1: *const c_void, n_gamma_abc: u64, out: *mut *mut B2sPvk) -> i32;
@@ -167,6 +175,11 @@ fn check(ctx: *mut B2sCtx, st: i32) -> Result<(), B200Error> {
 
 pub struct Groth16B200<E: Pairing>(core::marker::PhantomData<E>);
 
+/// ark-groth16's `LibsnarkReduction` (`Groth16<E>`): |h_query| = domain - 1.
+pub const QAP_LIBSNARK: i32 = 0;
+/// ark-circom's `CircomReduction` (`Groth16<Bn254, CircomReduction>`, keys converted from snarkjs zkeys): |h_query| = domain.
+pub const QAP_CIRCOM: i32 = 1;
+
 /// Device handles for one (proving key, circuit shape): matrices and key are witness independent.
 pub struct Resident { pub ctx: *mut B2sCtx, pub pk: *mut B2sPk, pub mat: *mut B2sR1cs }
 
@@ -213,9 +226,20 @@ impl<E: Pairing> Groth16B200<E> {
     /// with `validate`, checked (curve equation, prime-order subgroup) on the GPU, straight into the resident key.
     pub fn make_resident_from_bytes(curve_id: i32, pk_bytes: &[u8], compressed: bool, validate: bool, mats: &[Matrix<E::ScalarField>],
                                     n_inst: usize, n_wit: usize) -> Result<Resident, B200Error> {
+        Self::make_resident_from_bytes_qap(curve_id, pk_bytes, compressed, validate, QAP_LIBSNARK, mats, n_inst, n_wit)
+    }
+
+    /// The same for a key of either QAP reduction.  With `QAP_CIRCOM` the bytes are those of a
+    /// `ProvingKey<Bn254>` for `Groth16<Bn254, CircomReduction>` (what ark-circom's zkey reader returns, serialized), and
+    /// `mats` the circuit's A, B, C (C may have no entries: the circom witness map never reads it).  Every proof under the
+    /// resident key then runs the circom witness map and verifies with the key's ordinary `VerifyingKey`.
+    pub fn make_resident_from_bytes_qap(curve_id: i32, pk_bytes: &[u8], compressed: bool, validate: bool, qap: i32,
+                                        mats: &[Matrix<E::ScalarField>], n_inst: usize, n_wit: usize) -> Result<Resident, B200Error> {
         let (ctx, mat) = Self::ctx_and_matrices(curve_id, mats, n_inst, n_wit)?;
         let mut pkh: *mut B2sPk = core::ptr::null_mut();
-        check(ctx, unsafe { b2s_pk_deserialize(ctx, pk_bytes.as_ptr(), pk_bytes.len() as u64, compressed as i32, validate as i32, &mut pkh) })?;
+        check(ctx, unsafe {
+            b2s_pk_deserialize_qap(ctx, pk_bytes.as_ptr(), pk_bytes.len() as u64, compressed as i32, validate as i32, qap, &mut pkh)
+        })?;
         Ok(Resident { ctx, pk: pkh, mat })
     }
 

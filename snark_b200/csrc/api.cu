@@ -33,7 +33,7 @@ int32_t deserialize_points(Ctx* c, int group, const uint8_t* in, uint64_t len, u
 int32_t proof_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* a, void* b, void* cc);
 int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* alpha, void* beta, void* gamma,
                        void* delta, void* abc, uint64_t cap_abc, uint64_t* n_abc, uint64_t* consumed);
-int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, b2s_pk** out);
+int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, int32_t qap, b2s_pk** out);
 // verify.cu
 int32_t vk_prepare(Ctx* c, const void* alpha, const void* beta, const void* gamma, const void* delta, const void* abc, uint64_t n_abc,
                    b2s_pvk** out);
@@ -276,6 +276,13 @@ static bool z_missing(const b2s_r1cs* m, const void* z_inst, const void* z_wit, 
     return !z_dev && (!z_inst || (!z_wit && m->n_witness));
 }
 
+// the `qap` argument of the *_qap entry points
+static int32_t check_qap(b2s_ctx* ctx, int32_t qap, const char* who) {
+    if (qap != B2S_QAP_LIBSNARK && qap != B2S_QAP_CIRCOM)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "%s: unknown QAP reduction %d (B2S_QAP_LIBSNARK = 0, B2S_QAP_CIRCOM = 1)", who, (int)qap);
+    return B2S_OK;
+}
+
 // one proof on one GPU with a full key
 static int32_t prove_full(b2s_ctx* ctx, const b2s_pk* pk, const b2s_r1cs* m, const void* z_inst, const void* z_wit, const void* z_dev,
                           const void* r, const void* s, void* out_a_g1, void* out_b_g2, void* out_c_g1) {
@@ -364,20 +371,30 @@ int32_t b2s_spmv(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, vo
     return B2S_OK;
 }
 
-int32_t b2s_witness_map(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, void* out_h) {
-    LOCK(ctx);
+static int32_t witness_map_common(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, int32_t qap, void* out_h) {
     if (!m) return fail(ctx, B2S_ERR_MISSING_CS, "witness_map: null matrices");
     if (!z || !out_h) return fail(ctx, B2S_ERR_INVALID_ARG, "witness_map: null buffer");
+    B2S_TRY(check_qap(ctx, qap, "witness_map"));
     const size_t nz = (m->n_instance + m->n_witness) * 32, nh = (size_t)32 << m->log_domain;
-    if (mem == B2S_MEM_DEVICE) return witness_map_run(ctx, m, z, out_h);
+    if (mem == B2S_MEM_DEVICE) return witness_map_run(ctx, m, z, out_h, qap);
     InBuf zi;
     B2S_TRY(zi.bind(ctx, z, nz, mem));
     DevBuf h;
     B2S_TRY(h.alloc(ctx, nh));
-    B2S_TRY(witness_map_run(ctx, m, zi.dptr, h.p));
+    B2S_TRY(witness_map_run(ctx, m, zi.dptr, h.p, qap));
     B2S_CUDA(ctx, cudaMemcpyAsync(out_h, h.p, nh, cudaMemcpyDeviceToHost, ctx->stream));
     B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     return B2S_OK;
+}
+
+int32_t b2s_witness_map(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, void* out_h) {
+    LOCK(ctx);
+    return witness_map_common(ctx, m, z, mem, B2S_QAP_LIBSNARK, out_h);
+}
+
+int32_t b2s_witness_map_qap(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, int32_t qap, void* out_h) {
+    LOCK(ctx);
+    return witness_map_common(ctx, m, z, mem, qap, out_h);
 }
 
 int32_t b2s_witness_map_sim(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, uint32_t log_ranks, void* out_h) {
@@ -402,7 +419,15 @@ int32_t b2s_pk_upload(b2s_ctx* ctx, const b2s_pk_desc* desc, int32_t mem, b2s_pk
     LOCK(ctx);
     if (!desc || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_upload: null argument");
     *out = nullptr;
-    return pk_upload(ctx, desc, mem, out);
+    return pk_upload(ctx, desc, mem, B2S_QAP_LIBSNARK, out);
+}
+
+int32_t b2s_pk_upload_qap(b2s_ctx* ctx, const b2s_pk_desc* desc, int32_t mem, int32_t qap, b2s_pk** out) {
+    LOCK(ctx);
+    if (!desc || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_upload: null argument");
+    *out = nullptr;
+    B2S_TRY(check_qap(ctx, qap, "pk_upload"));
+    return pk_upload(ctx, desc, mem, qap, out);
 }
 
 void b2s_pk_free(b2s_ctx* ctx, b2s_pk* pk) {
@@ -506,14 +531,26 @@ int32_t b2s_profile_report(b2s_ctx* ctx, char* buf, uint64_t cap) {
 }
 
 
-int32_t b2s_groth16_setup(b2s_ctx* ctx, const b2s_r1cs* m, const void* trapdoor, b2s_pk** out_pk, void* out_alpha_g1,
-                          void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1) {
-    LOCK(ctx);
+static int32_t setup_common(b2s_ctx* ctx, const b2s_r1cs* m, const void* trapdoor, int32_t qap, b2s_pk** out_pk, void* out_alpha_g1,
+                            void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1) {
     if (!m) return fail(ctx, B2S_ERR_MISSING_CS, "setup: null matrices");
     if (!trapdoor || !out_pk || !out_alpha_g1 || !out_beta_g2 || !out_gamma_g2 || !out_delta_g2 || !out_gamma_abc_g1)
         return fail(ctx, B2S_ERR_INVALID_ARG, "setup: null argument");
     *out_pk = nullptr;
-    return groth16_setup(ctx, m, trapdoor, out_pk, out_alpha_g1, out_beta_g2, out_gamma_g2, out_delta_g2, out_gamma_abc_g1);
+    B2S_TRY(check_qap(ctx, qap, "setup"));
+    return groth16_setup(ctx, m, trapdoor, qap, out_pk, out_alpha_g1, out_beta_g2, out_gamma_g2, out_delta_g2, out_gamma_abc_g1);
+}
+
+int32_t b2s_groth16_setup(b2s_ctx* ctx, const b2s_r1cs* m, const void* trapdoor, b2s_pk** out_pk, void* out_alpha_g1,
+                          void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1) {
+    LOCK(ctx);
+    return setup_common(ctx, m, trapdoor, B2S_QAP_LIBSNARK, out_pk, out_alpha_g1, out_beta_g2, out_gamma_g2, out_delta_g2, out_gamma_abc_g1);
+}
+
+int32_t b2s_groth16_setup_qap(b2s_ctx* ctx, const b2s_r1cs* m, const void* trapdoor, int32_t qap, b2s_pk** out_pk, void* out_alpha_g1,
+                              void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1) {
+    LOCK(ctx);
+    return setup_common(ctx, m, trapdoor, qap, out_pk, out_alpha_g1, out_beta_g2, out_gamma_g2, out_delta_g2, out_gamma_abc_g1);
 }
 
 int32_t b2s_pk_query(b2s_ctx* ctx, const b2s_pk* pk, int32_t which, void* out, uint64_t cap_bytes) {
@@ -606,7 +643,15 @@ int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
     LOCK(ctx);
     if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_deserialize: null argument");
     *out = nullptr;
-    return pk_deserialize(ctx, in, len, compressed != 0, validate != 0, out);
+    return pk_deserialize(ctx, in, len, compressed != 0, validate != 0, B2S_QAP_LIBSNARK, out);
+}
+int32_t b2s_pk_deserialize_qap(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, int32_t qap,
+                               b2s_pk** out) {
+    LOCK(ctx);
+    if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_deserialize: null argument");
+    *out = nullptr;
+    B2S_TRY(check_qap(ctx, qap, "pk_deserialize"));
+    return pk_deserialize(ctx, in, len, compressed != 0, validate != 0, qap, out);
 }
 
 int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,

@@ -209,7 +209,7 @@ int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed,
     return st.decode_host(1, in + v.abc, v.n_abc, compressed, validate, abc, "gamma_abc_g1");
 }
 
-int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, b2s_pk** out) {
+int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, int32_t qap, b2s_pk** out) {
     Frame f{c, in, len, 0, compressed};
     VkFrame v;
     uint64_t beta1, delta1, at[PK_QUERIES], n[PK_QUERIES];
@@ -218,14 +218,16 @@ int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed,
     B2S_TRY(f.point(1, &delta1));
     for (int w = 0; w < PK_QUERIES; w++) B2S_TRY(f.vec(PK_QUERY[w].group, PK_QUERY[w].name, &at[w], &n[w]));
     if (f.at != len) return fail(c, B2S_ERR_INVALID_DATA, "pk: %llu trailing bytes", (unsigned long long)(len - f.at));
-    const uint64_t n_instance = v.n_abc, n_witness = n[Q_L], n_vars = n_instance + n_witness, domain = n[Q_H] + 1;
-    if (n[Q_A] != n_vars || n[Q_B_G1] != n_vars || n[Q_B_G2] != n_vars || (domain & (domain - 1)))
+    // |h_query| = domain - 1 (libsnark) or domain (circom), the domain a power of two
+    const uint64_t n_instance = v.n_abc, n_witness = n[Q_L], n_vars = n_instance + n_witness;
+    const uint64_t domain = qap == B2S_QAP_CIRCOM ? n[Q_H] : n[Q_H] + 1;
+    if (n[Q_A] != n_vars || n[Q_B_G1] != n_vars || n[Q_B_G2] != n_vars || domain == 0 || (domain & (domain - 1)))
         return fail(c, B2S_ERR_MALFORMED_VK, "pk: inconsistent dimensions (instance %llu, witness %llu, a %llu, b_g1 %llu, b_g2 %llu, h %llu)",
                     (unsigned long long)n_instance, (unsigned long long)n_witness, (unsigned long long)n[Q_A], (unsigned long long)n[Q_B_G1],
                     (unsigned long long)n[Q_B_G2], (unsigned long long)n[Q_H]);
     const size_t g1 = sizes(c).g1, g2 = sizes(c).g2;
     b2s_pk* pk = new b2s_pk();
-    pk->n_instance = n_instance; pk->n_witness = n_witness; pk->domain_size = domain;
+    pk->n_instance = n_instance; pk->n_witness = n_witness; pk->domain_size = domain; pk->qap = qap;
     for (int w = 0; w < PK_QUERIES; w++) pk->q[w].len = n[w];   // a full key: every range starts at 0
     auto body = [&]() -> int32_t {
         Stager st(c);

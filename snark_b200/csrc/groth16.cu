@@ -133,10 +133,11 @@ int32_t pk_finish(Ctx* c, b2s_pk* pk) {
     return B2S_OK;
 }
 
-int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
+int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, int32_t qap, b2s_pk** out) {
     const Sizes z = sizes(c);
     const uint64_t n_vars = d->n_instance + d->n_witness;
-    // [off, off + len) must lie in [0, bound).  h is held to domain_size only, although a full key's h is domain_size - 1 long
+    // [off, off + len) must lie in [0, bound).  h is held to domain_size under either reduction (a full libsnark key's h is
+    // domain_size - 1 long, a full circom key's domain_size)
     struct { const void* pts; uint64_t off, len, bound; } src[PK_QUERIES] = {
         {d->a_query, d->a_off, d->a_len, n_vars},
         {d->b_g1_query, d->b1_off, d->b1_len, n_vars},
@@ -147,8 +148,12 @@ int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
         if (s.off + s.len > s.bound) return fail(c, B2S_ERR_MALFORMED_VK, "pk: a query range exceeds the key dimensions");
     if (!d->alpha_g1 || !d->beta_g1 || !d->delta_g1 || !d->beta_g2 || !d->delta_g2)
         return fail(c, B2S_ERR_MALFORMED_VK, "pk: missing group constants");
+    if (qap == B2S_QAP_CIRCOM && d->h_off == 0 && d->h_len + 1 == d->domain_size && d->a_len == n_vars && d->b1_len == n_vars &&
+        d->b2_len == n_vars && d->l_len == d->n_witness)
+        return fail(c, B2S_ERR_MALFORMED_VK, "pk: a full circom key has domain_size = %llu h_query points, not %llu (a libsnark key?)",
+                    (unsigned long long)d->domain_size, (unsigned long long)d->h_len);
     b2s_pk* pk = new b2s_pk();
-    pk->n_instance = d->n_instance; pk->n_witness = d->n_witness; pk->domain_size = d->domain_size;
+    pk->n_instance = d->n_instance; pk->n_witness = d->n_witness; pk->domain_size = d->domain_size; pk->qap = qap;
     for (int w = 0; w < PK_QUERIES; w++) { pk->q[w].off = src[w].off; pk->q[w].len = src[w].len; }
     const cudaMemcpyKind kind = mem == B2S_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
     auto body = [&]() -> int32_t {
@@ -175,12 +180,12 @@ int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out) {
     return B2S_OK;
 }
 
-// the whole h on this GPU
+// the whole h on this GPU, under the key's reduction (a shard's h range is a slice of the coefficients or of the evaluations)
 struct ReplicatedH : HSource {
     DevBuf h;
     int32_t get(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, const void* z_dev, const void** h_for_shard) override {
         B2S_TRY(h.alloc(c, (size_t)32 << m->log_domain));
-        B2S_TRY(witness_map_run(c, m, z_dev, h.p));
+        B2S_TRY(witness_map_run(c, m, z_dev, h.p, pk->qap));
         *h_for_shard = h.as<char>() + pk->q[Q_H].off * 32;
         return B2S_OK;
     }
@@ -330,7 +335,7 @@ static int32_t prove_batch_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, uint64
         B2S_TRY(msm(Q_L, g1 + 1 * K, from_z(Q_L), row));
         {
             B2S_TRY(h.alloc(c, (size_t)K * N * fr));
-            B2S_TRY(witness_map_run(c, m, zd, h.p, K, row));
+            B2S_TRY(witness_map_run(c, m, zd, h.p, pk->qap, K, row));
             const Fr* hs = h.as<Fr>() + pk->q[Q_H].off;
             if (h_pre) B2S_TRY(msm(Q_H, g1, hs, N, pk->h_table.p, h_pre));
             else B2S_TRY(msm(Q_H, g1, hs, N));

@@ -143,6 +143,9 @@ static int32_t prove_group(b2s_group* g, const b2s_pk* pk, const b2s_r1cs* m, co
     if (!pk || !m) return fail(ctx, B2S_ERR_MISSING_CS, "prove_group: null key or matrices");
     if ((!z_dev && (!z_inst || (!z_wit && m->n_witness))) || !r || !s) return fail(ctx, B2S_ERR_ASSIGNMENT_MISSING, "prove_group: null assignment");
     if (g->rank == 0 && (!out_a || !out_b || !out_c)) return fail(ctx, B2S_ERR_INVALID_ARG, "prove_group: rank 0 needs the proof buffers");
+    if (pk->qap != B2S_QAP_LIBSNARK)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "prove_group: circom keys have no distributed witness map; prove with b2s_groth16_prove_shard "
+                                              "on each rank and join with b2s_groth16_finish");
     const Sizes z = sizes(ctx);
     const size_t p1 = z.g1x, p2 = z.g2x, per = 4 * p1 + p2;   // XYZZ sizes; one rank's packet
     DevBuf mine, all;

@@ -23,8 +23,10 @@
 // (N entries for the first boundary, N / R1 for the second) and the butterfly twiddles are precomputed per plan
 // (NttFull, 1 GiB per direction at 2^24) and streamed next to the data.  Multiplications per element at 2^24:
 // 10.5 in the butterflies (the last stage of a pass has twiddle 1) + 2 at the boundaries = 12.5, against 14.9 composed.
-// Coset scaling (g^j on the way in, g^-j * N^-1 on the way out) is fused into the first / last pass.
+// Coset scaling (g^j on the way in, g^-j * N^-1 on the way out) is fused into the first / last pass, and so is the odd-coset
+// scaling w2^j / N of the circom witness map (NTT_M_ODD).
 #define B2S_INLINE_MUL 1   // Fr butterflies: the multiplication is the kernel
+#include <cassert>
 #include <memory>
 
 #include "ntt.cuh"
@@ -285,6 +287,40 @@ static int32_t build_full(Ctx* c, NttPlan* pl) {
     return B2S_OK;
 }
 
+// Factors of the odd-coset forward transform (NTT_M_ODD): w2^j / N with w2 the primitive 2N-th root, w2^2 = w.  Built on the
+// first such transform of the size, so that a process that never runs the circom witness map allocates nothing for them: the
+// two-level table (2^ceil(log_n/2) + 2^floor(log_n/2) entries) always, the full N-entry table when the plan has full tables.
+template <class Curve>
+static int32_t build_odd(Ctx* c, NttPlan* pl) {
+    using Fr = typename Curve::Fr;
+    using FrP = typename Curve::FrP;
+    const uint32_t log_n = pl->log_n;
+    // domains stop at 2^27 (r1cs upload, b2s_ntt) and the two-adicity is 28 (BN254) / 32 (BLS12-381): w2 always exists
+    assert(log_n < (uint32_t)FrP::TWO_ADICITY);
+    const uint32_t a = (log_n + 1) / 2, b = log_n - a;
+    const uint32_t nlo = 1u << a, nhi = 1u << b;
+    B2S_TRY(pl->odd_tables.alloc(c, (size_t)(nlo + nhi) * sizeof(Fr)));
+    B2S_FR_CONST(w2, root) B2S_FR_CONST(half, half)
+    for (uint32_t i = log_n + 1; i < (uint32_t)FrP::TWO_ADICITY; i++) w2 = w2.sqr();
+    Fr n_inv = Fr::one();
+    for (uint32_t i = 0; i < log_n; i++) n_inv = n_inv * half;
+    Fr* lo = pl->odd_tables.as<Fr>();
+    B2S_LAUNCH(c, pow_table_kernel<Fr>, cdiv(nlo, 256), 256, 0, lo, nlo, w2, (uint64_t)1, Fr::one());
+    B2S_LAUNCH(c, pow_table_kernel<Fr>, cdiv(nhi, 256), 256, 0, lo + nlo, nhi, w2, 1ull << a, n_inv);
+    pl->odd_in.lo = lo; pl->odd_in.hi = lo + nlo; pl->odd_in.a = a;
+    NttFull* fu = pl->full;
+    if (!fu) return B2S_OK;
+    const uint64_t N = 1ull << log_n;
+    if (fu->odd_buf.alloc(c, N * sizeof(Fr)) != B2S_OK) {   // no room: not an error, the two-level table does
+        c->err.clear();
+        cudaGetLastError();
+        return B2S_OK;
+    }
+    B2S_LAUNCH(c, ntt_scale_table_kernel<Fr>, cdiv(N, 256), 256, 0, fu->odd_buf.as<Fr>(), pl->odd_in, reinterpret_cast<const Fr*>(pl->one), N);
+    fu->odd_pre = fu->odd_buf.p;
+    return B2S_OK;
+}
+
 int32_t ntt_get_full(Ctx* c, uint32_t log_n, NttPlan** out) {
     NttPlan* pl = nullptr;
     *out = nullptr;
@@ -298,12 +334,14 @@ template <class Curve>
 static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode, uint32_t K) {
     using Fr = typename Curve::Fr;
     const bool inverse = (mode & NTT_M_INVERSE) != 0, coset = (mode & NTT_M_COSET) != 0, wm = (mode & NTT_M_WM) != 0;
-    if (log_n == 0 && !wm) return B2S_OK;  // size-1 transform is the identity (coset scaling g^0 = 1, 1/N = 1)
+    const bool odd = (mode & NTT_M_ODD) != 0;
+    if (log_n == 0 && !wm) return B2S_OK;  // size-1 transform is the identity (coset scaling g^0 = 1, 1/N = 1, w2^0 / N = 1)
     NttPlan* pl = nullptr;
     B2S_TRY(ntt_get_plan(c, log_n, &pl));
     if (!pl->full_tried) B2S_TRY(build_full<Curve>(c, pl));
     const NttFull* fu = pl->full;
     if (wm && !fu) return fail(c, B2S_ERR_INVALID_ARG, "ntt: witness-map transform modes need the full-size tables");
+    if (odd && !inverse && !pl->odd_in.lo) B2S_TRY(build_odd<Curve>(c, pl));
     Fr* data = reinterpret_cast<Fr*>(data_dev);
     DevBuf scratch;
     if (pl->npass > 1) B2S_TRY(scratch.alloc(c, (sizeof(Fr) << log_n) * K));
@@ -311,10 +349,11 @@ static int32_t ntt_run_t(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode, 
 
     PowTab none;
     const PowTab tw = inverse ? pl->inv : pl->fwd;
-    const PowTab pre = (coset && !inverse && !wm) ? pl->coset_in : none;
+    const void* odd_full = (odd && !inverse && fu) ? fu->odd_pre : nullptr;
+    const PowTab pre = (coset && !inverse && !wm) ? pl->coset_in : ((odd && !inverse && !odd_full) ? pl->odd_in : none);
     const PowTab post = (inverse && coset && !wm) ? pl->coset_out_scaled : none;
-    const void* post_const = (inverse && !coset && !wm) ? pl->n_inv : nullptr;
-    const void* pre_full = (wm && coset && !inverse) ? fu->wm_pre : nullptr;
+    const void* post_const = (inverse && !coset && !wm && !odd) ? pl->n_inv : nullptr;
+    const void* pre_full = (wm && coset && !inverse) ? fu->wm_pre : odd_full;
     const void* post_full = (wm && coset && inverse) ? fu->wm_post : nullptr;
 
     const size_t smem_bytes = ((size_t)(1u << NTT_TILE_LOG) * 2 + (1u << NTT_MAX_RADIX_LOG) + 2) * sizeof(uint4) +

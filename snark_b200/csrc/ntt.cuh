@@ -27,6 +27,9 @@ struct NttFull {
     const void* wm_pre = nullptr;
     const void* wm_post = nullptr;
     const void* wm_beta = nullptr;   // one element: Zinv / N
+    // circom witness map (NTT_M_ODD): input w2^j / N, built on the first odd-coset transform of the size (N entries)
+    DevBuf odd_buf;
+    const void* odd_pre = nullptr;
 };
 
 struct NttPlan {
@@ -40,6 +43,9 @@ struct NttPlan {
     const void* one = nullptr;     // one element: 1
     bool full_tried = false;
     NttFull* full = nullptr;       // nullptr: factors are composed from the two-level tables
+    // NTT_M_ODD input scaling w2^j / N (w2 = primitive 2N-th root), two-level form; built on the first odd-coset transform
+    DevBuf odd_tables;
+    PowTab odd_in;
     ~NttPlan() { delete full; }
 };
 
@@ -127,7 +133,10 @@ int32_t ntt_get_plan(Ctx* c, uint32_t log_n, NttPlan** out);
 //   WM | INVERSE           inverse transform WITHOUT the 1/N scaling
 //   WM | COSET             forward coset transform whose input scaling is g^j / N   (makes up for the line above)
 //   WM | INVERSE | COSET   inverse coset transform whose output scaling is g^-j * Zinv / N
-enum : uint32_t { NTT_M_INVERSE = 1, NTT_M_COSET = 2, NTT_M_WM = 4 };
+// ODD marks the two variants of the circom witness map (odd coset w2 H, w2 a primitive 2N-th root; full tables optional):
+//   ODD | INVERSE          inverse transform WITHOUT the 1/N scaling
+//   ODD                    forward transform on the odd coset whose input scaling is w2^j / N (makes up for the line above)
+enum : uint32_t { NTT_M_INVERSE = 1, NTT_M_COSET = 2, NTT_M_WM = 4, NTT_M_ODD = 8 };
 // K > 1: K transforms of the vectors data_dev + k * 2^log_n, one launch per pass for all of them
 int32_t ntt_run_mode(Ctx* c, void* data_dev, uint32_t log_n, uint32_t mode, uint32_t K = 1);
 // plan with full-size tables, or *out = nullptr when they are switched off (B2S_NTT_FULL=0) or would not fit

@@ -1,5 +1,5 @@
 // K1: R1CS matrices x assignment (CSR SpMV), K3: the pointwise QAP quotient, and their composition
-// into `witness_map`.
+// into `witness_map`, under either QAP reduction (LibsnarkReduction, or ark-circom's CircomReduction).
 //
 // Replaces, on the GPU:
 //   mat_vec_mul                         /root/reference/relations/src/utils/matrix.rs:26-36
@@ -44,18 +44,18 @@ struct SpmvMat {
     void* out;
 };
 
-// One thread per (matrix, row).  Batch: blockIdx.y is the assignment k, read at z + k * z_stride, its rows written at
-// out + k * out_stride.
-template <class Fr>
+// One thread per (matrix, row) of the first NM matrices: 3 = A, B, C; 2 = A and B only (the circom witness map never reads
+// C).  Batch: blockIdx.y is the assignment k, read at z + k * z_stride, its rows written at out + k * out_stride.
+template <class Fr, int NM>
 __global__ void __launch_bounds__(256)
 spmv_kernel(SpmvMat m0, SpmvMat m1, SpmvMat m2, const Fr* __restrict__ pool, const Fr* __restrict__ z, uint64_t n_rows, uint64_t z_stride,
             uint64_t out_stride) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= 3 * n_rows) return;
+    if (t >= NM * n_rows) return;
     z += blockIdx.y * z_stride;
     const uint32_t k = (uint32_t)(t / n_rows);
     const uint64_t row = t - (uint64_t)k * n_rows;
-    const SpmvMat m = k == 0 ? m0 : (k == 1 ? m1 : m2);
+    const SpmvMat m = k == 0 ? m0 : (k == 1 || NM == 2 ? m1 : m2);
     const uint64_t beg = m.row_ptr[row], end = m.row_ptr[row + 1];
     Fr acc = Fr::zero();
     for (uint64_t e = beg; e < end; e++) {
@@ -87,6 +87,21 @@ __global__ void __launch_bounds__(256) qap_quotient_kernel(Fr* q, const Fr* c, c
     const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     fr_st(q + i, fr_ld(q + i) * fr_ld(alpha) - fr_ld(c + i) * fr_ld(beta));
+}
+
+// circom witness map, after the padding / instance rows: c[i] = a[i] * b[i]   (A z o B z on H; C is never read)
+template <class Fr>
+__global__ void __launch_bounds__(256) qap_prod_kernel(Fr* __restrict__ c, const Fr* __restrict__ a, const Fr* __restrict__ b, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    fr_st(c + i, fr_ld(a + i) * fr_ld(b + i));
+}
+// circom witness map, last step, on odd-coset EVALUATIONS: h[j] = a[j] * b[j] - c[j]   (in place over a)
+template <class Fr>
+__global__ void __launch_bounds__(256) qap_circom_h_kernel(Fr* a, const Fr* __restrict__ b, const Fr* __restrict__ c, uint64_t n) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    fr_st(a + i, fr_ld(a + i) * fr_ld(b + i) - fr_ld(c + i));
 }
 
 // -------------------------------------------------------------------------------------------
@@ -183,6 +198,7 @@ int32_t r1cs_upload(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_wit
     });
 }
 
+// oc == nullptr: A and B only
 template <class Curve>
 static int32_t spmv_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* oa, void* ob, void* oc, uint32_t K = 1, uint64_t z_stride = 0,
                       uint64_t out_stride = 0) {
@@ -190,10 +206,17 @@ static int32_t spmv_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* oa, vo
     if (m->n_rows == 0) return B2S_OK;
     SpmvMat mm[3];
     void* outs[3] = {oa, ob, oc};
+    const int nm = oc ? 3 : 2;
     for (int k = 0; k < 3; k++)
-        mm[k] = SpmvMat{m->row_ptr[k].as<uint64_t>(), m->col[k].as<uint32_t>(), m->coeff_id[k].as<uint32_t>(), outs[k]};
-    B2S_LAUNCH(c, spmv_kernel<Fr>, dim3(cdiv(3 * m->n_rows, 256), K), 256, 0, mm[0], mm[1], mm[2], m->pool.as<Fr>(),
-               reinterpret_cast<const Fr*>(z_dev), m->n_rows, z_stride, out_stride);
+        mm[k] = k < nm ? SpmvMat{m->row_ptr[k].as<uint64_t>(), m->col[k].as<uint32_t>(), m->coeff_id[k].as<uint32_t>(), outs[k]} : SpmvMat{};
+    auto* const spmv3 = spmv_kernel<Fr, 3>;
+    auto* const spmv2 = spmv_kernel<Fr, 2>;
+    if (nm == 3)
+        B2S_LAUNCH_N(c, "spmv_kernel<Fr>", spmv3, dim3(cdiv(3 * m->n_rows, 256), K), 256, 0, mm[0], mm[1], mm[2], m->pool.as<Fr>(),
+                   reinterpret_cast<const Fr*>(z_dev), m->n_rows, z_stride, out_stride);
+    else
+        B2S_LAUNCH_N(c, "spmv_kernel<Fr> A,B", spmv2, dim3(cdiv(2 * m->n_rows, 256), K), 256, 0, mm[0], mm[1], mm[2], m->pool.as<Fr>(),
+                   reinterpret_cast<const Fr*>(z_dev), m->n_rows, z_stride, out_stride);
     return B2S_OK;
 }
 
@@ -244,8 +267,42 @@ static int32_t witness_map_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void*
     return B2S_OK;
 }
 
-int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, uint32_t K, uint64_t z_stride) {
-    return dispatch_curve(c, [&](auto curve) { return witness_map_t<decltype(curve)>(c, m, z_dev, h_dev, K, z_stride); });
+// h = ark-circom CircomReduction::witness_map: the N evaluations of A B - C' on the odd coset w2 H (w2 a primitive 2N-th root,
+// w2^2 = w), where C' interpolates (A z) o (B z) on H.  C is never read, and nothing is divided by Z (it is the constant
+// w2^N - 1 = -2 there; the circom h query, the odd-indexed Lagrange basis of the size-2N domain, absorbs it).  a and b are
+// A z and B z with the instance rows in a, c = a o b pointwise on H, then each of a, b, c goes to the odd coset by an
+// unscaled inverse transform and a forward transform whose input scaling is w2^j / N: six transforms, none of them a closing
+// inverse.  The batch layout is that of witness_map_t.
+template <class Curve>
+static int32_t witness_map_circom_t(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, uint32_t K, uint64_t z_stride) {
+    using Fr = typename Curve::Fr;
+    const uint64_t N = 1ull << m->log_domain;
+    Fr* a = reinterpret_cast<Fr*>(h_dev);
+    DevBuf bb, cb;
+    B2S_TRY(bb.alloc(c, K * N * sizeof(Fr)));
+    B2S_TRY(cb.alloc(c, K * N * sizeof(Fr)));
+    Fr* b = bb.as<Fr>();
+    Fr* cc = cb.as<Fr>();
+    const size_t pitch = N * sizeof(Fr), pad = (N - m->n_rows) * sizeof(Fr);
+    B2S_CUDA(c, cudaMemset2DAsync(a + m->n_rows, pitch, 0, pad, K, c->stream));
+    B2S_CUDA(c, cudaMemset2DAsync(b + m->n_rows, pitch, 0, pad, K, c->stream));
+    B2S_TRY(spmv_t<Curve>(c, m, z_dev, a, b, nullptr, K, z_stride, N));
+    B2S_LAUNCH(c, copy_instance_kernel<Fr>, dim3(cdiv(m->n_instance, 256), K), 256, 0, a, reinterpret_cast<const Fr*>(z_dev),
+               m->n_rows, m->n_instance, z_stride, N);
+    B2S_LAUNCH(c, qap_prod_kernel<Fr>, cdiv(K * N, 256), 256, 0, cc, (const Fr*)a, (const Fr*)b, K * N);
+    Fr* bufs[3] = {a, b, cc};
+    for (Fr* v : bufs) B2S_TRY(ntt_run_mode(c, v, m->log_domain, NTT_M_INVERSE | NTT_M_ODD, K));
+    for (Fr* v : bufs) B2S_TRY(ntt_run_mode(c, v, m->log_domain, NTT_M_ODD, K));
+    B2S_LAUNCH(c, qap_circom_h_kernel<Fr>, cdiv(K * N, 256), 256, 0, a, (const Fr*)b, (const Fr*)cc, K * N);
+    return B2S_OK;
+}
+
+int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, int32_t qap, uint32_t K, uint64_t z_stride) {
+    return dispatch_curve(c, [&](auto curve) {
+        using C = decltype(curve);
+        return qap == B2S_QAP_CIRCOM ? witness_map_circom_t<C>(c, m, z_dev, h_dev, K, z_stride)
+                                     : witness_map_t<C>(c, m, z_dev, h_dev, K, z_stride);
+    });
 }
 
 }  // namespace b2s

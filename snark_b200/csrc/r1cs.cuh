@@ -43,6 +43,9 @@ struct PkQuery {
 
 struct b2s_pk {
     uint64_t n_instance = 0, n_witness = 0, domain_size = 0;
+    // the QAP reduction the key was made for (B2S_QAP_LIBSNARK / B2S_QAP_CIRCOM), fixed when the handle is created: it selects
+    // the witness map of every proof under the key and the length of a full key's h query
+    int32_t qap = B2S_QAP_LIBSNARK;
     b2s::DevBuf consts_g1;            // alpha_g1, beta_g1, delta_g1 (affine)
     b2s::DevBuf consts_g2;            // beta_g2, delta_g2 (affine)
     b2s::PkQuery q[b2s::PK_QUERIES];  // indexed by PkQueryId
@@ -52,12 +55,15 @@ struct b2s_pk {
 };
 
 namespace b2s {
-// a full (unsharded) key: every query covers its whole vector, h being domain_size - 1 long
+// length of a full key's h query: tau^i Z(tau) / delta for i < domain_size - 1 (libsnark), or the domain_size odd-indexed
+// Lagrange points of the size-2N domain (circom)
+inline uint64_t pk_full_h_len(int32_t qap, uint64_t domain_size) { return qap == B2S_QAP_CIRCOM ? domain_size : domain_size - 1; }
+// a full (unsharded) key: every query covers its whole vector
 inline bool pk_is_full(const b2s_pk* pk) {
     const uint64_t n_vars = pk->n_instance + pk->n_witness;
     const PkQuery* q = pk->q;
     return q[Q_A].len == n_vars && q[Q_B_G1].len == n_vars && q[Q_B_G2].len == n_vars && q[Q_L].len == pk->n_witness &&
-           q[Q_H].len + 1 == pk->domain_size;
+           q[Q_H].len == pk_full_h_len(pk->qap, pk->domain_size);
 }
 
 int32_t r1cs_upload(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness, const uint64_t* const row_ptr[3],
@@ -68,11 +74,12 @@ int32_t r1cs_upload_lcmap(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t
                           const void* pool, uint32_t pool_len, b2s_r1cs** out);
 // out_k: device arrays with at least n_rows elements each
 int32_t spmv_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* out_a, void* out_b, void* out_c);
-// h_dev: device array of domain elements (output); z_dev: n_instance + n_witness elements.  K > 1: K assignments at
-// z_dev + k * z_stride (elements) give K vectors h_dev + k * domain, with the launches of one
-int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, uint32_t K = 1, uint64_t z_stride = 0);
-int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, b2s_pk** out);
-int32_t groth16_setup(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
+// h_dev: device array of domain elements (output); z_dev: n_instance + n_witness elements; qap: the reduction (libsnark: h's
+// coefficients, circom: its odd-coset evaluations).  K > 1: K assignments at z_dev + k * z_stride (elements) give K vectors
+// h_dev + k * domain, with the launches of one
+int32_t witness_map_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* h_dev, int32_t qap, uint32_t K = 1, uint64_t z_stride = 0);
+int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, int32_t qap, b2s_pk** out);
+int32_t groth16_setup(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, int32_t qap, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
                       void* o_gamma_g2, void* o_delta_g2, void* o_gamma_abc);
 int32_t pk_query_download(Ctx* c, const b2s_pk* pk, int which, void* out_host, uint64_t cap_bytes);
 // Where the h-query MSM of a shard takes its scalars from: the default computes the whole h on this GPU (replicated

@@ -11,7 +11,12 @@
 //   a_query[j] = A_j(tau) G1, b_g1/g2_query[j] = B_j(tau) G1/G2, h_query[i] = tau^i Z(tau)/delta G1,
 //   l_query[j] = (beta A_j + alpha B_j + C_j)/delta G1 (witness j), gamma_abc_g1[j] = (...)/gamma G1 (instance j)
 //            all through the fixed-base kernel (setup.cu)
+// Under ark-circom's CircomReduction (snarkjs keys) only the h query differs: h_query[j] = L^(2N)_{2j+1}(tau)/delta G1, j < N,
+// the odd-indexed Lagrange basis of the size-2N domain at tau (w2 = primitive 2N-th root):
+//   L^(2N)_{2j+1}(tau) = (tau^2N - 1) w2^(2j+1) / (2N (tau - w2^(2j+1)))
 #define B2S_INLINE_MUL 1   // Fr only
+#include <cassert>
+
 #include "r1cs.cuh"
 
 namespace b2s {
@@ -106,8 +111,17 @@ __global__ void h_scalars_kernel(SetupConsts<Fr> k, uint64_t count, Fr* __restri
     hq[i] = k.zt_dinv * k.tau.pow_u64(i);
 }
 
+// circom h query scalars, one thread per j < N: scale * x / (tau - x), x = w2^(2j+1), scale = (tau^2N - 1) / (2N delta)
+template <class Fr>
+__global__ void h_scalars_circom_kernel(Fr tau, Fr w2, Fr scale, uint64_t N, Fr* __restrict__ hq) {
+    const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= N) return;
+    const Fr x = w2.pow_u64(2 * j + 1);
+    hq[j] = scale * x * (tau - x).inverse();
+}
+
 template <class Curve>
-static int32_t setup_t(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
+static int32_t setup_t(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, int32_t qap, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
                        void* o_gamma_g2, void* o_delta_g2, void* o_gamma_abc) {
     using Fr = typename Curve::Fr;
     using FrP = typename Curve::FrP;
@@ -131,6 +145,17 @@ static int32_t setup_t(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s
     for (uint32_t i = 0; i < m->log_domain; i++) n_inv = n_inv * half;
     k.dinv = k.delta.inverse(); k.ginv = k.gamma.inverse();
     k.zt_over_n = zt * n_inv; k.zt_dinv = zt * k.dinv;
+    // circom: w2 (w2^2 = w; domains stop at 2^27 below both two-adicities) and (tau^2N - 1) / (2N delta)
+    Fr w2, circom_scale;
+    HostWipe wipe_cs{&circom_scale, sizeof(circom_scale)};
+    if (qap == B2S_QAP_CIRCOM) {
+        assert(m->log_domain < (uint32_t)FrP::TWO_ADICITY);
+        for (int i = 0; i < Fr::N; i++) w2.v[i] = FrP::root(i);
+        for (uint32_t i = m->log_domain + 1; i < (uint32_t)FrP::TWO_ADICITY; i++) w2 = w2.sqr();
+        const Fr zt2 = (zt + Fr::one()).sqr() - Fr::one();   // tau^2N - 1
+        if (zt2.is_zero()) return fail(c, B2S_ERR_DIVISION_BY_ZERO, "setup: tau^(2N) = 1 (circom h query)");
+        circom_scale = zt2 * n_inv * half * k.dinv;
+    }
 
     DevBuf u, abc3, lq, gabc, hq;
     u.secret = abc3.secret = lq.secret = gabc.secret = hq.secret = true;   // powers of tau, delta^-1, ...
@@ -166,7 +191,9 @@ static int32_t setup_t(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s
     B2S_TRY(gabc.alloc(c, ell * sizeof(Fr)));
     B2S_TRY(hq.alloc(c, N * sizeof(Fr)));
     B2S_LAUNCH(c, query_scalars_kernel<Fr>, cdiv(n_vars, 128), 128, 0, k, n_rows, ell, n_vars, u.as<Fr>(), a, b, cc, lq.as<Fr>(), gabc.as<Fr>());
-    B2S_LAUNCH(c, h_scalars_kernel<Fr>, cdiv(N - 1, 128), 128, 0, k, N - 1, hq.as<Fr>());
+    const uint64_t h_len = pk_full_h_len(qap, N);
+    if (qap == B2S_QAP_CIRCOM) B2S_LAUNCH(c, h_scalars_circom_kernel<Fr>, cdiv(N, 128), 128, 0, k.tau, w2, circom_scale, N, hq.as<Fr>());
+    else B2S_LAUNCH(c, h_scalars_kernel<Fr>, cdiv(N - 1, 128), 128, 0, k, N - 1, hq.as<Fr>());
     // group part
     const size_t g1 = sizeof(typename Curve::G1Affine), g2 = sizeof(typename Curve::G2Affine);
     DevBuf qa, qb1, qb2, qh, ql, qabc, k1, k2, ks;
@@ -176,7 +203,7 @@ static int32_t setup_t(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s
     B2S_TRY(fixed_base_run(c, 1, a, n_vars, true, qa.p));
     B2S_TRY(fixed_base_run(c, 1, b, n_vars, true, qb1.p));
     B2S_TRY(fixed_base_run(c, 2, b, n_vars, true, qb2.p));
-    B2S_TRY(fixed_base_run(c, 1, hq.p, N - 1, true, qh.p));
+    B2S_TRY(fixed_base_run(c, 1, hq.p, h_len, true, qh.p));
     B2S_TRY(fixed_base_run(c, 1, lq.p, mw, true, ql.p));
     B2S_TRY(fixed_base_run(c, 1, gabc.p, ell, true, qabc.p));
     // constants: G1 [alpha, beta, delta], G2 [beta, gamma, delta]
@@ -201,14 +228,14 @@ static int32_t setup_t(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s
     d.n_instance = ell; d.n_witness = mw; d.domain_size = N;
     d.alpha_g1 = p1; d.beta_g1 = p1 + g1; d.delta_g1 = p1 + 2 * g1; d.beta_g2 = p2; d.delta_g2 = p2 + 2 * g2;
     d.a_query = qa.p; d.a_len = n_vars; d.b_g1_query = qb1.p; d.b1_len = n_vars; d.b_g2_query = qb2.p; d.b2_len = n_vars;
-    d.h_query = qh.p; d.h_len = N - 1; d.l_query = ql.p; d.l_len = mw;
-    return pk_upload(c, &d, B2S_MEM_DEVICE, out_pk);
+    d.h_query = qh.p; d.h_len = h_len; d.l_query = ql.p; d.l_len = mw;
+    return pk_upload(c, &d, B2S_MEM_DEVICE, qap, out_pk);
 }
 
-int32_t groth16_setup(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
+int32_t groth16_setup(Ctx* c, const b2s_r1cs* m, const void* trapdoor_host, int32_t qap, b2s_pk** out_pk, void* o_alpha_g1, void* o_beta_g2,
                       void* o_gamma_g2, void* o_delta_g2, void* o_gamma_abc) {
     return dispatch_curve(c, [&](auto curve) {
-        return setup_t<decltype(curve)>(c, m, trapdoor_host, out_pk, o_alpha_g1, o_beta_g2, o_gamma_g2, o_delta_g2, o_gamma_abc);
+        return setup_t<decltype(curve)>(c, m, trapdoor_host, qap, out_pk, o_alpha_g1, o_beta_g2, o_gamma_g2, o_delta_g2, o_gamma_abc);
     });
 }
 

@@ -9,6 +9,7 @@ import numpy as np
 
 BLS12_381, BN254 = 0, 1
 MEM_HOST, MEM_DEVICE = 0, 1
+QAP_LIBSNARK, QAP_CIRCOM = 0, 1   # QAP reduction of a Groth16 key: ark-groth16's LibsnarkReduction / ark-circom's CircomReduction
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -60,11 +61,14 @@ SIGNATURES = {
     "b2s_r1cs_free": (None, [c_void_p, c_void_p]),
     "b2s_spmv": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_void_p, c_void_p, c_void_p]),
     "b2s_witness_map": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_void_p]),
+    "b2s_witness_map_qap": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p]),
     "b2s_r1cs_domain_size": (c_uint64, [c_void_p]),
     "b2s_witness_map_sim": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_uint32, c_void_p]),
     "b2s_pk_upload": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, POINTER(c_void_p)]),
+    "b2s_pk_upload_qap": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_pk_free": (None, [c_void_p, c_void_p]),
     "b2s_groth16_setup": (c_int32, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p)] + [c_void_p] * 5),
+    "b2s_groth16_setup_qap": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, POINTER(c_void_p)] + [c_void_p] * 5),
     "b2s_pk_query": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_uint64]),
     "b2s_groth16_prove": (c_int32, [c_void_p] * 10),
     "b2s_groth16_prove_shard": (c_int32, [c_void_p] * 9),
@@ -92,6 +96,7 @@ SIGNATURES = {
     "b2s_vk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32] + [c_void_p] * 5
                            + [c_uint64, POINTER(c_uint64), POINTER(c_uint64)]),
     "b2s_pk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, POINTER(c_void_p)]),
+    "b2s_pk_deserialize_qap": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_vk_prepare": (c_int32, [c_void_p] * 6 + [c_uint64, POINTER(c_void_p)]),
     "b2s_pvk_free": (None, [c_void_p, c_void_p]),
     "b2s_groth16_verify_batch": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_int32,
@@ -305,11 +310,15 @@ class Backend:
         self._ck(self.lib.b2s_spmv(self.h, m, pz, mem, *[o.ctypes.data for o in outs]))
         return outs
 
-    def witness_map(self, m, z):
+    def witness_map(self, m, z, qap=QAP_LIBSNARK):
+        """h of the reduction `qap` (domain_size elements): libsnark coefficients, or circom odd-coset evaluations."""
         pz, mem = _ptr(z)
         assert mem == MEM_HOST
         h = np.zeros(self.domain_size(m) * 8, dtype=np.uint32)
-        self._ck(self.lib.b2s_witness_map(self.h, m, pz, mem, h.ctypes.data))
+        if qap == QAP_LIBSNARK:
+            self._ck(self.lib.b2s_witness_map(self.h, m, pz, mem, h.ctypes.data))
+        else:
+            self._ck(self.lib.b2s_witness_map_qap(self.h, m, pz, mem, qap, h.ctypes.data))
         return h
 
     def witness_map_sim(self, m, z, log_ranks):
@@ -321,20 +330,27 @@ class Backend:
         return h
 
     # ---- Groth16 ------------------------------------------------------------------------------
-    def pk_upload(self, desc: PkDesc, mem=MEM_HOST):
+    def pk_upload(self, desc: PkDesc, mem=MEM_HOST, qap=QAP_LIBSNARK):
         h = c_void_p()
-        self._ck(self.lib.b2s_pk_upload(self.h, ctypes.byref(desc), mem, ctypes.byref(h)))
+        if qap == QAP_LIBSNARK:
+            self._ck(self.lib.b2s_pk_upload(self.h, ctypes.byref(desc), mem, ctypes.byref(h)))
+        else:
+            self._ck(self.lib.b2s_pk_upload_qap(self.h, ctypes.byref(desc), mem, qap, ctypes.byref(h)))
         return h
 
-    def groth16_setup(self, m, trapdoor, n_instance):
-        """trapdoor: uint32[5*8] Montgomery (tau, alpha, beta, gamma, delta) -> (pk handle, vk dict of numpy arrays)."""
+    def groth16_setup(self, m, trapdoor, n_instance, qap=QAP_LIBSNARK):
+        """trapdoor: uint32[5*8] Montgomery (tau, alpha, beta, gamma, delta) -> (pk handle, vk dict of numpy arrays).
+        qap: the key's reduction (QAP_CIRCOM: the N-point circom h query)."""
         h = c_void_p()
         vk = {"alpha_g1": np.zeros(self.g1_bytes // 4, dtype=np.uint32), "beta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
               "gamma_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32), "delta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
               "gamma_abc_g1": np.zeros(max(n_instance, 1) * self.g1_bytes // 4, dtype=np.uint32)}
-        self._ck(self.lib.b2s_groth16_setup(self.h, m, trapdoor.ctypes.data, ctypes.byref(h), vk["alpha_g1"].ctypes.data,
-                                            vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data, vk["delta_g2"].ctypes.data,
-                                            vk["gamma_abc_g1"].ctypes.data))
+        outs = (vk["alpha_g1"].ctypes.data, vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data, vk["delta_g2"].ctypes.data,
+                vk["gamma_abc_g1"].ctypes.data)
+        if qap == QAP_LIBSNARK:
+            self._ck(self.lib.b2s_groth16_setup(self.h, m, trapdoor.ctypes.data, ctypes.byref(h), *outs))
+        else:
+            self._ck(self.lib.b2s_groth16_setup_qap(self.h, m, trapdoor.ctypes.data, qap, ctypes.byref(h), *outs))
         return h, vk
 
     def pk_query(self, pk, which, count):
@@ -404,11 +420,16 @@ class Backend:
         vk["gamma_abc_g1"] = vk["gamma_abc_g1"][: n.value * self.g1_bytes // 4]
         return vk, used.value
 
-    def pk_from_bytes(self, data, compressed=True, validate=True):
-        """ark-groth16 ProvingKey bytes -> device-resident full key handle (as pk_upload returns)."""
+    def pk_from_bytes(self, data, compressed=True, validate=True, qap=QAP_LIBSNARK):
+        """ark-groth16 ProvingKey bytes -> device-resident full key handle (as pk_upload returns).  qap=QAP_CIRCOM reads the
+        bytes of a Groth16<E, CircomReduction> key (|h_query| = domain size)."""
         buf = np.frombuffer(bytes(data), dtype=np.uint8)
         h = c_void_p()
-        self._ck(self.lib.b2s_pk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), ctypes.byref(h)))
+        if qap == QAP_LIBSNARK:
+            self._ck(self.lib.b2s_pk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), ctypes.byref(h)))
+        else:
+            self._ck(self.lib.b2s_pk_deserialize_qap(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), qap,
+                                                     ctypes.byref(h)))
         return h
 
     def pk_free(self, pk):
