@@ -9,6 +9,7 @@
  *   instance_assignment() / witness_assignment()         relations/src/gr1cs/constraint_system.rs:193-206
  *   Matrix<F>, mat_vec_mul                               relations/src/utils/matrix.rs:4,26-36
  *   Sr1csAdapter::evaluate_constraint                    relations/src/sr1cs/mod.rs:24-56
+ *   ConstraintSystem::is_satisfied / which_is_unsatisfied relations/src/gr1cs/constraint_system.rs:652-687
  *   SynthesisError (status codes)                        relations/src/utils/error.rs:5-21
  *   (out of tree, SURVEY.md App. A)  ark-poly Radix2EvaluationDomain::{fft,ifft}, get_coset;
  *                                    ark-ec VariableBaseMSM::msm; ark-groth16 prover / generator
@@ -168,6 +169,51 @@ uint64_t b2s_r1cs_domain_size(const b2s_r1cs* m);
  * Exists so that the index algebra of the multi-GPU path is checked bit for bit on a one-GPU box; B2S_ERR_INVALID_ARG
  * when the domain cannot be cut that way (log2(domain) odd, or too few rows per rank). */
 int32_t b2s_witness_map_sim(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, uint32_t log_ranks, void* out_h);
+
+/* ---- constraint satisfaction (ConstraintSystem::is_satisfied / which_is_unsatisfied) ------------------------------------
+ * The check of relations/src/gr1cs/constraint_system.rs:652-687 (-> predicate/mod.rs:185-204 -> polynomial_constraint.rs:46-48)
+ * on the GPU, for one assignment or a batch: constraint i of a polynomial predicate is satisfied when its polynomial, evaluated
+ * at the arity row products <M_j row i, z>, is 0 mod r.  One thread per (constraint, assignment); the CSR reads are those of
+ * b2s_spmv.  A prover computes a proof for any z (the witness map is defined for every assignment), so a service can run this
+ * first and keep bad witnesses out of b2s_groth16_prove_batch.
+ *   b2s_gr1cs_upload  the predicates of a GR1CS as to_matrices() (BTreeMap<Label, Vec<Matrix>>, one matrix per argument) and
+ *                     get_all_predicate_types() (Predicate::Polynomial: terms, num_vars) return them; pass them in label order
+ *                     to get the reference's order.  Coefficients of all matrices share one interned pool.  Errors as for
+ *                     b2s_r1cs_upload: B2S_ERR_INVALID_ARG for an arity of 0 or above B2S_GR1CS_MAX_ARITY (rejected, never
+ *                     truncated: the arguments live in registers), factor_var >= arity, term_offsets or row_ptr not monotone or
+ *                     not starting at 0, null pointers (b2s_last_error names the predicate and the index);
+ *                     B2S_ERR_ASSIGNMENT_MISSING for a column >= n_instance + n_witness; B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE for
+ *                     more than 2^32 variables (columns are u32) or 2^32 or more constraints in one predicate.  HOST pointers.
+ *   b2s_gr1cs_check   which_is_unsatisfied for n_assign assignments (below).  A handle from another curve's ctx is
+ *                     B2S_ERR_INVALID_ARG.
+ *   b2s_r1cs_check    the same on a Groth16 handle, with the R1CS predicate x0 * x1 - x2 over its A, B, C (n_predicates = 1).
+ *                     A handle whose C was left empty for the circom reduction checks a * b = 0.
+ * z: n_assign rows of n_instance + n_witness Montgomery Fr (z[0] = 1, as for b2s_groth16_prove_batch).
+ * first_unsat[i * n_predicates + p] = the index of the first constraint of predicate p (upload order) that assignment i does not
+ * satisfy, or UINT64_MAX; n_unsat (may be NULL) the number of such constraints, same layout.  z and the outputs share `mem`; host
+ * batches go through bounded device scratch in chunks.  n_assign == 0 -> B2S_OK, nothing written.  An unsatisfied assignment is
+ * a result, not an error. */
+#define B2S_GR1CS_MAX_ARITY 8
+typedef struct b2s_gr1cs b2s_gr1cs;        /* device-resident predicates of a GR1CS (to_matrices() + get_all_predicate_types()) */
+typedef struct b2s_predicate_desc {
+    uint32_t arity;                        /* 1..B2S_GR1CS_MAX_ARITY (PolynomialPredicate::arity = num_vars) */
+    uint32_t n_terms;                      /* 0 = the zero polynomial: every constraint satisfied */
+    const void* term_coeffs;               /* n_terms Montgomery Fr */
+    const uint32_t* term_offsets;          /* n_terms + 1; term t = coeff_t * prod over [off_t, off_t+1) of x[var]^pow */
+    const uint32_t* factor_var;            /* < arity */
+    const uint32_t* factor_pow;            /* any u32; x^0 = 1 (ark-poly SparseTerm) */
+    uint64_t n_rows;                       /* this predicate's num_constraints */
+    const uint64_t* row_ptr[B2S_GR1CS_MAX_ARITY];   /* argument j's matrix, CSR exactly as b2s_r1cs_upload, j < arity */
+    const uint32_t* col[B2S_GR1CS_MAX_ARITY];
+    const void* coeff[B2S_GR1CS_MAX_ARITY];
+} b2s_predicate_desc;
+int32_t b2s_gr1cs_upload(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates,
+                         const b2s_predicate_desc* preds, b2s_gr1cs** out);
+void b2s_gr1cs_free(b2s_ctx* ctx, b2s_gr1cs* g);
+int32_t b2s_gr1cs_check(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem,
+                        uint64_t* first_unsat, uint64_t* n_unsat);
+int32_t b2s_r1cs_check(b2s_ctx* ctx, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem,
+                       uint64_t* first_unsat, uint64_t* n_unsat);
 
 /* ---- Groth16 (ark-groth16 ProvingKey / create_proof_with_reduction, SURVEY App. A.1) ------------
  * Query vectors are affine point arrays in HOST or DEVICE memory (`mem`); they are copied to the GPU.

@@ -4,8 +4,10 @@ use std::os::raw::c_void;
 
 use ark_ec::{pairing::Pairing, AffineRepr};
 use ark_groth16::{Groth16, PreparedVerifyingKey, Proof, ProvingKey, VerifyingKey};
+use ark_ff::PrimeField;
 use ark_relations::gr1cs::{
-    ConstraintSynthesizer, ConstraintSystem, Matrix, OptimizationGoal, SynthesisError, R1CS_PREDICATE_LABEL,
+    predicate::Predicate, ConstraintSynthesizer, ConstraintSystem, Label, Matrix, OptimizationGoal, SynthesisError,
+    R1CS_PREDICATE_LABEL,
 };
 use ark_snark::{CircuitSpecificSetupSNARK, SNARK};
 use ark_std::{rand::{CryptoRng, RngCore}, UniformRand};
@@ -14,6 +16,18 @@ use ark_std::{rand::{CryptoRng, RngCore}, UniformRand};
 #[repr(C)] pub struct B2sR1cs { _p: [u8; 0] }
 #[repr(C)] pub struct B2sPk { _p: [u8; 0] }
 #[repr(C)] pub struct B2sPvk { _p: [u8; 0] }
+#[repr(C)] pub struct B2sGr1cs { _p: [u8; 0] }
+
+/// Widest predicate the satisfaction check takes (its arguments live in registers); wider ones are rejected.
+pub const B2S_GR1CS_MAX_ARITY: usize = 8;
+#[repr(C)]
+pub struct B2sPredicateDesc {
+    pub arity: u32, pub n_terms: u32,
+    pub term_coeffs: *const c_void, pub term_offsets: *const u32, pub factor_var: *const u32, pub factor_pow: *const u32,
+    pub n_rows: u64,
+    pub row_ptr: [*const u64; B2S_GR1CS_MAX_ARITY], pub col: [*const u32; B2S_GR1CS_MAX_ARITY],
+    pub coeff: [*const c_void; B2S_GR1CS_MAX_ARITY],
+}
 
 #[repr(C)]
 pub struct B2sPkDesc {
@@ -101,6 +115,13 @@ extern "C" {
                        n: u64, mem: i32) -> i32;
     pub fn b2s_poly_geom(ctx: *mut B2sCtx, c: *const c_void, s: *const c_void, n: u64, mem: i32, out: *mut c_void) -> i32;
     pub fn b2s_poly_eval(ctx: *mut B2sCtx, coeffs: *const c_void, n: u64, z: *const c_void, mem: i32, out: *mut c_void) -> i32;
+    pub fn b2s_gr1cs_upload(ctx: *mut B2sCtx, n_instance: u64, n_witness: u64, n_predicates: u32, preds: *const B2sPredicateDesc,
+                            out: *mut *mut B2sGr1cs) -> i32;
+    pub fn b2s_gr1cs_free(ctx: *mut B2sCtx, g: *mut B2sGr1cs);
+    pub fn b2s_gr1cs_check(ctx: *mut B2sCtx, g: *const B2sGr1cs, n_assign: u64, z: *const c_void, mem: i32, first_unsat: *mut u64,
+                           n_unsat: *mut u64) -> i32;
+    pub fn b2s_r1cs_check(ctx: *mut B2sCtx, m: *const B2sR1cs, n_assign: u64, z: *const c_void, mem: i32, first_unsat: *mut u64,
+                          n_unsat: *mut u64) -> i32;
 }
 #[repr(C)]
 pub struct B2sGroup {
@@ -454,3 +475,98 @@ impl<E: Pairing + B200Curve> CircuitSpecificSetupSNARK<E::ScalarField> for Groth
 
 // e.g. in the application:  impl B200Curve for ark_bls12_381::Bls12_381 { const CURVE_ID: i32 = 0; }
 //                           impl B200Curve for ark_bn254::Bn254 { const CURVE_ID: i32 = 1; }
+
+/// `ConstraintSystem::is_satisfied` / `which_is_unsatisfied` (relations/src/gr1cs/constraint_system.rs:652-687) on the GPU:
+/// the predicates of a finalized constraint system, uploaded once per circuit shape, checked against any assignment of the
+/// same shape.  `F` is fixed at upload, so an assignment of another field does not type-check.
+pub struct Gr1csB200<F: PrimeField> {
+    pub ctx: *mut B2sCtx,
+    pub g: *mut B2sGr1cs,
+    pub labels: Vec<Label>,
+    /// n_instance + n_witness: the length of every assignment
+    pub n_vars: usize,
+    _f: core::marker::PhantomData<F>,
+}
+
+/// `B2S_ERR_INVALID_ARG`
+const ERR_INVALID_ARG: i32 = 16;
+
+impl<F: PrimeField> Gr1csB200<F> {
+    /// Uploads `cs.to_matrices()` (one matrix per argument) and `cs.get_all_predicate_types()` (the polynomial of each
+    /// predicate), in the BTreeMap's label order.  `curve_id`: 0 = BLS12-381, 1 = BN254; it must be `F`'s curve
+    /// (checked by the modulus size: 255 / 254 bits).  A predicate that is not polynomial (`Predicate` is `#[non_exhaustive]`,
+    /// predicate/mod.rs:19-25) is `B200Error::Backend(B2S_ERR_INVALID_ARG)`.
+    pub fn upload(curve_id: i32, cs: &ConstraintSystem<F>) -> Result<Self, B200Error> {
+        let bits = match curve_id { 0 => 255, 1 => 254, _ => return Err(B200Error::Backend(ERR_INVALID_ARG)) };
+        if F::MODULUS_BIT_SIZE != bits || core::mem::size_of::<F>() != 32 { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        let mats = cs.to_matrices()?;
+        let types = cs.get_all_predicate_types();
+        // per predicate: (arity, coefficients, term offsets, factor variables, factor powers) and its CSR matrices
+        let mut terms = Vec::new();
+        let mut csrs = Vec::new();
+        let mut labels = Vec::new();
+        for (label, ms) in &mats {
+            let p = match types.get(label) {
+                Some(Predicate::Polynomial(p)) => p,
+                _ => return Err(B200Error::Backend(ERR_INVALID_ARG)),
+            };
+            let (mut co, mut off, mut var, mut pow) = (Vec::new(), vec![0u32], Vec::new(), Vec::new());
+            for (c, term) in &p.polynomial.terms {
+                co.push(*c);
+                for (v, e) in term.iter() { var.push(*v as u32); pow.push(*e as u32); }
+                off.push(var.len() as u32);
+            }
+            terms.push((p.polynomial.num_vars as u32, co, off, var, pow));
+            csrs.push(ms.iter().map(to_csr).collect::<Vec<_>>());
+            labels.push(label.clone());
+        }
+        let descs: Vec<B2sPredicateDesc> = terms.iter().zip(&csrs).map(|((arity, co, off, var, pow), csr)| {
+            let mut d = B2sPredicateDesc {
+                arity: *arity, n_terms: co.len() as u32, term_coeffs: co.as_ptr().cast(), term_offsets: off.as_ptr(),
+                factor_var: var.as_ptr(), factor_pow: pow.as_ptr(), n_rows: csr.first().map_or(0, |m| m.0.len() as u64 - 1),
+                row_ptr: [core::ptr::null(); B2S_GR1CS_MAX_ARITY], col: [core::ptr::null(); B2S_GR1CS_MAX_ARITY],
+                coeff: [core::ptr::null(); B2S_GR1CS_MAX_ARITY],
+            };
+            for (j, m) in csr.iter().take(B2S_GR1CS_MAX_ARITY).enumerate() {
+                d.row_ptr[j] = m.0.as_ptr();
+                d.col[j] = m.1.as_ptr();
+                d.coeff[j] = m.2.as_ptr().cast();
+            }
+            d
+        }).collect();
+        let n_vars = cs.num_instance_variables() + cs.num_witness_variables();
+        let mut ctx: *mut B2sCtx = core::ptr::null_mut();
+        check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
+        let mut g: *mut B2sGr1cs = core::ptr::null_mut();
+        let st = unsafe {
+            b2s_gr1cs_upload(ctx, cs.num_instance_variables() as u64, cs.num_witness_variables() as u64, descs.len() as u32,
+                             descs.as_ptr(), &mut g)
+        };
+        if st != 0 { unsafe { b2s_ctx_destroy(ctx) }; }
+        check(ctx, st)?;
+        Ok(Gr1csB200 { ctx, g, labels, n_vars, _f: core::marker::PhantomData })
+    }
+
+    /// The reference's answer without a `ConstraintLayer`: `Some("{label} - {index}")` for the first unsatisfied constraint
+    /// in label order, `None` when z = instance || witness (z[0] = 1) satisfies every predicate.  A z whose length is not
+    /// n_vars is `SynthesisError::AssignmentMissing`; nothing is read from it.
+    pub fn which_is_unsatisfied(&self, z: &[F]) -> Result<Option<String>, B200Error> {
+        if z.len() != self.n_vars { return Err(SynthesisError::AssignmentMissing.into()); }
+        let mut first = vec![u64::MAX; self.labels.len()];
+        check(self.ctx, unsafe {
+            b2s_gr1cs_check(self.ctx, self.g, 1, z.as_ptr().cast(), 0, first.as_mut_ptr(), core::ptr::null_mut())
+        })?;
+        Ok(self.labels.iter().zip(&first).find(|(_, f)| **f != u64::MAX).map(|(l, f)| format!("{l} - {f}")))
+    }
+
+    pub fn is_satisfied(&self, z: &[F]) -> Result<bool, B200Error> { Ok(self.which_is_unsatisfied(z)?.is_none()) }
+
+    /// instance_assignment || witness_assignment of `cs` (constraint_system.rs:193-206), the z the checks take
+    pub fn assignment(cs: &ConstraintSystem<F>) -> Result<Vec<F>, B200Error> {
+        Ok([cs.instance_assignment()?, cs.witness_assignment()?].concat())
+    }
+}
+
+impl<F: PrimeField> Drop for Gr1csB200<F> {
+    fn drop(&mut self) { unsafe { b2s_gr1cs_free(self.ctx, self.g); b2s_ctx_destroy(self.ctx); } }
+}

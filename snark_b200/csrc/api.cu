@@ -415,6 +415,37 @@ int32_t b2s_witness_map_sim(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int3
     return B2S_OK;
 }
 
+int32_t b2s_gr1cs_upload(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_desc* preds,
+                         b2s_gr1cs** out) {
+    LOCK(ctx);
+    if (!out || (!preds && n_predicates)) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_upload: null argument");
+    *out = nullptr;
+    return gr1cs_upload(ctx, n_instance, n_witness, n_predicates, preds, out);
+}
+
+void b2s_gr1cs_free(b2s_ctx* ctx, b2s_gr1cs* g) {
+    if (!ctx || !g) return;
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    delete g;
+}
+
+int32_t b2s_gr1cs_check(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat,
+                        uint64_t* n_unsat) {
+    LOCK(ctx);
+    if (!g) return fail(ctx, B2S_ERR_MISSING_CS, "gr1cs_check: null constraint system");
+    if (n_assign && (!z || !first_unsat)) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_check: null buffer");
+    return gr1cs_check(ctx, g, n_assign, z, mem, first_unsat, n_unsat);
+}
+
+int32_t b2s_r1cs_check(b2s_ctx* ctx, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat,
+                       uint64_t* n_unsat) {
+    LOCK(ctx);
+    if (!m) return fail(ctx, B2S_ERR_MISSING_CS, "r1cs_check: null matrices");
+    if (n_assign && (!z || !first_unsat)) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_check: null buffer");
+    return r1cs_check(ctx, m, n_assign, z, mem, first_unsat, n_unsat);
+}
+
 int32_t b2s_pk_upload(b2s_ctx* ctx, const b2s_pk_desc* desc, int32_t mem, b2s_pk** out) {
     LOCK(ctx);
     if (!desc || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_upload: null argument");

@@ -105,19 +105,46 @@ __global__ void __launch_bounds__(256) qap_circom_h_kernel(Fr* a, const Fr* __re
 }
 
 // -------------------------------------------------------------------------------------------
-struct Key32 {
-    uint64_t w[4];
-    bool operator==(const Key32& o) const { return w[0] == o.w[0] && w[1] == o.w[1] && w[2] == o.w[2] && w[3] == o.w[3]; }
-};
-struct Key32Hash {
-    size_t operator()(const Key32& k) const {
-        uint64_t h = k.w[0] * 0x9E3779B97F4A7C15ull;
-        h ^= (k.w[1] + 0x7F4A7C15ull) * 0xC2B2AE3D27D4EB4Full;
-        h ^= (k.w[2] + 0x165667B1ull) * 0x9E3779B97F4A7C15ull;
-        h ^= (k.w[3] + 0x27D4EB2Full) * 0xC2B2AE3D27D4EB4Full;
-        return (size_t)(h ^ (h >> 29));
+int32_t csr_intern_upload(Ctx* c, CoeffInterner& in, const char* who, int k, uint64_t n_rows, uint64_t n_vars, const uint64_t* row_ptr,
+                          const uint32_t* col, const void* coeff, DevBuf& d_row_ptr, DevBuf& d_col, DevBuf& d_cid, uint64_t* nnz_out) {
+    if (row_ptr[0] != 0) return fail(c, B2S_ERR_INVALID_ARG, "%s: row_ptr[%d][0] != 0", who, k);
+    const uint64_t nnz = row_ptr[n_rows];
+    *nnz_out = nnz;
+    std::vector<uint32_t> cid(nnz);
+    const Key32* vals = reinterpret_cast<const Key32*>(coeff);
+    for (uint64_t e = 0; e < nnz; e++) {
+        if (col[e] >= n_vars) return fail(c, B2S_ERR_ASSIGNMENT_MISSING, "%s: column %u >= %llu variables", who, col[e], (unsigned long long)n_vars);
+        Key32 v;
+        memcpy(&v, vals + e, 32);
+        if (v == in.one) { cid[e] = 0; continue; }
+        auto it = in.ids.find(v);
+        if (it == in.ids.end()) {
+            it = in.ids.emplace(v, (uint32_t)in.pool.size()).first;
+            in.pool.push_back(v);
+        }
+        cid[e] = it->second;
     }
-};
+    for (uint64_t r = 0; r < n_rows; r++)
+        if (row_ptr[r + 1] < row_ptr[r]) return fail(c, B2S_ERR_INVALID_ARG, "%s: row_ptr[%d] not monotone", who, k);
+    B2S_TRY(d_row_ptr.alloc(c, (n_rows + 1) * 8));
+    B2S_TRY(d_col.alloc(c, nnz * 4));
+    B2S_TRY(d_cid.alloc(c, nnz * 4));
+    cudaError_t ce = cudaMemcpyAsync(d_row_ptr.p, row_ptr, (n_rows + 1) * 8, cudaMemcpyHostToDevice, c->stream);
+    if (ce == cudaSuccess && nnz) ce = cudaMemcpyAsync(d_col.p, col, nnz * 4, cudaMemcpyHostToDevice, c->stream);
+    if (ce == cudaSuccess && nnz) ce = cudaMemcpyAsync(d_cid.p, cid.data(), nnz * 4, cudaMemcpyHostToDevice, c->stream);
+    const cudaError_t se = cudaStreamSynchronize(c->stream);  // cid goes out of scope
+    if (ce == cudaSuccess) ce = se;
+    if (ce != cudaSuccess) return fail(c, B2S_ERR_CUDA, "%s upload of matrix %d failed: %s", who, k, cudaGetErrorString(ce));
+    return B2S_OK;
+}
+
+int32_t coeff_pool_upload(Ctx* c, const CoeffInterner& in, const char* who, DevBuf& pool, uint32_t* pool_size) {
+    *pool_size = (uint32_t)in.pool.size();
+    B2S_TRY(pool.alloc(c, in.pool.size() * 32));
+    cudaMemcpyAsync(pool.p, in.pool.data(), in.pool.size() * 32, cudaMemcpyHostToDevice, c->stream);
+    if (cudaStreamSynchronize(c->stream) != cudaSuccess) return fail(c, B2S_ERR_CUDA, "%s upload failed", who);
+    return B2S_OK;
+}
 
 template <class Curve>
 static int32_t r1cs_upload_t(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness,
@@ -134,58 +161,11 @@ static int32_t r1cs_upload_t(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint6
         return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "r1cs: domain 2^%u unsupported", logd);
     b2s_r1cs* m = new b2s_r1cs();
     m->n_rows = n_rows; m->n_instance = n_instance; m->n_witness = n_witness; m->log_domain = logd;
-    // intern coefficients (host, once per circuit; byte comparisons only -- no field arithmetic)
-    Key32 one;
-    {
-        uint32_t o[8];
-        for (int i = 0; i < 8; i++) o[i] = FrP::r1(i);
-        memcpy(one.w, o, 32);
-    }
-    std::unordered_map<Key32, uint32_t, Key32Hash> ids;
-    std::vector<Key32> pool;
-    pool.push_back(one);
-    ids.emplace(one, 0u);
+    CoeffInterner in(fr_one_key<FrP>());
     int32_t st = B2S_OK;
-    for (int k = 0; k < 3 && st == B2S_OK; k++) {
-        if (row_ptr[k][0] != 0) { st = fail(c, B2S_ERR_INVALID_ARG, "r1cs: row_ptr[%d][0] != 0", k); break; }
-        const uint64_t nnz = row_ptr[k][n_rows];
-        m->nnz[k] = nnz;
-        std::vector<uint32_t> cid(nnz);
-        const Key32* vals = reinterpret_cast<const Key32*>(coeff[k]);
-        for (uint64_t e = 0; e < nnz; e++) {
-            if (col[k][e] >= n_vars) { st = fail(c, B2S_ERR_ASSIGNMENT_MISSING, "r1cs: column %u >= %llu variables", col[k][e], (unsigned long long)n_vars); break; }
-            Key32 v;
-            memcpy(&v, vals + e, 32);
-            if (v == one) { cid[e] = 0; continue; }
-            auto it = ids.find(v);
-            if (it == ids.end()) {
-                it = ids.emplace(v, (uint32_t)pool.size()).first;
-                pool.push_back(v);
-            }
-            cid[e] = it->second;
-        }
-        if (st != B2S_OK) break;
-        for (uint64_t r = 0; r < n_rows; r++)
-            if (row_ptr[k][r + 1] < row_ptr[k][r]) { st = fail(c, B2S_ERR_INVALID_ARG, "r1cs: row_ptr[%d] not monotone", k); break; }
-        if (st != B2S_OK) break;
-        if ((st = m->row_ptr[k].alloc(c, (n_rows + 1) * 8)) != B2S_OK) break;
-        if ((st = m->col[k].alloc(c, nnz * 4)) != B2S_OK) break;
-        if ((st = m->coeff_id[k].alloc(c, nnz * 4)) != B2S_OK) break;
-        cudaError_t ce = cudaMemcpyAsync(m->row_ptr[k].p, row_ptr[k], (n_rows + 1) * 8, cudaMemcpyHostToDevice, c->stream);
-        if (ce == cudaSuccess && nnz) ce = cudaMemcpyAsync(m->col[k].p, col[k], nnz * 4, cudaMemcpyHostToDevice, c->stream);
-        if (ce == cudaSuccess && nnz) ce = cudaMemcpyAsync(m->coeff_id[k].p, cid.data(), nnz * 4, cudaMemcpyHostToDevice, c->stream);
-        const cudaError_t se = cudaStreamSynchronize(c->stream);  // cid goes out of scope
-        if (ce == cudaSuccess) ce = se;
-        if (ce != cudaSuccess) { st = fail(c, B2S_ERR_CUDA, "r1cs upload of matrix %d failed: %s", k, cudaGetErrorString(ce)); break; }
-    }
-    if (st == B2S_OK) {
-        m->pool_size = (uint32_t)pool.size();
-        st = m->pool.alloc(c, pool.size() * 32);
-        if (st == B2S_OK) {
-            cudaMemcpyAsync(m->pool.p, pool.data(), pool.size() * 32, cudaMemcpyHostToDevice, c->stream);
-            if (cudaStreamSynchronize(c->stream) != cudaSuccess) st = fail(c, B2S_ERR_CUDA, "r1cs upload failed");
-        }
-    }
+    for (int k = 0; k < 3 && st == B2S_OK; k++)
+        st = csr_intern_upload(c, in, "r1cs", k, n_rows, n_vars, row_ptr[k], col[k], coeff[k], m->row_ptr[k], m->col[k], m->coeff_id[k], &m->nnz[k]);
+    if (st == B2S_OK) st = coeff_pool_upload(c, in, "r1cs", m->pool, &m->pool_size);
     if (st != B2S_OK) { delete m; return st; }
     *out = m;
     return B2S_OK;

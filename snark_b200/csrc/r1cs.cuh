@@ -1,5 +1,9 @@
-// Device-resident R1CS matrices and Groth16 proving key (the handles behind b2s_r1cs / b2s_pk).
+// Device-resident R1CS matrices, GR1CS predicates and Groth16 proving key (the handles behind b2s_r1cs / b2s_gr1cs / b2s_pk).
 #pragma once
+#include <cstring>
+#include <memory>
+#include <unordered_map>
+
 #include "common.cuh"
 
 struct b2s_r1cs {
@@ -16,6 +20,79 @@ struct b2s_r1cs {
 };
 
 namespace b2s {
+// One polynomial predicate of a GR1CS (predicate/mod.rs, polynomial_constraint.rs): argument j's matrix in CSR, coefficients
+// interned into the handle's pool, and the polynomial as flattened terms (term t = coeff[t] * prod over factors
+// [term_off[t], term_off[t+1]) of x[factor_var]^factor_pow).
+struct Gr1csPredicate {
+    uint32_t arity = 0, n_terms = 0;
+    uint64_t n_rows = 0;
+    uint64_t nnz[B2S_GR1CS_MAX_ARITY] = {};
+    DevBuf row_ptr[B2S_GR1CS_MAX_ARITY];   // uint64[n_rows + 1], j < arity
+    DevBuf col[B2S_GR1CS_MAX_ARITY];       // uint32[nnz]
+    DevBuf coeff_id[B2S_GR1CS_MAX_ARITY];  // uint32[nnz]
+    DevBuf term_coeff;                     // Fr[n_terms]
+    DevBuf term_off;                       // uint32[n_terms + 1]
+    DevBuf factor_var, factor_pow;         // uint32[term_off[n_terms]]
+};
+}  // namespace b2s
+
+struct b2s_gr1cs {
+    int curve = 0;                        // of the ctx that uploaded it
+    uint64_t n_instance = 0, n_witness = 0;
+    b2s::DevBuf pool;                     // Fr[pool_size], shared by every predicate; id 0 == ONE
+    uint32_t pool_size = 0;
+    std::vector<std::unique_ptr<b2s::Gr1csPredicate>> preds;   // upload order
+};
+
+namespace b2s {
+// Coefficient interning of the matrix uploads (host, once per circuit; byte comparisons only -- no field arithmetic), like the
+// reference's FieldInterner (relations/src/gr1cs/field_interner.rs:13-35): id 0 is ONE, whose multiplication the kernels
+// skip; every other value gets the next id on first use.
+struct Key32 {
+    uint64_t w[4];
+    bool operator==(const Key32& o) const { return w[0] == o.w[0] && w[1] == o.w[1] && w[2] == o.w[2] && w[3] == o.w[3]; }
+};
+struct Key32Hash {
+    size_t operator()(const Key32& k) const {
+        uint64_t h = k.w[0] * 0x9E3779B97F4A7C15ull;
+        h ^= (k.w[1] + 0x7F4A7C15ull) * 0xC2B2AE3D27D4EB4Full;
+        h ^= (k.w[2] + 0x165667B1ull) * 0x9E3779B97F4A7C15ull;
+        h ^= (k.w[3] + 0x27D4EB2Full) * 0xC2B2AE3D27D4EB4Full;
+        return (size_t)(h ^ (h >> 29));
+    }
+};
+struct CoeffInterner {
+    Key32 one;
+    std::unordered_map<Key32, uint32_t, Key32Hash> ids;
+    std::vector<Key32> pool;
+    explicit CoeffInterner(const Key32& one_mont) : one(one_mont) {
+        pool.push_back(one);
+        ids.emplace(one, 0u);
+    }
+};
+// Montgomery ONE of a field's parameters as an interning key
+template <class P>
+inline Key32 fr_one_key() {
+    uint32_t o[8];
+    for (int i = 0; i < 8; i++) o[i] = P::r1(i);
+    Key32 k;
+    memcpy(k.w, o, 32);
+    return k;
+}
+// Checks one CSR matrix (row_ptr[0] == 0, columns < n_vars, row_ptr monotone), interns its coefficients and copies row_ptr,
+// col and the coefficient ids to the device.  Failure messages read "<who>: row_ptr[<k>] ...".  Shared by b2s_r1cs_upload
+// (k = matrix) and b2s_gr1cs_upload (k = argument).
+int32_t csr_intern_upload(Ctx* c, CoeffInterner& in, const char* who, int k, uint64_t n_rows, uint64_t n_vars, const uint64_t* row_ptr,
+                          const uint32_t* col, const void* coeff, DevBuf& d_row_ptr, DevBuf& d_col, DevBuf& d_cid, uint64_t* nnz);
+// the interned values to the device: *pool_size = in.pool.size()
+int32_t coeff_pool_upload(Ctx* c, const CoeffInterner& in, const char* who, DevBuf& pool, uint32_t* pool_size);
+
+// gr1cs.cu
+int32_t gr1cs_upload(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_desc* preds,
+                     b2s_gr1cs** out);
+// first_unsat / n_unsat (n_unsat may be null): n_assign x n_predicates, in `mem` like z
+int32_t gr1cs_check(Ctx* c, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
+int32_t r1cs_check(Ctx* c, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
 // The five query vectors of a proving key, in the order of b2s_pk_query's `which`.
 enum PkQueryId { Q_A, Q_B_G1, Q_B_G2, Q_H, Q_L, PK_QUERIES };
 // Where the scalars of a query's MSM start: z + off, z + n_instance + off (the witness), or the h shard (HSource).

@@ -37,6 +37,49 @@ class PkDesc(ctypes.Structure):
     ]
 
 
+GR1CS_MAX_ARITY = 8
+NOT_FOUND = np.uint64(0xFFFFFFFFFFFFFFFF)   # first_unsat of a satisfied predicate
+# scalar-field moduli, for the Montgomery form of the Python-int coefficients gr1cs_upload takes
+FR_MODULUS = {BLS12_381: 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001,
+              BN254: 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001}
+
+
+class PredicateDesc(ctypes.Structure):
+    _fields_ = [
+        ("arity", c_uint32), ("n_terms", c_uint32),
+        ("term_coeffs", c_void_p), ("term_offsets", c_void_p), ("factor_var", c_void_p), ("factor_pow", c_void_p),
+        ("n_rows", c_uint64),
+        ("row_ptr", c_void_p * GR1CS_MAX_ARITY), ("col", c_void_p * GR1CS_MAX_ARITY), ("coeff", c_void_p * GR1CS_MAX_ARITY),
+    ]
+
+
+def _mont_limbs(r, xs):
+    """Python ints -> uint32[len(xs) * 8] Montgomery limbs mod r"""
+    out = np.zeros((len(xs), 8), dtype=np.uint32)
+    for i, x in enumerate(xs):
+        v = (x % r) * (1 << 256) % r
+        out[i] = [(v >> (32 * j)) & 0xFFFFFFFF for j in range(8)]
+    return out.reshape(-1)
+
+
+def _csr(r, matrix):
+    """Matrix (rows of (coeff, col), as to_matrices() returns it) -> (row_ptr u64, col u32, coeff Montgomery limbs)"""
+    row_ptr = np.zeros(len(matrix) + 1, dtype=np.uint64)
+    row_ptr[1:] = np.cumsum([len(row) for row in matrix], dtype=np.uint64)
+    cols = np.array([col for row in matrix for _, col in row], dtype=np.uint32)
+    return row_ptr, cols, _mont_limbs(r, [c for row in matrix for c, _ in row])
+
+
+class Gr1cs:
+    """A device-resident GR1CS (b2s_gr1cs), the labels of its predicates in upload (BTreeMap) order and the number of
+    variables (n_instance + n_witness) every assignment holds."""
+
+    def __init__(self, handle, labels, n_vars):
+        self.h = handle
+        self.labels = labels
+        self.n_vars = n_vars
+
+
 # name -> (restype, argtypes): every symbol include/b200snark.h declares
 SIGNATURES = {
     "b2s_version": (c_char_p, []),
@@ -64,6 +107,10 @@ SIGNATURES = {
     "b2s_witness_map_qap": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_void_p]),
     "b2s_r1cs_domain_size": (c_uint64, [c_void_p]),
     "b2s_witness_map_sim": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_uint32, c_void_p]),
+    "b2s_gr1cs_upload": (c_int32, [c_void_p, c_uint64, c_uint64, c_uint32, c_void_p, POINTER(c_void_p)]),
+    "b2s_gr1cs_free": (None, [c_void_p, c_void_p]),
+    "b2s_gr1cs_check": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_void_p]),
+    "b2s_r1cs_check": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_void_p]),
     "b2s_pk_upload": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, POINTER(c_void_p)]),
     "b2s_pk_upload_qap": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_pk_free": (None, [c_void_p, c_void_p]),
@@ -179,6 +226,7 @@ class Backend:
 
     def __init__(self, curve=BLS12_381, device=0):
         self.h = None
+        self._r1cs_vars = {}   # n_instance + n_witness of each matrix handle, for the width check of r1cs_check
         self.lib = load_library()
         h = c_void_p()
         st = self.lib.b2s_ctx_create(curve, device, ctypes.byref(h))
@@ -285,6 +333,7 @@ class Backend:
         co = (c_void_p * 3)(*[m[2].ctypes.data for m in csr])
         h = c_void_p()
         self._ck(self.lib.b2s_r1cs_upload(self.h, n_rows, n_instance, n_witness, rp, col, co, ctypes.byref(h)))
+        self._r1cs_vars[h.value] = n_instance + n_witness
         return h
 
     def r1cs_upload_lcmap(self, n_rows, n_instance, n_witness, args, lc_offsets, lc_vars, lc_coeffs, pool):
@@ -295,9 +344,11 @@ class Backend:
         self._ck(self.lib.b2s_r1cs_upload_lcmap(self.h, n_rows, n_instance, n_witness, a, len(lc_offsets) - 1, lc_offsets.ctypes.data,
                                                 lc_vars.ctypes.data, lc_coeffs.ctypes.data, pool.ctypes.data, len(pool) // 8,
                                                 ctypes.byref(h)))
+        self._r1cs_vars[h.value] = n_instance + n_witness
         return h
 
     def r1cs_free(self, m):
+        self._r1cs_vars.pop(m.value if isinstance(m, c_void_p) else m, None)
         self.lib.b2s_r1cs_free(self.h, m)
 
     def domain_size(self, m):
@@ -328,6 +379,84 @@ class Backend:
         h = np.zeros(self.domain_size(m) * 8, dtype=np.uint32)
         self._ck(self.lib.b2s_witness_map_sim(self.h, m, pz, mem, log_ranks, h.ctypes.data))
         return h
+
+    # ---- constraint satisfaction (ConstraintSystem::which_is_unsatisfied on the GPU) --------------------------------
+    def gr1cs_upload(self, n_instance, n_witness, predicates):
+        """predicates: {label: (arity, terms, matrices)}: terms [(coeff, [(argument, exponent), ...])] as
+        ConstraintSystem.register_predicate takes them (constraint satisfied iff the polynomial is 0), matrices the predicate's
+        `arity` matrices as to_matrices_all returns them (rows of (coeff, col)); Python ints.  Uploaded in sorted label order,
+        the reference's BTreeMap order.  Returns a Gr1cs."""
+        r = FR_MODULUS[self.curve]
+        labels = sorted(predicates)
+        descs = (PredicateDesc * max(len(labels), 1))()
+        keep = []
+        for d, label in zip(descs, labels):
+            arity, terms, mats = predicates[label]
+            offs = np.zeros(len(terms) + 1, dtype=np.uint32)
+            offs[1:] = np.cumsum([len(mono) for _, mono in terms])
+            arrs = [_mont_limbs(r, [c for c, _ in terms]), offs, np.array([v for _, mono in terms for v, _ in mono], dtype=np.uint32),
+                    np.array([e for _, mono in terms for _, e in mono], dtype=np.uint32)]
+            keep += arrs
+            d.arity, d.n_terms, d.n_rows = arity, len(terms), len(mats[0]) if mats else 0
+            d.term_coeffs, d.term_offsets, d.factor_var, d.factor_pow = (a.ctypes.data for a in arrs)
+            for j, m in enumerate(mats[:GR1CS_MAX_ARITY]):
+                csr = _csr(r, m)
+                keep += csr
+                d.row_ptr[j], d.col[j], d.coeff[j] = (a.ctypes.data for a in csr)
+        h = c_void_p()
+        self._ck(self.lib.b2s_gr1cs_upload(self.h, n_instance, n_witness, len(labels), descs, ctypes.byref(h)))
+        return Gr1cs(h, labels, n_instance + n_witness)
+
+    def gr1cs_free(self, g):
+        self.lib.b2s_gr1cs_free(self.h, g.h)
+
+    def _check(self, fn, handle, n_pred, n_vars, z, counts):
+        """z: (n_assign, n_vars * 8) 32-bit numpy array or CUDA torch tensor -> (first, count) uint64 numpy arrays of shape
+        (n_assign, n_pred); count is None when counts=False (n_unsat = NULL).  The library reads n_assign * n_vars elements
+        from z, so its shape is checked first."""
+        width_ok = len(z.shape) == 2 and z.shape[1] == 8 * n_vars
+        size_ok = (z.itemsize if isinstance(z, np.ndarray) else z.element_size()) == 4
+        if not (width_ok and size_ok):
+            raise ValueError(f"z must be (n_assign, {8 * n_vars}) 32-bit limbs for {n_vars} variables, got shape {tuple(z.shape)}")
+        pz, mem = _ptr(z)
+        n = z.shape[0]
+        if mem == MEM_HOST:
+            first = np.zeros((n, n_pred), dtype=np.uint64)
+            count = np.zeros((n, n_pred), dtype=np.uint64) if counts else None
+        else:
+            import torch
+
+            first = torch.zeros((n, n_pred), dtype=torch.int64, device=z.device)
+            count = torch.zeros((n, n_pred), dtype=torch.int64, device=z.device) if counts else None
+            torch.cuda.current_stream(z.device).synchronize()
+        self._ck(fn(self.h, handle, n, pz, mem, _ptr(first)[0], _ptr(count)[0] if counts else None))
+        if mem == MEM_DEVICE:
+            first = first.cpu().numpy().view(np.uint64)
+            count = count.cpu().numpy().view(np.uint64) if counts else None
+        return first, count
+
+    def gr1cs_check(self, g, z, counts=True):
+        """b2s_gr1cs_check: first[i, p] = the first constraint of predicate g.labels[p] that assignment i does not satisfy
+        (NOT_FOUND if none), count[i, p] how many it does not satisfy.  z: (n_assign, n_vars * 8) uint32 Montgomery limbs,
+        HOST numpy or CUDA torch tensor."""
+        return self._check(self.lib.b2s_gr1cs_check, g.h, len(g.labels), g.n_vars, z, counts)
+
+    def r1cs_check(self, m, z, counts=True):
+        """b2s_r1cs_check: the same for the R1CS predicate x0 * x1 - x2 of a Groth16 matrix handle (from r1cs_upload or
+        r1cs_upload_lcmap of this Backend, which record its n_vars); arrays of shape (n_assign, 1)."""
+        n_vars = self._r1cs_vars.get(m.value if isinstance(m, c_void_p) else m)
+        if n_vars is None:
+            raise ValueError("r1cs_check: not a live matrix handle of this Backend")
+        return self._check(self.lib.b2s_r1cs_check, m, 1, n_vars, z, counts)
+
+    def which_is_unsatisfied(self, g, z):
+        """ConstraintSystem::which_is_unsatisfied for one assignment z (n_vars * 8 limbs): None, or (label, index) of the first
+        unsatisfied constraint in label order."""
+        first, _ = self.gr1cs_check(g, np.ascontiguousarray(z).reshape(1, -1), counts=False)
+        for label, f in zip(g.labels, first[0]):
+            if f != NOT_FOUND:
+                return label, int(f)
+        return None
 
     # ---- Groth16 ------------------------------------------------------------------------------
     def pk_upload(self, desc: PkDesc, mem=MEM_HOST, qap=QAP_LIBSNARK):
