@@ -16,11 +16,11 @@
  *
  * DATA CONVENTIONS (what a Rust caller already has in memory):
  *   - Field element: little-endian limbs, MONTGOMERY form with R = 2^(64*N64), N64 = 4 for both
- *     scalar fields and BN254 Fq, 6 for BLS12-381 Fq.  Identical to ark-ff `Fp<MontBackend>`'s in-memory
+ *     scalar fields and BN254 Fq, 6 for BLS12-381 and BLS12-377 Fq.  Identical to ark-ff `Fp<MontBackend>`'s in-memory
  *     `BigInt<N>` -- `&[F]` can be passed as is.  "canonical" scalars (ark `into_bigint()`) are accepted
  *     where a `scalars_mont` flag says so.
  *   - G1 affine point: x || y (2 field elements, packed, no padding).  G2 affine: x.c0 || x.c1 || y.c0 ||
- *     y.c1.  The point at infinity is ALL-ZERO bytes ((0,0) is not on either curve).  ark-ec's `Affine`
+ *     y.c1.  The point at infinity is ALL-ZERO bytes ((0,0) is on none of the curves).  ark-ec's `Affine`
  *     carries a separate `infinity: bool`; the adapter writes zeros for such points (INTEGRATION.md).
  *   - Matrices: CSR per matrix (row_ptr[n_rows+1] u64, col[nnz] u32, coeff[nnz] field elements) built
  *     from `to_matrices()` rows in order; duplicate / unsorted columns are allowed and are summed
@@ -48,6 +48,7 @@ extern "C" {
 
 #define B2S_CURVE_BLS12_381 0
 #define B2S_CURVE_BN254 1
+#define B2S_CURVE_BLS12_377 2   /* ark-bls12-377: Fq 377 bits (N64 = 6), Fr 253 bits (N64 = 4), SWFlags serialization */
 
 #define B2S_MEM_HOST 0
 #define B2S_MEM_DEVICE 1
@@ -319,15 +320,15 @@ int32_t b2s_groth16_prove_group_resident(b2s_group* group, const b2s_pk* pk_shar
 
 /* ---- wire format (SURVEY 8(f) row 3): CanonicalSerialize::serialize_compressed of group elements / Proof --------
  * (snark/src/lib.rs:25-36 bounds).  BLS12-381: zcash/IETF big-endian form, 48 B (G1) / 96 B (G2); BN254: ark-ec
- * SWFlags little-endian form, 32 B / 64 B.  HOST affine Montgomery points in, bytes out; `cap` = size of `out`. */
+ * SWFlags little-endian form, 32 B / 64 B; BLS12-377: the same SWFlags form, 48 B / 96 B.  HOST affine Montgomery points in, bytes out; `cap` = size of `out`. */
 int32_t b2s_serialize_g1_compressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap);
 int32_t b2s_serialize_g2_compressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap);
-/* Proof { a, b, c } -> a || b || c (192 B on BLS12-381, 128 B on BN254). */
+/* Proof { a, b, c } -> a || b || c (192 B on BLS12-381 and BLS12-377, 128 B on BN254). */
 int32_t b2s_proof_serialize_compressed(b2s_ctx* ctx, const void* a_g1, const void* b_g2, const void* c_g1, uint8_t* out,
                                        uint64_t cap);
 
 /* serialize_uncompressed of the same types: x || y in the curve's byte / component order (96 / 192 B on BLS12-381 with only
- * the infinity bit in byte 0; 64 / 128 B on BN254 with both SWFlags in the last byte). */
+ * the infinity bit in byte 0; 64 / 128 B on BN254 and 96 / 192 B on BLS12-377 with both SWFlags in the last byte). */
 int32_t b2s_serialize_g1_uncompressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap);
 int32_t b2s_serialize_g2_uncompressed(b2s_ctx* ctx, const void* affine, uint32_t count, uint8_t* out, uint64_t cap);
 int32_t b2s_proof_serialize_uncompressed(b2s_ctx* ctx, const void* a_g1, const void* b_g2, const void* c_g1, uint8_t* out,
@@ -380,10 +381,10 @@ int32_t b2s_pk_deserialize_qap(b2s_ctx* ctx, const uint8_t* in, uint64_t len, in
 
 /* ---- verification: pairings and batched Groth16 verify ----------------------------------------------------------------
  * The optimal ate pairing in CUDA (snark_b200/csrc/pairing.cuh): BLS12-381 loops over |x| and conjugates, BN254 over the
- * signed digits of 6x + 2 with the two Frobenius lines.  GT is ark's Fp12 in memory (c0 = Fp6 {c0, c1, c2 : Fp2}, c1),
+ * signed digits of 6x + 2 with the two Frobenius lines, BLS12-377 over the bits of x > 0 with neither.  GT is ark's Fp12 in memory (c0 = Fp6 {c0, c1, c2 : Fp2}, c1),
  * Montgomery limbs, fully reduced.  The value is a fixed power of the textbook reduced ate pairing
- * o(P, Q) = f_{|t-1|,Q}(P)^((p^12 - 1) / r):  e = o^k with k = -3 mod r (BLS12-381) and
- * k = 147946756881789319005730692170996259610 (BN254), both coprime to r (pairing.cuh derives them).
+ * o(P, Q) = f_{|t-1|,Q}(P)^((p^12 - 1) / r):  e = o^k with k = -3 mod r (BLS12-381),
+ * k = 147946756881789319005730692170996259610 (BN254) and k = 3 (BLS12-377), all coprime to r (pairing.cuh derives them).
  *   b2s_vk_prepare   SNARK::process_vk (snark/src/lib.rs:68-71): HOST affine points, as returned by b2s_groth16_setup /
  *                    b2s_vk_deserialize.  Computes e(alpha_g1, beta_g2) in GT, the line coefficients of -gamma_g2 and
  *                    -delta_g2 (ark's G2Prepared), and per gamma_abc base j >= 1 a fixed-base table of 32 x 255 affine

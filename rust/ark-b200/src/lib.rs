@@ -204,9 +204,11 @@ pub const QAP_CIRCOM: i32 = 1;
 /// Device handles for one (proving key, circuit shape): matrices and key are witness independent.
 pub struct Resident { pub ctx: *mut B2sCtx, pub pk: *mut B2sPk, pub mat: *mut B2sR1cs }
 
-impl<E: Pairing> Groth16B200<E> {
+impl<E: Pairing + B200Curve> Groth16B200<E> {
     fn ctx_and_matrices(curve_id: i32, mats: &[Matrix<E::ScalarField>], n_inst: usize, n_wit: usize)
         -> Result<(*mut B2sCtx, *mut B2sR1cs), B200Error> {
+        // the id passed in must be E's: a BLS12-377 key on a BLS12-381 ctx would be read as the wrong curve's points
+        if curve_id != E::CURVE_ID { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
         let mut ctx: *mut B2sCtx = core::ptr::null_mut();
         check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
         let csr: Vec<_> = mats.iter().map(to_csr).collect();
@@ -218,7 +220,8 @@ impl<E: Pairing> Groth16B200<E> {
         Ok((ctx, mat))
     }
 
-    /// Upload the matrices and the key once per (key, circuit shape).  `curve_id`: 0 = BLS12-381, 1 = BN254.
+    /// Upload the matrices and the key once per (key, circuit shape).  `curve_id` must be `E::CURVE_ID` (0 = BLS12-381,
+    /// 1 = BN254, 2 = BLS12-377); another id is `B2S_ERR_INVALID_ARG`.
     pub fn make_resident(curve_id: i32, pk: &ProvingKey<E>, mats: &[Matrix<E::ScalarField>], n_inst: usize, n_wit: usize)
         -> Result<Resident, B200Error> {
         let (ctx, mat) = Self::ctx_and_matrices(curve_id, mats, n_inst, n_wit)?;
@@ -395,8 +398,8 @@ impl<E: Pairing> Groth16B200<E> {
 
     /// runs `f` with a ctx and the key prepared on it, and frees both whatever `f` returns
     fn with_prepared<T>(vk: &VerifyingKey<E>, f: impl FnOnce(*mut B2sCtx, *mut B2sPvk) -> Result<T, B200Error>) -> Result<T, B200Error> {
-        // the curve from the base field width: 48-byte Fq is BLS12-381, 32-byte Fq BN254
-        let curve_id = if core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>() == 48 { 0 } else { 1 };
+        // the curve from E's B200Curve impl: the base field width cannot tell BLS12-381 from BLS12-377 (both 48 bytes)
+        let curve_id = E::CURVE_ID;
         let mut ctx: *mut B2sCtx = core::ptr::null_mut();
         check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
         let run = || -> Result<T, B200Error> {
@@ -420,7 +423,7 @@ impl Drop for Resident {
     fn drop(&mut self) { unsafe { b2s_pk_free(self.ctx, self.pk); b2s_r1cs_free(self.ctx, self.mat); b2s_ctx_destroy(self.ctx); } }
 }
 
-/// Which curve id the backend should use for `E` (the backend supports the two curves of the north-star).
+/// Which curve id the backend should use for `E`: 0 = BLS12-381, 1 = BN254, 2 = BLS12-377.
 pub trait B200Curve { const CURVE_ID: i32; }
 
 impl<E: Pairing + B200Curve> SNARK<E::ScalarField> for Groth16B200<E> {
@@ -475,6 +478,7 @@ impl<E: Pairing + B200Curve> CircuitSpecificSetupSNARK<E::ScalarField> for Groth
 
 // e.g. in the application:  impl B200Curve for ark_bls12_381::Bls12_381 { const CURVE_ID: i32 = 0; }
 //                           impl B200Curve for ark_bn254::Bn254 { const CURVE_ID: i32 = 1; }
+//                           impl B200Curve for ark_bls12_377::Bls12_377 { const CURVE_ID: i32 = 2; }
 
 /// `ConstraintSystem::is_satisfied` / `which_is_unsatisfied` (relations/src/gr1cs/constraint_system.rs:652-687) on the GPU:
 /// the predicates of a finalized constraint system, uploaded once per circuit shape, checked against any assignment of the
@@ -493,11 +497,11 @@ const ERR_INVALID_ARG: i32 = 16;
 
 impl<F: PrimeField> Gr1csB200<F> {
     /// Uploads `cs.to_matrices()` (one matrix per argument) and `cs.get_all_predicate_types()` (the polynomial of each
-    /// predicate), in the BTreeMap's label order.  `curve_id`: 0 = BLS12-381, 1 = BN254; it must be `F`'s curve
-    /// (checked by the modulus size: 255 / 254 bits).  A predicate that is not polynomial (`Predicate` is `#[non_exhaustive]`,
+    /// predicate), in the BTreeMap's label order.  `curve_id`: 0 = BLS12-381, 1 = BN254, 2 = BLS12-377; it must be
+    /// `F`'s curve (checked by the modulus size: 255 / 254 / 253 bits).  A predicate that is not polynomial (`Predicate` is `#[non_exhaustive]`,
     /// predicate/mod.rs:19-25) is `B200Error::Backend(B2S_ERR_INVALID_ARG)`.
     pub fn upload(curve_id: i32, cs: &ConstraintSystem<F>) -> Result<Self, B200Error> {
-        let bits = match curve_id { 0 => 255, 1 => 254, _ => return Err(B200Error::Backend(ERR_INVALID_ARG)) };
+        let bits = match curve_id { 0 => 255, 1 => 254, 2 => 253, _ => return Err(B200Error::Backend(ERR_INVALID_ARG)) };
         if F::MODULUS_BIT_SIZE != bits || core::mem::size_of::<F>() != 32 { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
         let mats = cs.to_matrices()?;
         let types = cs.get_all_predicate_types();

@@ -63,7 +63,7 @@ const char* b2s_version(void) { return "b200snark 0.1 (sm_90a)"; }
 int32_t b2s_ctx_create(int32_t curve_id, int32_t device_ordinal, b2s_ctx** out) {
     if (!out) return B2S_ERR_INVALID_ARG;
     *out = nullptr;
-    if (curve_id != B2S_CURVE_BLS12_381 && curve_id != B2S_CURVE_BN254) return B2S_ERR_INVALID_ARG;
+    if (curve_id != B2S_CURVE_BLS12_381 && curve_id != B2S_CURVE_BN254 && curve_id != B2S_CURVE_BLS12_377) return B2S_ERR_INVALID_ARG;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return B2S_ERR_NO_DEVICE;
     if (device_ordinal < 0 || device_ordinal >= ndev) return B2S_ERR_NO_DEVICE;

@@ -171,6 +171,7 @@ inline int32_t dispatch_curve(Ctx* c, F&& f) {
     switch (c->curve) {
         case B2S_CURVE_BLS12_381: return f(Bls12_381{});
         case B2S_CURVE_BN254: return f(Bn254{});
+        case B2S_CURVE_BLS12_377: return f(Bls12_377{});
     }
     return fail(c, B2S_ERR_INVALID_ARG, "unknown curve id %d", c->curve);
 }

@@ -1,4 +1,4 @@
-// Curve bundles: the field / group types and generators for the two supported pairing curves.
+// Curve bundles: the field / group types and generators for the three supported pairing curves.
 // curve ids match B2S_CURVE_* in include/b200snark.h.
 #pragma once
 #include "ec.cuh"
@@ -38,5 +38,6 @@ struct CurveT {
 
 using Bls12_381 = CurveT<BlsFqP, BlsFrP, 0>;
 using Bn254 = CurveT<BnFqP, BnFrP, 1>;
+using Bls12_377 = CurveT<Bls377FqP, Bls377FrP, 2>;
 
 }  // namespace b2s

@@ -10,13 +10,17 @@
 //   | compressed   | 0x80 must be set                                      | (no mode bit)                                      |
 //   | uncompressed | 0x80 and 0x20 must be clear                           | flags in the last byte of y; the sign is not used  |
 //   | infinity     | every other bit and byte zero; 0x20 clear             | every other bit and byte zero                      |
+//   BLS12-377 uses the SWFlags form of the right-hand column (ark-bls12-377 keeps ark-ec's default); its Fq has 7 spare
+//   bits, so any bit between bit 376 and the two flag bits leaves the coordinate >= p: DEC_NONCANONICAL.
 //
-// Every coordinate must be canonical (< p).  Compressed points take y = sqrt(x^3 + b), the root chosen by the
+// Every coordinate must be canonical (< p).  Compressed points take y = sqrt(x^3 + b) (a^((p+1)/4) for p = 3 mod 4,
+// Tonelli-Shanks for BLS12-377's p = 1 mod 2^46), the root chosen by the
 // "lexicographically larger" bit (y_is_larger, shared with the serializer); no root means the encoding is invalid whatever
 // `validate` says.  With validate (ark's Validate::Yes) uncompressed points must satisfy the curve equation and every point
 // must lie in the prime-order subgroup, tested by endomorphism criteria instead of r * P = O:
 //   BLS12-381 G1  phi(P) = -[x^2]P, phi(x, y) = (beta x, y)       BLS12-381 G2  psi(P) = [x]P, x = -0xd201000000010000
 //   BN254 G1      cofactor 1: on the curve is enough               BN254 G2      psi(P) = [6 x^2]P
+//   BLS12-377 G1  phi(P) = -[x^2]P                                 BLS12-377 G2  psi(P) = [x]P, x = 0x8508c00000000001
 // with psi(x, y) = (conj(x) cx, conj(y) cy).  beta, cx, cy and the scalars are generated (tools/gen_field_params.py, which
 // checks each criterion on the generator); tests/test_host_deserialize.py checks the verdicts against r * P = O on points
 // outside the subgroup.  Comparisons are projective: no inversion per point.
@@ -115,9 +119,61 @@ B2S_DEC_NOINLINE Fp<P> pow_sqrt_exp(const Fp<P>& a) {
     for (int i = 0; i < Fp<P>::N; i++) e[i] = P::sqrt_exp(i);
     return a.pow_words(e, Fp<P>::N);
 }
+// Tonelli-Shanks for p - 1 = 2^S q (BLS12-377: S = 46): x = a^((q+1)/2) is a root up to the 2^S-th root of unity
+// b = a^q; each round finds the order 2^k of b and multiplies x by a power of the precomputed root z^q
+template <class P>
+B2S_DEC_NOINLINE bool sqrt_ts(const Fp<P>& a, Fp<P>& r) {
+    using B = Fp<P>;
+    if (a.is_zero()) { r = a; return true; }
+    uint32_t e[B::N];
+    B z;
+    for (int i = 0; i < B::N; i++) { e[i] = P::ts_exp(i); z.v[i] = P::ts_root(i); }
+    const B w = a.pow_words(e, B::N);   // a^((q-1)/2)
+    B x = a * w, b = x * w;             // a^((q+1)/2), a^q
+    int v = P::TS_S;
+    while (b != B::one()) {
+        int k = 0;
+        for (B t = b; t != B::one(); t = t.sqr())
+            if (++k == v) return false;   // b has order 2^v: a is not a square
+        B g = z;
+        for (int i = 0; i < v - k - 1; i++) g = g.sqr();
+        z = g.sqr();
+        b = b * z;
+        x = x * g;
+        v = k;
+    }
+    r = x;
+    return true;
+}
 template <class P>
 B2S_DEC_NOINLINE bool sqrt(const Fp<P>& a, Fp<P>& r) {
-    r = pow_sqrt_exp(a) * a;
+    if constexpr (P::SQRT_TS) {
+        return sqrt_ts(a, r);
+    } else {
+        r = pow_sqrt_exp(a) * a;
+        return r.sqr() == a;
+    }
+}
+// Fq2 = Fq[u]/(u^2 + 5) by the norm method with square roots by sqrt(): alpha = sqrt(a0^2 + 5 a1^2), delta =
+// (a0 +- alpha) / 2, x0 = sqrt(delta), x1 = a1 / (2 x0); for a1 = 0 either sqrt(a0) or sqrt(-a0 / 5) u
+template <class P>
+B2S_DEC_NOINLINE bool sqrt_nr5(const Fp2<P>& a, Fp2<P>& r) {
+    using B = Fp<P>;
+    if (a.c1.is_zero()) {
+        B s;
+        if (sqrt(a.c0, s)) { r = {s, B::zero()}; return true; }
+        B nr_inv;
+        for (int i = 0; i < B::N; i++) nr_inv.v[i] = P::fq2_nr_inv(i);
+        if (sqrt(a.c0 * nr_inv, s)) { r = {B::zero(), s}; return true; }   // (s u)^2 = -5 s^2 = a0
+        return false;
+    }
+    B alpha;
+    if (!sqrt(a.c0.sqr() + Fp2<P>::times5(a.c1.sqr()), alpha)) return false;
+    B half;
+    for (int i = 0; i < B::N; i++) half.v[i] = P::fq_half(i);
+    B x0;
+    if (!sqrt((a.c0 + alpha) * half, x0) && !sqrt((a.c0 - alpha) * half, x0)) return false;
+    r = {x0, a.c1 * x0.dbl().inverse()};
     return r.sqr() == a;
 }
 // Fq2 = Fq[u]/(u^2 + 1) by the norm method: with alpha = sqrt(a0^2 + a1^2) one of (a0 +- alpha) / 2 is a square delta;
@@ -125,24 +181,28 @@ B2S_DEC_NOINLINE bool sqrt(const Fp<P>& a, Fp<P>& r) {
 template <class P>
 B2S_DEC_NOINLINE bool sqrt(const Fp2<P>& a, Fp2<P>& r) {
     using B = Fp<P>;
-    if (a.c1.is_zero()) {
-        B s;
-        if (sqrt(a.c0, s)) { r = {s, B::zero()}; return true; }
-        if (sqrt(a.c0.neg(), s)) { r = {B::zero(), s}; return true; }   // sqrt(-a0) u
-        return false;
+    if constexpr (P::FQ2_NR == -5) {
+        return sqrt_nr5(a, r);
+    } else {
+        if (a.c1.is_zero()) {
+            B s;
+            if (sqrt(a.c0, s)) { r = {s, B::zero()}; return true; }
+            if (sqrt(a.c0.neg(), s)) { r = {B::zero(), s}; return true; }   // sqrt(-a0) u
+            return false;
+        }
+        B alpha;
+        if (!sqrt(a.c0.sqr() + a.c1.sqr(), alpha)) return false;
+        B half;
+        for (int i = 0; i < B::N; i++) half.v[i] = P::fq_half(i);
+        B delta = (a.c0 + alpha) * half;
+        B t = pow_sqrt_exp(delta);
+        if (t.sqr() * delta != B::one()) {
+            delta = (a.c0 - alpha) * half;
+            t = pow_sqrt_exp(delta);
+        }
+        r = {t * delta, a.c1 * t * half};
+        return r.sqr() == a;
     }
-    B alpha;
-    if (!sqrt(a.c0.sqr() + a.c1.sqr(), alpha)) return false;
-    B half;
-    for (int i = 0; i < B::N; i++) half.v[i] = P::fq_half(i);
-    B delta = (a.c0 + alpha) * half;
-    B t = pow_sqrt_exp(delta);
-    if (t.sqr() * delta != B::one()) {
-        delta = (a.c0 - alpha) * half;
-        t = pow_sqrt_exp(delta);
-    }
-    r = {t * delta, a.c1 * t * half};
-    return r.sqr() == a;
 }
 
 // q == a for q projective (XYZZ), a affine, without an inversion
@@ -164,7 +224,7 @@ template <class Curve>
 B2S_DEC_NOINLINE bool in_subgroup(const Affine<typename Curve::Fq>& p) {
     using P = typename Curve::FqP;
     using F = typename Curve::Fq;
-    if (Curve::id == Bn254::id || p.is_inf()) return true;
+    if (!P::BLS12_FAMILY || p.is_inf()) return true;   // BN254: cofactor 1
     // -[x^2]P == (beta x, y)  <=>  [|x|]([|x|]P) == (beta x, -y)
     F beta;
     for (int i = 0; i < F::N; i++) beta.v[i] = P::beta(i);
@@ -183,8 +243,8 @@ B2S_DEC_NOINLINE bool in_subgroup(const Affine<typename Curve::Fq2>& p) {
     }
     const F xc{p.x.c0, p.x.c1.neg()}, yc{p.y.c0, p.y.c1.neg()};
     Affine<F> psi{xc * cx, yc * cy};
-    // BLS12-381: psi(P) == [x]P = -[|x|]P;  BN254: psi(P) == [6 x^2]P
-    if (Curve::id == Bls12_381::id) psi = psi.neg();
+    // BLS12-381: psi(P) == [x]P = -[|x|]P;  BLS12-377: psi(P) == [x]P;  BN254: psi(P) == [6 x^2]P
+    if (P::X_NEG) psi = psi.neg();
     return eq_affine(mul_endo_scalar<P>(XYZZ<F>::from_affine(p)), psi);
 }
 
@@ -195,7 +255,7 @@ B2S_DEC_NOINLINE bool in_subgroup(const Affine<typename Curve::Fq2>& p) {
 template <class Curve, class F>
 B2S_HD uint32_t decode_point(const uint8_t* in, bool compressed, bool validate, Affine<F>& out) {
     using P = typename Curve::FqP;
-    constexpr bool bls = Curve::id == Bls12_381::id;
+    constexpr bool bls = P::ZCASH_SERIAL;
     constexpr int CB = (int)(sizeof(F) / sizeof(Fp<P>)) * 4 * Fp<P>::N;   // bytes of one coordinate
     constexpr int TOP = Fp<P>::N - 1;
     F x, y = F::zero();

@@ -57,6 +57,8 @@ B2S_D uint32_t madc_hi_cc(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm 
 B2S_D uint32_t madc_hi(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm volatile("madc.hi.u32 %0,%1,%2,%3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
 B2S_D uint32_t mul_lo(uint32_t a, uint32_t b) { return a * b; }
 B2S_D uint32_t mul_hi(uint32_t a, uint32_t b) { return __umulhi(a, b); }
+// x, through an identity byte permutation that ptxas does not see through (see redc_row)
+B2S_D uint32_t opaque(uint32_t x) { uint32_t r; asm volatile("prmt.b32 %0,%1,0,0x3210;" : "=r"(r) : "r"(x)); return r; }
 #else
 // Host emulation of the PTX condition-code register (tests only).
 inline uint32_t& cf() { static thread_local uint32_t f = 0; return f; }
@@ -82,6 +84,7 @@ inline uint32_t mad_lo_cc(uint32_t a, uint32_t b, uint32_t c) { return add3_(mul
 inline uint32_t madc_lo_cc(uint32_t a, uint32_t b, uint32_t c) { return add3_(mul_lo(a, b), c, cf(), true); }
 inline uint32_t madc_hi_cc(uint32_t a, uint32_t b, uint32_t c) { return add3_(mul_hi(a, b), c, cf(), true); }
 inline uint32_t madc_hi(uint32_t a, uint32_t b, uint32_t c) { return add3_(mul_hi(a, b), c, cf(), false); }
+inline uint32_t opaque(uint32_t x) { return x; }
 #endif
 }  // namespace cc
 
@@ -206,7 +209,10 @@ struct Fp {
             O[N - 1] = cc::addc(O[N - 1], 0);
             return;
         }
-        const uint32_t m = cc::mul_lo(E[0], P::NINV);
+        // NINV = -1 (p = 1 mod 2^32: BLS12-377 Fq and Fr): m = -E[0].  Seen as a negation, that m makes ptxas split every
+        // fused IMAD.WIDE.U32.X of the chains below into IMAD.HI.U32.X + IMAD.X (an inlined 12-limb product: 952 instead of
+        // 832 instructions), so the negation goes through cc::opaque.
+        const uint32_t m = P::NINV == 0xffffffffu ? cc::opaque(0u - E[0]) : cc::mul_lo(E[0], P::NINV);
         // odd limbs of p -> O
         O[0] = cc::mad_lo_cc(P::mod(1), m, O[0]);
         O[1] = cc::madc_hi_cc(P::mod(1), m, O[1]);
@@ -330,11 +336,12 @@ struct Fp {
 };
 
 // ------------------------------------------------------------------------------------------
-// Quadratic extension Fq2 = Fq[u]/(u^2 + 1)  (both BLS12-381 and BN254 use nonresidue -1).
+// Quadratic extension Fq2 = Fq[u]/(u^2 - P::FQ2_NR): -1 for BLS12-381 and BN254, -5 for BLS12-377.
 // ------------------------------------------------------------------------------------------
 template <class P>
 struct Fp2 {
     using B = Fp<P>;
+    static_assert(P::FQ2_NR == -1 || P::FQ2_NR == -5, "u^2 = -1 or -5");
     B c0, c1;
     B2S_HD static Fp2 zero() { return {B::zero(), B::zero()}; }
     B2S_HD static Fp2 one() { return {B::one(), B::zero()}; }
@@ -345,24 +352,38 @@ struct Fp2 {
     B2S_HD friend Fp2 operator-(const Fp2& a, const Fp2& b) { return {a.c0 - b.c0, a.c1 - b.c1}; }
     B2S_HD Fp2 neg() const { return {c0.neg(), c1.neg()}; }
     B2S_HD Fp2 dbl() const { return {c0.dbl(), c1.dbl()}; }
-    // Karatsuba: 3 base multiplications
+    // 5 a: two doublings and an add (u^2 = -5)
+    B2S_HD static B times5(const B& a) { return a.dbl().dbl() + a; }
+    // Karatsuba: 3 base multiplications; c0 = t0 + FQ2_NR t1
     B2S_HD friend Fp2 operator*(const Fp2& a, const Fp2& b) {
         B t0 = a.c0 * b.c0;
         B t1 = a.c1 * b.c1;
         B t2 = (a.c0 + a.c1) * (b.c0 + b.c1);
-        return {t0 - t1, t2 - t0 - t1};
+        if constexpr (P::FQ2_NR == -1) return {t0 - t1, t2 - t0 - t1};
+        else return {t0 - times5(t1), t2 - t0 - t1};
     }
-    // (c0 + c1 u)^2 = (c0 + c1)(c0 - c1) + 2 c0 c1 u
+    // u^2 = -1: (c0 + c1 u)^2 = (c0 + c1)(c0 - c1) + 2 c0 c1 u
+    // u^2 = -5: c0^2 - 5 c1^2 = (c0 + c1)(c0 - 5 c1) + 4 c0 c1
     B2S_HD Fp2 sqr() const {
-        B s = (c0 + c1) * (c0 - c1);
-        B t = c0 * c1;
-        return {s, t.dbl()};
+        if constexpr (P::FQ2_NR == -1) {
+            B s = (c0 + c1) * (c0 - c1);
+            B t = c0 * c1;
+            return {s, t.dbl()};
+        } else {
+            B t = c0 * c1;
+            B t2 = t.dbl();
+            B s = (c0 + c1) * (c0 - times5(c1)) + t2.dbl();
+            return {s, t2};
+        }
     }
     B2S_HD Fp2& operator+=(const Fp2& o) { *this = *this + o; return *this; }
     B2S_HD Fp2& operator-=(const Fp2& o) { *this = *this - o; return *this; }
     B2S_HD Fp2& operator*=(const Fp2& o) { *this = *this * o; return *this; }
+    // 1 / (c0 + c1 u) = (c0 - c1 u) / (c0^2 - FQ2_NR c1^2)
     B2S_HD Fp2 inverse() const {
-        B n = (c0.sqr() + c1.sqr()).inverse();
+        B n;
+        if constexpr (P::FQ2_NR == -1) n = (c0.sqr() + c1.sqr()).inverse();
+        else n = (c0.sqr() + times5(c1.sqr())).inverse();
         return {c0 * n, (c1 * n).neg()};
     }
 };

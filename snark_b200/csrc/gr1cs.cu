@@ -279,6 +279,7 @@ constexpr R1csPoly r1cs_poly() {
 }
 __device__ R1csPoly r1cs_poly_bls = r1cs_poly<BlsFrP>();
 __device__ R1csPoly r1cs_poly_bn = r1cs_poly<BnFrP>();
+__device__ R1csPoly r1cs_poly_bls377 = r1cs_poly<Bls377FrP>();
 
 }  // namespace
 
@@ -303,9 +304,12 @@ int32_t r1cs_check(Ctx* c, const b2s_r1cs* m, uint64_t n_assign, const void* z, 
     return dispatch_curve(c, [&](auto curve) {
         using C = decltype(curve);
         using FrP = typename C::FrP;
-        static_assert(std::is_same<FrP, BlsFrP>::value || std::is_same<FrP, BnFrP>::value, "one R1CS polynomial per curve");
+        static_assert(std::is_same<FrP, BlsFrP>::value || std::is_same<FrP, BnFrP>::value || std::is_same<FrP, Bls377FrP>::value,
+                      "one R1CS polynomial per curve");
         void* poly = nullptr;
-        B2S_CUDA(c, cudaGetSymbolAddress(&poly, std::is_same<FrP, BlsFrP>::value ? r1cs_poly_bls : r1cs_poly_bn));
+        B2S_CUDA(c, cudaGetSymbolAddress(&poly, std::is_same<FrP, BlsFrP>::value  ? r1cs_poly_bls
+                                                : std::is_same<FrP, BnFrP>::value ? r1cs_poly_bn
+                                                                                  : r1cs_poly_bls377));
         const char* d = static_cast<const char*>(poly);
         PredView v{};
         for (int j = 0; j < 3; j++) {

@@ -1184,10 +1184,17 @@ int32_t msm_run_batch(Ctx* c, int group, const void* bases_dev, const void* scal
     });
 }
 
+// bits of the ctx curve's scalar field: 255 (BLS12-381), 254 (BN254), 253 (BLS12-377)
+static uint32_t fr_bits(Ctx* c) {
+    uint32_t bits = 0;
+    dispatch_curve(c, [&](auto curve) { bits = decltype(curve)::FrP::BITS; return (int32_t)B2S_OK; });
+    return bits;
+}
+
 // Per vector of a batch: device bytes of an MSM over n points, and how many vectors the u32 entry and bucket indices allow.
 uint64_t msm_batch_bytes(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint64_t* max_k) {
     const Sizes z = sizes(c);
-    const uint32_t bits = c->curve == B2S_CURVE_BLS12_381 ? 255 : 254;
+    const uint32_t bits = fr_bits(c);
     const size_t pt = z.xyzz(group);
     const MsmShape sh = msm_shape(std::max<uint64_t>(n, 1), bits, pt, pre);
     const uint64_t T = (uint64_t)sh.nwin * n, G = sh.G;
@@ -1220,7 +1227,7 @@ __global__ void __launch_bounds__(128) msm_precompute_kernel(const Affine<F>* __
 uint32_t msm_precompute_windows(Ctx* c, uint64_t n, uint32_t* c_out) {
     // one bucket set whatever the number of windows: c = 20 balances n * nwin additions against 2^(c-1) buckets from 2^18 points up
     (void)n;
-    const uint32_t bits = c->curve == B2S_CURVE_BLS12_381 ? 255 : 254;
+    const uint32_t bits = fr_bits(c);
     const uint32_t cc = env_u32("B2S_MSM_PRE_C", 20);
     uint32_t nw = (bits + cc - 1) / cc;
     if (bits - (nw - 1) * cc >= cc) nw += 1;

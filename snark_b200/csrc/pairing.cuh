@@ -1,4 +1,4 @@
-// Optimal ate pairing on BLS12-381 and BN254: the Fq6 / Fq12 tower, the Miller loop (on-the-fly or prepared lines, several
+// Optimal ate pairing on BLS12-381, BN254 and BLS12-377: the Fq6 / Fq12 tower, the Miller loop (on-the-fly or prepared lines, several
 // pairs sharing one squaring per step), the final exponentiation, and the Groth16 verdict.  Written B2S_HD like
 // deserialize.cuh, so tests/native/host_pairing.cpp compiles the same code for the CPU and checks it against the oracle.
 //
@@ -11,11 +11,14 @@
 //     because x < 0.  A line through T evaluated at P, times w^3 and an Fq2 factor, is  l0 + l1 xP w^2 + l2 yP w^3.
 //   BN254 (D-type twist y^2 = x^3 + 3 / xi, untwist (x w^2, y w^3)): over the signed digits of 6x + 2, then the lines
 //     through pi(Q) and -pi^2(Q).  A line, times an Fq2 factor, is  l0 yP + l1 xP w + l2 w^3.
+//   BLS12-377 (D-type twist y^2 = x^3 + 1 / u, xi = u with u^2 = -5): over the bits of x > 0, no conjugation and no
+//     Frobenius lines; the lines have BN254's shape.  The twist type (M_TWIST) and the family (BLS12_FAMILY) are traits.
 //   The dropped factors (w^3, Fq2 scalars) and the vertical lines lie in proper subfields of Fq12 that the easy part
 //   of the final exponentiation maps to 1.  A pair with P or Q at infinity (all-zero) contributes 1.
 //
 // Final exponentiation: the easy part (p^6 - 1)(p^2 + 1), then a hard part that computes f^(m h), h = (p^4 - p^2 + 1) / r:
-//   BLS12-381  m = 3:  3 h = (x - 1)^2 (x + p)(x^2 + p^2 - 1) + 3                 (Hayashida, Hayasaka, Teruya 2020)
+//   BLS12      m = 3:  3 h = (x - 1)^2 (x + p)(x^2 + p^2 - 1) + 3                 (Hayashida, Hayasaka, Teruya 2020)
+//              (both BLS12 curves; cyclotomic_exp_x takes the sign of x into account)
 //   BN254      m = 2x (6x^2 + 3x + 1):  m h = l0 + l1 p + l2 p^2 + l3 p^3 with      (Fuentes-Castaneda, Knapp,
 //              l0 = 1 + 6x + 12x^2 + 12x^3, l1 = 4x + 6x^2 + 12x^3,                    Rodriguez-Henriquez 2011)
 //              l2 = 6x + 6x^2 + 12x^3, l3 = -1 + 4x + 6x^2 + 12x^3
@@ -32,7 +35,8 @@
 //                6x + 2 + p - p^2 + p^3 = n r, and the optimal ate value (Vercauteren 2010) is
 //                e_opt = [f_{nr,Q}(P)] / a_p^(1 - 2p + 3p^2) = t^n / a_p^(1 - 2p + 3p^2)
 //              so e = e_opt^m with m the hard-part multiplier above; k is that exponent reduced mod r.
-//   Both k are coprime to r, so e is bilinear and non-degenerate; tests/test_host_pairing.py recomputes k from these
+//   BLS12-377  k = 3.  T = x > 0, the same Miller function and no conjugation; the hard part raises to m = 3.
+//   Every k is coprime to r, so e is bilinear and non-degenerate; tests/test_host_pairing.py recomputes k from these
 //   formulas and checks e = o^k on random pairs.
 #pragma once
 #include "curves.cuh"
@@ -52,13 +56,18 @@ template <class P>
 B2S_HD Fp2<P> conj(const Fp2<P>& a) { return {a.c0, a.c1.neg()}; }
 template <class P>
 B2S_HD Fp2<P> scale(const Fp2<P>& a, const Fp<P>& s) { return {a.c0 * s, a.c1 * s}; }
-// a * xi, xi = XI0 + u:  (XI0 a0 - a1) + (a0 + XI0 a1) u
+// a * xi, xi = XI0 + u:  (XI0 a0 - a1) + (a0 + XI0 a1) u for u^2 = -1;  a * u = -5 a1 + a0 u for xi = u, u^2 = -5
 template <class P>
 B2S_HD Fp2<P> mul_xi(const Fp2<P>& a) {
-    static_assert(P::XI0 == 1 || P::XI0 == 9, "xi = 1 + u or 9 + u");
-    if (P::XI0 == 1) return {a.c0 - a.c1, a.c0 + a.c1};
-    const Fp<P> n0 = a.c0.dbl().dbl().dbl() + a.c0, n1 = a.c1.dbl().dbl().dbl() + a.c1;
-    return {n0 - a.c1, a.c0 + n1};
+    static_assert((P::FQ2_NR == -1 && (P::XI0 == 1 || P::XI0 == 9)) || (P::FQ2_NR == -5 && P::XI0 == 0),
+                  "xi = 1 + u or 9 + u with u^2 = -1, or xi = u with u^2 = -5");
+    if constexpr (P::XI0 == 0) {
+        return {Fp2<P>::times5(a.c1).neg(), a.c0};
+    } else {
+        if (P::XI0 == 1) return {a.c0 - a.c1, a.c0 + a.c1};
+        const Fp<P> n0 = a.c0.dbl().dbl().dbl() + a.c0, n1 = a.c1.dbl().dbl().dbl() + a.c1;
+        return {n0 - a.c1, a.c0 + n1};
+    }
 }
 template <class P>
 B2S_HD Fp2<P> frob_coeff(int j, int k) {   // xi^(k (p^j - 1) / 6), j = 1..3, k = 1..5
@@ -234,7 +243,7 @@ struct G2Proj { Fp2<P> x, y, z; };     // (X : Y : Z) = (X/Z, Y/Z) on the twist
 template <class Curve>
 struct PairingShape {
     using P = typename Curve::FqP;
-    static constexpr bool M_TWIST = Curve::id == Bls12_381::id;   // BN254: D-type
+    static constexpr bool M_TWIST = P::M_TWIST;   // BLS12-381: M-type; BN254, BLS12-377: D-type
     static constexpr int digits_nonzero() {
         int n = 0;
         for (int i = 0; i < P::ATE_WORDS; i++) {
@@ -244,7 +253,7 @@ struct PairingShape {
         return n;
     }
     // doublings + additions (the top digit starts T = Q) + the two Frobenius lines of BN254
-    static constexpr int LINES = (P::ATE_BITS - 1) + (digits_nonzero() - 1) + (M_TWIST ? 0 : 2);
+    static constexpr int LINES = (P::ATE_BITS - 1) + (digits_nonzero() - 1) + (P::BLS12_FAMILY ? 0 : 2);
 };
 
 // ark's G2Prepared for one fixed Q: the lines in the order the Miller loop consumes them; inf = Q at infinity
@@ -338,7 +347,7 @@ B2S_HD void line_schedule(const Affine<Fp2<typename Curve::FqP>>& q, Emit&& emit
         const int d = ate_digit<P>(b);
         if (d) emit(add_step<Curve>(t, d > 0 ? q : qn));
     }
-    if (!PairingShape<Curve>::M_TWIST) {
+    if (!P::BLS12_FAMILY) {
         const Affine<Fp2<P>> q1 = twist_frobenius(q);
         emit(add_step<Curve>(t, q1));
         emit(add_step<Curve>(t, twist_frobenius(q1).neg()));
@@ -391,7 +400,7 @@ B2S_PAIR_NOINLINE Fp12<typename Curve::FqP> multi_miller_loop(const Affine<Fp<ty
             prepared();
         }
     }
-    if (!PairingShape<Curve>::M_TWIST) {
+    if (!P::BLS12_FAMILY) {
         for (int i = 0; i < NF; i++) {
             const Affine<Fp2<P>> q1 = twist_frobenius(qf[i]);
             const Line<P> l1 = add_step<Curve>(t[i], q1);
@@ -409,7 +418,7 @@ B2S_PAIR_NOINLINE Fp12<P> final_exponentiation(const Fp12<P>& f) {
     // easy part: f^((p^6 - 1)(p^2 + 1)); afterwards f lies in the cyclotomic subgroup
     Fp12<P> e = fp12_mul(f.conj(), fp12_inverse(f));
     e = fp12_mul(fp12_frobenius(e, 2), e);
-    if (P::X_NEG) {   // BLS12-381: e^((x - 1)^2 (x + p)(x^2 + p^2 - 1) + 3)
+    if (P::BLS12_FAMILY) {   // BLS12-381, BLS12-377: e^((x - 1)^2 (x + p)(x^2 + p^2 - 1) + 3)
         Fp12<P> t = fp12_mul(cyclotomic_exp_x(e), e.conj());        // e^(x - 1)
         t = fp12_mul(cyclotomic_exp_x(t), t.conj());                  // e^((x - 1)^2)
         t = fp12_mul(cyclotomic_exp_x(t), fp12_frobenius(t, 1));      // ^(x + p)

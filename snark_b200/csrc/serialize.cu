@@ -4,7 +4,7 @@
 // /root/reference, SURVEY.md Appendix A.7):
 //   BLS12-381 (zcash / IETF form): x big-endian; top bits of byte 0: 0x80 compressed, 0x40 infinity, 0x20 y is the
 //                                  lexicographically larger root; G2 writes x.c1 || x.c0
-//   BN254 (ark-ec SWFlags):        x little-endian; top bits of the LAST byte: 0x80 y > -y, 0x40 infinity; G2 writes
+//   BN254, BLS12-377 (ark-ec SWFlags): x little-endian; top bits of the LAST byte: 0x80 y > -y, 0x40 infinity; G2 writes
 //                                  x.c0 || x.c1
 //   "larger" compares canonical integers; for Fq2, c1 first then c0.   Proof = A || B || C.
 //   Uncompressed: x || y in the same byte / component order; BLS12-381 keeps only the infinity bit (0x40) in byte 0, BN254
@@ -82,7 +82,8 @@ static void encode_point(bool bls, int group, bool compressed, size_t fq, const 
 
 // `count` affine Montgomery points (HOST or DEVICE) -> encoded bytes on the host; chunked so that keys of any size stream through
 int32_t serialize_points_ex(Ctx* c, int group, const void* affine, int32_t mem, uint64_t count, bool compressed, uint8_t* out, uint64_t cap) {
-    const bool bls = c->curve == B2S_CURVE_BLS12_381;
+    bool bls = false;   // zcash / IETF form (BLS12-381); otherwise ark-ec SWFlags (BN254, BLS12-377)
+    B2S_TRY(dispatch_curve(c, [&](auto curve) { bls = decltype(curve)::FqP::ZCASH_SERIAL; return (int32_t)B2S_OK; }));
     const Sizes z = sizes(c);
     const size_t in_bytes = z.aff(group), out_bytes = z.enc(group, compressed);
     if (count * out_bytes > cap) return fail(c, B2S_ERR_INVALID_ARG, "serialize: output buffer too small");

@@ -7,7 +7,7 @@ from ctypes import POINTER, c_char_p, c_int32, c_uint32, c_uint64, c_void_p
 
 import numpy as np
 
-BLS12_381, BN254 = 0, 1
+BLS12_381, BN254, BLS12_377 = 0, 1, 2
 MEM_HOST, MEM_DEVICE = 0, 1
 QAP_LIBSNARK, QAP_CIRCOM = 0, 1   # QAP reduction of a Groth16 key: ark-groth16's LibsnarkReduction / ark-circom's CircomReduction
 
@@ -41,7 +41,8 @@ GR1CS_MAX_ARITY = 8
 NOT_FOUND = np.uint64(0xFFFFFFFFFFFFFFFF)   # first_unsat of a satisfied predicate
 # scalar-field moduli, for the Montgomery form of the Python-int coefficients gr1cs_upload takes
 FR_MODULUS = {BLS12_381: 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001,
-              BN254: 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001}
+              BN254: 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001,
+              BLS12_377: 0x12AB655E9A2CA55660B44D1E5C37B00159AA76FED00000010A11800000000001}
 
 
 class PredicateDesc(ctypes.Structure):

@@ -23,6 +23,10 @@ _PARAMS = {
         r=21888242871839275222246405745257275088548364400416034343698204186575808495617,
         p=21888242871839275222246405745257275088696311157297823662689037894645226208583,
         gen=5, two_adicity=28),
+    L.BLS12_377: dict(
+        r=0x12ab655e9a2ca55660b44d1e5c37b00159aa76fed00000010a11800000000001,
+        p=0x01ae3a4617c510eac63b05c06ca1493b1a22d9f300f5138f1ef3622fba094800170b5d44300000008508c00000000001,
+        gen=22, two_adicity=47),
 }
 
 
