@@ -63,8 +63,8 @@ extern "C" {
  *                     h_query[j] = L^(2N)_{2j+1}(tau) / delta (the odd-indexed Lagrange basis of the size-2N domain, as snarkjs
  *                     writes it).  The rest of the key and the proof are unchanged; the verifiers below take circom proofs as
  *                     they are.  Not provided: the distributed witness map (b2s_groth16_prove_group* refuse circom keys with
- *                     B2S_ERR_INVALID_ARG; b2s_groth16_prove_shard + b2s_groth16_finish work), and readers of snarkjs
- *                     .zkey / .wtns files (ark-circom turns a zkey into an ark ProvingKey: b2s_pk_deserialize_qap).
+ *                     B2S_ERR_INVALID_ARG; b2s_groth16_prove_shard + b2s_groth16_finish work).  snarkjs .zkey and circom
+ *                     .wtns files load directly: b2s_zkey_load / b2s_wtns_read below.
  * Any other value is B2S_ERR_INVALID_ARG. */
 #define B2S_QAP_LIBSNARK 0
 #define B2S_QAP_CIRCOM 1
@@ -378,6 +378,38 @@ int32_t b2s_vk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_
 int32_t b2s_pk_deserialize(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, b2s_pk** out);
 int32_t b2s_pk_deserialize_qap(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t compressed, int32_t validate, int32_t qap,
                                b2s_pk** out);
+
+/* ---- snarkjs files: Groth16 .zkey and circom .wtns (ark-circom read_zkey, snarkjs zkey_utils.js / wtns_utils.js) ---------
+ * The formats are restated from snarkjs / ark-circom in snark_b200/csrc/zkey.cu; they are NOT pinned against bytes written
+ * by snarkjs.  Bytes on the HOST; the host reads headers and section offsets only, and every framing and size check runs
+ * before anything is allocated.  Points (Montgomery little-endian limbs in the file, this library's own layout) are checked
+ * on the device: every coordinate < q always; with validate = 1 also the curve equation and the prime-order subgroup.
+ * Coefficient and witness values must always be < r.
+ *   b2s_zkey_read_info  the framing and the header: nVars, nPublic, domainSize and the number of coefficient entries.
+ *   b2s_zkey_load       a Groth16 zkey -> the handles b2s_pk_upload_qap(.., B2S_QAP_CIRCOM, ..) and b2s_r1cs_upload would
+ *                       build from the same points and matrices: a full circom key (n_instance = nPublic + 1, the h query
+ *                       table built as by b2s_pk_deserialize) and a matrix handle of A and B over the circuit's constraints
+ *                       with an EMPTY C (snarkjs's trailing input rows are checked and left to the witness map).  On such a
+ *                       handle b2s_r1cs_check checks A z o B z = 0, which is not the circuit's satisfaction.  The verifying key
+ *                       goes to the HOST in the form b2s_vk_prepare takes: alpha_g1, beta_g2, gamma_g2, delta_g2 and
+ *                       nPublic + 1 gamma_abc_g1 points (cap_gamma_abc = room in out_gamma_abc_g1).
+ *   b2s_wtns_read       a .wtns -> z = instance || witness, n_vars Montgomery Fr in `mem` (HOST or DEVICE), for
+ *                       b2s_groth16_prove_resident / _prove_batch (one call per row of a batch, at a row offset).
+ * Errors (b2s_last_error names the section or vector, the lowest failing index and the reason, e.g.
+ * "zkey B2[17]: not in the prime-order subgroup"):
+ *   B2S_ERR_INVALID_DATA    bad magic, version, framing, truncation or protocol (only Groth16 = 1); a matrix, constraint or
+ *                           signal field out of range; a non-canonical, off-curve or non-subgroup value; wtns z[0] != 1
+ *   B2S_ERR_INVALID_ARG     q / r of another curve than the ctx's; a null buffer; cap_gamma_abc too small
+ *   B2S_ERR_MALFORMED_VK    section sizes that disagree with nVars / nPublic / domainSize; missing or altered input rows;
+ *                           domainSize != next_pow2(constraints + nPublic + 1)
+ *   B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE  a domain past the limits of b2s_r1cs_upload
+ *   B2S_ERR_ASSIGNMENT_MISSING           nWitness != n_vars (snarkjs's "Invalid witness length") */
+typedef struct b2s_zkey_info { uint64_t n_vars, n_public, domain_size, n_coeffs; } b2s_zkey_info;
+int32_t b2s_zkey_read_info(b2s_ctx* ctx, const uint8_t* in, uint64_t len, b2s_zkey_info* out);
+int32_t b2s_zkey_load(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t validate, b2s_pk** out_pk, b2s_r1cs** out_m,
+                      void* out_alpha_g1, void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1,
+                      uint64_t cap_gamma_abc);
+int32_t b2s_wtns_read(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t n_vars, int32_t mem, void* out_z);
 
 /* ---- verification: pairings and batched Groth16 verify ----------------------------------------------------------------
  * The optimal ate pairing in CUDA (snark_b200/csrc/pairing.cuh): BLS12-381 loops over |x| and conjugates, BN254 over the

@@ -30,6 +30,10 @@ pub struct B2sPredicateDesc {
 }
 
 #[repr(C)]
+#[derive(Default)]
+pub struct B2sZkeyInfo { pub n_vars: u64, pub n_public: u64, pub domain_size: u64, pub n_coeffs: u64 }
+
+#[repr(C)]
 pub struct B2sPkDesc {
     pub n_instance: u64, pub n_witness: u64, pub domain_size: u64,
     pub alpha_g1: *const c_void, pub beta_g1: *const c_void, pub delta_g1: *const c_void,
@@ -86,6 +90,12 @@ extern "C" {
     pub fn b2s_pk_deserialize_qap(ctx: *mut B2sCtx, inp: *const u8, len: u64, compressed: i32, validate: i32, qap: i32,
                                   out: *mut *mut B2sPk) -> i32;
     pub fn b2s_pk_upload_qap(ctx: *mut B2sCtx, desc: *const B2sPkDesc, mem: i32, qap: i32, out: *mut *mut B2sPk) -> i32;
+    // snarkjs files (ark-circom read_zkey, snarkjs zkey_utils.js / wtns_utils.js), read and checked on the GPU
+    pub fn b2s_zkey_read_info(ctx: *mut B2sCtx, inp: *const u8, len: u64, out: *mut B2sZkeyInfo) -> i32;
+    pub fn b2s_zkey_load(ctx: *mut B2sCtx, inp: *const u8, len: u64, validate: i32, out_pk: *mut *mut B2sPk, out_m: *mut *mut B2sR1cs,
+                         out_alpha_g1: *mut c_void, out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void, out_delta_g2: *mut c_void,
+                         out_gamma_abc_g1: *mut c_void, cap_gamma_abc: u64) -> i32;
+    pub fn b2s_wtns_read(ctx: *mut B2sCtx, inp: *const u8, len: u64, n_vars: u64, mem: i32, out_z: *mut c_void) -> i32;
     pub fn b2s_groth16_setup_qap(ctx: *mut B2sCtx, m: *const B2sR1cs, trapdoor: *const c_void, qap: i32, out_pk: *mut *mut B2sPk,
                                  out_alpha_g1: *mut c_void, out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void,
                                  out_delta_g2: *mut c_void, out_gamma_abc_g1: *mut c_void) -> i32;
@@ -265,6 +275,37 @@ impl<E: Pairing + B200Curve> Groth16B200<E> {
             b2s_pk_deserialize_qap(ctx, pk_bytes.as_ptr(), pk_bytes.len() as u64, compressed as i32, validate as i32, qap, &mut pkh)
         })?;
         Ok(Resident { ctx, pk: pkh, mat })
+    }
+
+    /// The resident circom key, its matrices and its `VerifyingKey` straight from the bytes of a snarkjs Groth16 `.zkey`,
+    /// without ark-circom: the file is parsed and checked on the GPU (b2s_zkey_load; with `validate`, the curve equation
+    /// and the prime-order subgroup of every point).  The matrix handle holds A and B; C is empty, as the circom witness map
+    /// never reads it.  z for its proofs comes from the witness generator's `.wtns` via `b2s_wtns_read`.  The format is
+    /// restated from snarkjs, not pinned against its bytes.
+    pub fn make_resident_from_zkey(curve_id: i32, zkey: &[u8], validate: bool) -> Result<(Resident, VerifyingKey<E>), B200Error>
+    where <E::G1Affine as AffineRepr>::BaseField: Copy, <E::G2Affine as AffineRepr>::BaseField: Copy {
+        if curve_id != E::CURVE_ID { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        let mut ctx: *mut B2sCtx = core::ptr::null_mut();
+        check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
+        let fail = |ctx: *mut B2sCtx, st: i32| -> B200Error { unsafe { b2s_ctx_destroy(ctx) }; B200Error::from_status(st) };
+        let mut info = B2sZkeyInfo::default();
+        let st = unsafe { b2s_zkey_read_info(ctx, zkey.as_ptr(), zkey.len() as u64, &mut info) };
+        if st != 0 { return Err(fail(ctx, st)); }
+        let g1 = 2 * core::mem::size_of::<<E::G1Affine as AffineRepr>::BaseField>();
+        let n_abc = info.n_public as usize + 1;
+        let (mut alpha, mut beta, mut gamma, mut delta, mut abc) = (vec![0u8; g1], vec![0u8; 2 * g1], vec![0u8; 2 * g1], vec![0u8; 2 * g1],
+                                                                    vec![0u8; n_abc * g1]);
+        let (mut pk, mut mat): (*mut B2sPk, *mut B2sR1cs) = (core::ptr::null_mut(), core::ptr::null_mut());
+        let st = unsafe {
+            b2s_zkey_load(ctx, zkey.as_ptr(), zkey.len() as u64, validate as i32, &mut pk, &mut mat, alpha.as_mut_ptr().cast(),
+                          beta.as_mut_ptr().cast(), gamma.as_mut_ptr().cast(), delta.as_mut_ptr().cast(), abc.as_mut_ptr().cast(), n_abc as u64)
+        };
+        if st != 0 { return Err(fail(ctx, st)); }
+        let vk = VerifyingKey {
+            alpha_g1: unpack_point(&alpha), beta_g2: unpack_point(&beta), gamma_g2: unpack_point(&gamma), delta_g2: unpack_point(&delta),
+            gamma_abc_g1: abc.chunks(g1).map(unpack_point::<E::G1Affine>).collect(),
+        };
+        Ok((Resident { ctx, pk, mat }, vk))
     }
 
     /// `prove` for many circuits of one shape under one resident key, in one GPU call (b2s_groth16_prove_batch): each

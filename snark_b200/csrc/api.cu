@@ -34,6 +34,11 @@ int32_t proof_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compress
 int32_t vk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, void* alpha, void* beta, void* gamma,
                        void* delta, void* abc, uint64_t cap_abc, uint64_t* n_abc, uint64_t* consumed);
 int32_t pk_deserialize(Ctx* c, const uint8_t* in, uint64_t len, bool compressed, bool validate, int32_t qap, b2s_pk** out);
+// zkey.cu
+int32_t zkey_read_info(Ctx* c, const uint8_t* in, uint64_t len, b2s_zkey_info* out);
+int32_t zkey_load(Ctx* c, const uint8_t* in, uint64_t len, bool validate, b2s_pk** out_pk, b2s_r1cs** out_m, void* alpha_g1,
+                  void* beta_g2, void* gamma_g2, void* delta_g2, void* gamma_abc, uint64_t cap_abc);
+int32_t wtns_read(Ctx* c, const uint8_t* in, uint64_t len, uint64_t n_vars, int32_t mem, void* out_z);
 // verify.cu
 int32_t vk_prepare(Ctx* c, const void* alpha, const void* beta, const void* gamma, const void* delta, const void* abc, uint64_t n_abc,
                    b2s_pvk** out);
@@ -683,6 +688,28 @@ int32_t b2s_pk_deserialize_qap(b2s_ctx* ctx, const uint8_t* in, uint64_t len, in
     *out = nullptr;
     B2S_TRY(check_qap(ctx, qap, "pk_deserialize"));
     return pk_deserialize(ctx, in, len, compressed != 0, validate != 0, qap, out);
+}
+
+int32_t b2s_zkey_read_info(b2s_ctx* ctx, const uint8_t* in, uint64_t len, b2s_zkey_info* out) {
+    LOCK(ctx);
+    if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "zkey_read_info: null argument");
+    return zkey_read_info(ctx, in, len, out);
+}
+int32_t b2s_zkey_load(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t validate, b2s_pk** out_pk, b2s_r1cs** out_m,
+                      void* out_alpha_g1, void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1,
+                      uint64_t cap_gamma_abc) {
+    LOCK(ctx);
+    if (!in || !out_pk || !out_m || !out_alpha_g1 || !out_beta_g2 || !out_gamma_g2 || !out_delta_g2 || !out_gamma_abc_g1)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "zkey_load: null argument");
+    *out_pk = nullptr;
+    *out_m = nullptr;
+    return zkey_load(ctx, in, len, validate != 0, out_pk, out_m, out_alpha_g1, out_beta_g2, out_gamma_g2, out_delta_g2,
+                     out_gamma_abc_g1, cap_gamma_abc);
+}
+int32_t b2s_wtns_read(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t n_vars, int32_t mem, void* out_z) {
+    LOCK(ctx);
+    if (!in || !out_z) return fail(ctx, B2S_ERR_INVALID_ARG, "wtns_read: null argument");
+    return wtns_read(ctx, in, len, n_vars, mem, out_z);
 }
 
 int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,

@@ -12,127 +12,11 @@
 #include "common.cuh"
 #include "deserialize.cuh"
 #include "r1cs.cuh"
+#include "stager.cuh"
 
 namespace b2s {
 
 int32_t pk_finish(Ctx* c, b2s_pk* pk);   // groth16.cu
-
-template <class Curve, class F>
-__global__ void decode_points_kernel(const uint8_t* in, uint32_t n, uint32_t pb, int compressed, int validate, uint64_t base,
-                                     Affine<F>* out, unsigned long long* err) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    Affine<F> p = Affine<F>::inf();
-    const uint32_t st = decode_point<Curve, F>(in + (size_t)i * pb, compressed != 0, validate != 0, p);
-    if (st != DEC_OK) {
-        atomicMin(err, (unsigned long long)((base + i) << 3 | st));   // lowest failing index, with its reason
-        p = Affine<F>::inf();
-    }
-    out[i] = p;
-}
-
-static const char* reason_text(uint32_t st) {
-    switch (st) {
-        case DEC_BAD_FLAGS: return "bad flags";
-        case DEC_NONCANONICAL: return "coordinate not below p";
-        case DEC_NOT_ON_CURVE: return "not on the curve";
-        case DEC_NOT_IN_SUBGROUP: return "not in the prime-order subgroup";
-    }
-    return "invalid";
-}
-
-// Two pinned host buffers and two device buffers, reused by every vector of one call.
-struct Stager {
-    static constexpr uint64_t CH = 1u << 18;   // points per chunk
-    Ctx* c;
-    size_t cap = 0;
-    uint8_t* pinned[2] = {nullptr, nullptr};
-    DevBuf dev[2], err;
-    cudaEvent_t copied[2] = {nullptr, nullptr}, consumed[2] = {nullptr, nullptr};
-    explicit Stager(Ctx* ctx) : c(ctx) {}
-    ~Stager() {
-        cudaStreamSynchronize(c->side);
-        cudaStreamSynchronize(c->stream);
-        for (int s = 0; s < 2; s++) {
-            if (pinned[s]) cudaFreeHost(pinned[s]);
-            if (copied[s]) cudaEventDestroy(copied[s]);
-            if (consumed[s]) cudaEventDestroy(consumed[s]);
-        }
-    }
-    int32_t reserve(size_t bytes) {
-        if (!err.p) {
-            B2S_TRY(err.alloc(c, sizeof(unsigned long long)));
-            for (int s = 0; s < 2; s++) {
-                B2S_CUDA(c, cudaEventCreateWithFlags(&copied[s], cudaEventDisableTiming));
-                B2S_CUDA(c, cudaEventCreateWithFlags(&consumed[s], cudaEventDisableTiming));
-            }
-        }
-        if (bytes <= cap) return B2S_OK;
-        B2S_CUDA(c, cudaStreamSynchronize(c->side));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        for (int s = 0; s < 2; s++) {
-            if (pinned[s]) cudaFreeHost(pinned[s]);
-            pinned[s] = nullptr;
-            B2S_CUDA(c, cudaMallocHost(&pinned[s], bytes));
-            B2S_TRY(dev[s].alloc(c, bytes));
-        }
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));   // the side stream copies into dev[] allocated on the ctx stream
-        cap = bytes;
-        return B2S_OK;
-    }
-
-    // `count` encodings from the HOST -> affine Montgomery points at out_dev; `name` labels the error message
-    int32_t decode(int group, const uint8_t* in, uint64_t count, bool compressed, bool validate, void* out_dev, const char* name) {
-        if (!count) return B2S_OK;
-        const size_t pb = sizes(c).enc(group, compressed), ab = sizes(c).aff(group);
-        B2S_TRY(reserve((size_t)std::min<uint64_t>(count, CH) * pb));
-        B2S_CUDA(c, cudaMemsetAsync(err.p, 0xFF, sizeof(unsigned long long), c->stream));
-        for (uint64_t base = 0, k = 0; base < count; base += CH, k++) {
-            const int s = (int)(k & 1);
-            const uint32_t n = (uint32_t)std::min<uint64_t>(CH, count - base);
-            if (k >= 2) B2S_CUDA(c, cudaEventSynchronize(copied[s]));   // pinned[s] is free again
-            memcpy(pinned[s], in + base * pb, (size_t)n * pb);
-            if (k >= 2) B2S_CUDA(c, cudaStreamWaitEvent(c->side, consumed[s], 0));   // dev[s] has been decoded
-            B2S_CUDA(c, cudaMemcpyAsync(dev[s].p, pinned[s], (size_t)n * pb, cudaMemcpyHostToDevice, c->side));
-            B2S_CUDA(c, cudaEventRecord(copied[s], c->side));
-            B2S_CUDA(c, cudaStreamWaitEvent(c->stream, copied[s], 0));
-            char* dst = static_cast<char*>(out_dev) + base * ab;
-            const uint8_t* src = dev[s].as<uint8_t>();
-            unsigned long long* e = err.as<unsigned long long>();
-            int32_t st = dispatch_curve(c, [&](auto curve) {
-                using C = decltype(curve);
-                if (group == 1) {
-                    auto kern = decode_points_kernel<C, typename C::Fq>;
-                    B2S_LAUNCH_N(c, "decode_points_g1", kern, cdiv(n, 128), 128, 0, src, n, (uint32_t)pb, (int)compressed, (int)validate,
-                                 base, reinterpret_cast<Affine<typename C::Fq>*>(dst), e);
-                } else {
-                    auto kern = decode_points_kernel<C, typename C::Fq2>;
-                    B2S_LAUNCH_N(c, "decode_points_g2", kern, cdiv(n, 128), 128, 0, src, n, (uint32_t)pb, (int)compressed, (int)validate,
-                                 base, reinterpret_cast<Affine<typename C::Fq2>*>(dst), e);
-                }
-                return (int32_t)B2S_OK;
-            });
-            B2S_TRY(st);
-            B2S_CUDA(c, cudaEventRecord(consumed[s], c->stream));
-        }
-        unsigned long long word = 0;
-        B2S_CUDA(c, cudaMemcpyAsync(&word, err.p, sizeof(word), cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        if (word != ~0ull)
-            return fail(c, B2S_ERR_INVALID_DATA, "%s[%llu]: %s", name, (unsigned long long)(word >> 3), reason_text((uint32_t)(word & 7)));
-        return B2S_OK;
-    }
-    // the same into HOST memory
-    int32_t decode_host(int group, const uint8_t* in, uint64_t count, bool compressed, bool validate, void* out_host, const char* name) {
-        if (!count) return B2S_OK;
-        DevBuf out;
-        B2S_TRY(out.alloc(c, count * sizes(c).aff(group)));
-        B2S_TRY(decode(group, in, count, compressed, validate, out.p, name));
-        B2S_CUDA(c, cudaMemcpyAsync(out_host, out.p, count * sizes(c).aff(group), cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        return B2S_OK;
-    }
-};
 
 int32_t deserialize_points(Ctx* c, int group, const uint8_t* in, uint64_t len, uint64_t count, bool compressed, bool validate,
                            void* out_host) {

@@ -87,12 +87,19 @@ B2S_HD Fp<P>& top_elem(Fp<P>& x) { return x; }
 template <class P>
 B2S_HD Fp<P>& top_elem(Fp2<P>& x) { return x.c1; }
 
+// raw limbs below the modulus (of either field: P is FqP or FrP)
+template <class P>
+B2S_HD bool below_p(const Fp<P>& a) {
+    int c = 0;
+    for (int i = Fp<P>::N - 1; i >= 0 && c == 0; i--) c = a.v[i] < P::mod(i) ? -1 : a.v[i] > P::mod(i) ? 1 : 0;
+    return c < 0;
+}
+template <class P>
+B2S_HD bool below_p(const Fp2<P>& a) { return below_p(a.c0) && below_p(a.c1); }
 // raw limbs -> Montgomery form; false if the value is not below p
 template <class P>
 B2S_HD bool to_field(Fp<P>& a) {
-    int c = 0;
-    for (int i = Fp<P>::N - 1; i >= 0 && c == 0; i--) c = a.v[i] < P::mod(i) ? -1 : a.v[i] > P::mod(i) ? 1 : 0;
-    if (c >= 0) return false;
+    if (!below_p(a)) return false;
     a = a.to_mont();
     return true;
 }
@@ -292,6 +299,27 @@ B2S_HD uint32_t decode_point(const uint8_t* in, bool compressed, bool validate, 
         if (!dec::to_field(y)) return DEC_NONCANONICAL;
         if (validate && y.sqr() != rhs) return DEC_NOT_ON_CURVE;
     }
+    out = Affine<F>{x, y};
+    if (validate && !dec::in_subgroup<Curve>(out)) return DEC_NOT_IN_SUBGROUP;
+    return DEC_OK;
+}
+
+// One point as a snarkjs .zkey stores it (zkey.cu): x || y as Montgomery little-endian limbs, G2 coordinates c0 || c1 --
+// already this library's affine layout -- with infinity all-zero.  No flags and no square root: every coordinate must be
+// below p; with validate the point must satisfy the curve equation and the subgroup criterion of decode_point.
+template <class Curve, class F>
+B2S_HD uint32_t decode_point_mont(const uint8_t* in, bool validate, Affine<F>& out) {
+    using P = typename Curve::FqP;
+    constexpr int CB = (int)(sizeof(F) / sizeof(Fp<P>)) * 4 * Fp<P>::N;
+    F x, y;
+    dec::load_coord(in, false, x);
+    dec::load_coord(in + CB, false, y);
+    if (x.is_zero() && y.is_zero()) {
+        out = Affine<F>::inf();
+        return DEC_OK;
+    }
+    if (!dec::below_p(x) || !dec::below_p(y)) return DEC_NONCANONICAL;
+    if (validate && y.sqr() != x.sqr() * x + dec::curve_b((const F*)nullptr)) return DEC_NOT_ON_CURVE;
     out = Affine<F>{x, y};
     if (validate && !dec::in_subgroup<Curve>(out)) return DEC_NOT_IN_SUBGROUP;
     return DEC_OK;

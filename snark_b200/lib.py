@@ -45,6 +45,10 @@ FR_MODULUS = {BLS12_381: 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFF
               BLS12_377: 0x12AB655E9A2CA55660B44D1E5C37B00159AA76FED00000010A11800000000001}
 
 
+class ZkeyInfo(ctypes.Structure):
+    _fields_ = [("n_vars", c_uint64), ("n_public", c_uint64), ("domain_size", c_uint64), ("n_coeffs", c_uint64)]
+
+
 class PredicateDesc(ctypes.Structure):
     _fields_ = [
         ("arity", c_uint32), ("n_terms", c_uint32),
@@ -145,6 +149,9 @@ SIGNATURES = {
                            + [c_uint64, POINTER(c_uint64), POINTER(c_uint64)]),
     "b2s_pk_deserialize": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_pk_deserialize_qap": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, c_int32, c_int32, POINTER(c_void_p)]),
+    "b2s_zkey_read_info": (c_int32, [c_void_p, c_void_p, c_uint64, POINTER(ZkeyInfo)]),
+    "b2s_zkey_load": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, POINTER(c_void_p), POINTER(c_void_p)] + [c_void_p] * 5 + [c_uint64]),
+    "b2s_wtns_read": (c_int32, [c_void_p, c_void_p, c_uint64, c_uint64, c_int32, c_void_p]),
     "b2s_vk_prepare": (c_int32, [c_void_p] * 6 + [c_uint64, POINTER(c_void_p)]),
     "b2s_pvk_free": (None, [c_void_p, c_void_p]),
     "b2s_groth16_verify_batch": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_int32,
@@ -564,6 +571,48 @@ class Backend:
 
     def pk_free(self, pk):
         self.lib.b2s_pk_free(self.h, pk)
+
+    # ---- snarkjs files (.zkey / .wtns) --------------------------------------------------------------------------------
+    @staticmethod
+    def _file_bytes(data):
+        """bytes-like or numpy array (an np.memmap of the file included) -> a uint8 view of the same memory, not a copy"""
+        if isinstance(data, np.ndarray):
+            assert data.flags["C_CONTIGUOUS"]
+            return data.reshape(-1).view(np.uint8)
+        return np.frombuffer(data, dtype=np.uint8)
+
+    def zkey_info(self, data):
+        """Header of a snarkjs Groth16 .zkey: {n_vars, n_public, domain_size, n_coeffs}."""
+        buf = self._file_bytes(data)
+        info = ZkeyInfo()
+        self._ck(self.lib.b2s_zkey_read_info(self.h, buf.ctypes.data, buf.nbytes, ctypes.byref(info)))
+        return {name: int(getattr(info, name)) for name, _ in ZkeyInfo._fields_}
+
+    def zkey_load(self, data, validate=True):
+        """A snarkjs Groth16 .zkey (bytes, or a numpy array / np.memmap of the file) -> (pk, m, vk): the device-resident
+        circom key, the matrix handle (A and B, C empty) and the verifying key in the layout vk_from_bytes returns."""
+        buf = self._file_bytes(data)
+        info = self.zkey_info(buf)
+        n_abc = info["n_public"] + 1
+        vk = {"alpha_g1": np.zeros(self.g1_bytes // 4, dtype=np.uint32), "beta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
+              "gamma_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32), "delta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
+              "gamma_abc_g1": np.zeros(n_abc * self.g1_bytes // 4, dtype=np.uint32)}
+        pk, m = c_void_p(), c_void_p()
+        self._ck(self.lib.b2s_zkey_load(self.h, buf.ctypes.data, buf.nbytes, int(validate), ctypes.byref(pk), ctypes.byref(m),
+                                        vk["alpha_g1"].ctypes.data, vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data,
+                                        vk["delta_g2"].ctypes.data, vk["gamma_abc_g1"].ctypes.data, n_abc))
+        self._r1cs_vars[m.value] = info["n_vars"]
+        return pk, m, vk
+
+    def wtns_read(self, data, n_vars, out=None):
+        """A circom .wtns -> z = instance || witness, n_vars Montgomery Fr: a new uint32 numpy array, or written into `out`
+        (a host numpy array, or a CUDA torch tensor / device address, e.g. one row of a prove_batch z) and returned."""
+        buf = self._file_bytes(data)
+        if out is None:
+            out = np.zeros(n_vars * self.fr_bytes // 4, dtype=np.uint32)
+        po, mem = _ptr(out)
+        self._ck(self.lib.b2s_wtns_read(self.h, buf.ctypes.data, buf.nbytes, n_vars, mem, po))
+        return out
 
     # ---- verification (pairings in CUDA) ----------------------------------------------------------------------------
     def vk_prepare(self, vk):
