@@ -216,6 +216,10 @@ int32_t msm_run_batch(Ctx* c, int group, const void* bases_dev, const void* scal
                       bool scalars_mont, void* out_xyzz_dev, const MsmPre* pre = nullptr);
 // device bytes per vector of msm_run_batch over n points; *max_k = the most vectors its u32 indices allow
 uint64_t msm_batch_bytes(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint64_t* max_k);
+// device bytes of one msm_run over n points while it sorts, and what its batched-affine rounds add when they run in one piece
+void msm_working_set(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint64_t* sort_bytes, uint64_t* round_bytes);
+// bytes the stream-ordered pool holds but no allocation uses (free for the next allocation, not counted by cudaMemGetInfo)
+uint64_t pool_idle_bytes(Ctx* c);
 // table[w * n + i] = 2^(c w) bases[i] (affine), w < nwin; picks c / nwin for n points itself and reports them in *pre
 int32_t msm_precompute(Ctx* c, int group, const void* bases_dev, uint64_t n, void* table_dev, MsmPre* pre);
 uint32_t msm_precompute_windows(Ctx* c, uint64_t n, uint32_t* c_out);

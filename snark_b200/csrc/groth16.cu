@@ -115,18 +115,32 @@ int32_t pk_finish(Ctx* c, b2s_pk* pk) {
     const PkQuery& h = pk->q[Q_H];
     // Fixed-base window table for the h query: its scalars (the quotient polynomial) are never repeated values, so this is
     // the MSM that always pays the full Pippenger price; the other queries run over the witness, where the multiplicity-aware
-    // front end usually leaves little.  13 x the query (18 GiB at 2^24): only when it fits comfortably.
+    // front end usually leaves little.  13 x the query (20.9 GB at 2^24), built when it fits next to the proof's peak working
+    // set with a 2 GiB margin: the witness map (a, b, c, h and the NTT factor tables, 7 scalars per domain element), the sort
+    // scratch of the largest MSM, and the batched-affine rounds of the h MSM over the table in one piece.  The rounds of the
+    // other MSMs need no room here: when they do not fit beside the table they run in slices of the bucket range (msm.cu).
     {
         const char* env = getenv("B2S_PK_PRECOMP");
         const uint64_t min_n = getenv("B2S_PK_PRECOMP_MIN") ? strtoull(getenv("B2S_PK_PRECOMP_MIN"), nullptr, 10) : (1ull << 18);
         uint32_t cc = 0;
         const uint32_t nw = msm_precompute_windows(c, h.len, &cc);
-        size_t free_b = 0, total_b = 0;
-        cudaMemGetInfo(&free_b, &total_b);
         const uint64_t need = (uint64_t)nw * h.len * z.g1;
-        if (!(env && env[0] == '0') && h.len >= min_n && (uint64_t)nw * h.len < (1ull << 31) && need * 4 < (uint64_t)free_b) {
-            B2S_TRY(pk->h_table.alloc(c, need));
-            B2S_TRY(msm_precompute(c, 1, h.pts.p, h.len, pk->h_table.p, &pk->h_pre));
+        if (!(env && env[0] == '0') && h.len >= min_n && (uint64_t)nw * h.len < (1ull << 31)) {
+            const MsmPre h_shape{cc, nw, (uint32_t)h.len};
+            uint64_t sort_max = 0, rounds_h = 0;
+            for (int w = 0; w < PK_QUERIES; w++) {
+                uint64_t sort_b = 0, round_b = 0;
+                msm_working_set(c, PK_QUERY[w].group, pk->q[w].len + pk->q[w].ext, w == Q_H ? &h_shape : nullptr, &sort_b, &round_b);
+                sort_max = std::max(sort_max, sort_b);
+                if (w == Q_H) rounds_h = round_b;
+            }
+            const uint64_t working = 7 * pk->domain_size * z.fr + sort_max + rounds_h + ((uint64_t)2 << 30);
+            size_t free_b = 0, total_b = 0;
+            cudaMemGetInfo(&free_b, &total_b);
+            if (need + working <= (uint64_t)free_b + pool_idle_bytes(c)) {
+                B2S_TRY(pk->h_table.alloc(c, need));
+                B2S_TRY(msm_precompute(c, 1, h.pts.p, h.len, pk->h_table.p, &pk->h_pre));
+            }
         }
     }
     B2S_CUDA(c, cudaStreamSynchronize(c->stream));

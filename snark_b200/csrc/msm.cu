@@ -567,6 +567,15 @@ static uint32_t env_u32(const char* name, uint32_t dflt) {
     return v ? (uint32_t)strtoul(v, nullptr, 10) : dflt;
 }
 
+uint64_t pool_idle_bytes(Ctx* c) {
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, c->device) != cudaSuccess) return 0;
+    uint64_t reserved = 0, used = 0;
+    cudaMemPoolGetAttribute(pool, cudaMemPoolAttrReservedMemCurrent, &reserved);
+    cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used);
+    return reserved > used ? reserved - used : 0;
+}
+
 // Window size: minimise  n * nwin  (bucket accumulation, mixed additions)  +  nwin * 2^(c-1) * 4.7
 // (bucket reduction: two general additions per bucket at ~1.4x the cost of a mixed one, plus the
 // per-segment double-and-add), subject to the bucket array staying under 4 GiB.  A batch of K scalar vectors keeps the
@@ -612,41 +621,22 @@ static MsmShape msm_shape(uint64_t n, uint32_t scalar_bits, size_t point_bytes, 
 }
 
 // ---- bucket sums of an arbitrary bucket structure ---------------------------------------------------------------
-// How many batched-affine rounds pay for T entries in G buckets, and the XYZZ task length after them.
-struct RoundPlan { uint32_t rounds, L; uint64_t max_tasks; };
-template <class F>
-static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_t L_default) {
-    RoundPlan rp{0, L_default, T / L_default + G + 1};
-    uint32_t ba_auto = 0;
-    const uint64_t per_bucket = G ? T / G : 0;
-    while ((1ull << ba_auto) < per_bucket) ba_auto++;
-    // a round has a fixed price -- one latency-bound inversion level plus a dozen small launches -- and
-    // saves 4 (G1) / 11 (G2) base multiplications on each of its T / 2^(r+1) additions: keep the rounds that pay
-    const double min_adds = is_g1 ? 6.0e6 : 2.5e6;
-    uint32_t pays = 0;
-    while (pays < 16 && (double)(T >> (pays + 1)) > min_adds) pays++;
-    ba_auto = std::min(ba_auto, pays);
-    rp.rounds = env_u32("B2S_MSM_AFFINE_ROUNDS", ba_auto);
-    if (rp.rounds && !getenv("B2S_MSM_AFFINE_ROUNDS")) {
-        // scratch of the rounds: two output buffers, the prefix products and the lane totals (bounded by the first round)
-        const uint64_t t0 = std::min<uint64_t>(T, (T + G) / 2 + 1);
-        const uint64_t need = t0 * (sizeof(Affine<F>) * 3 / 2 + sizeof(F)) + t0 / 4;
-        // free-memory queries only when the scratch is a large part of the device (they cost milliseconds of host time with a
-        // multi-GiB pool, and this runs once per MSM): anything under a third of the device is simply allocated
-        size_t free_b = (size_t)c->total_mem, total_b = 0;
-        uint64_t pool_held = 0;
-        if (need * 3 > c->total_mem) {
-            cudaMemGetInfo(&free_b, &total_b);
-            cudaMemPool_t pool;
-            if (cudaDeviceGetDefaultMemPool(&pool, c->device) == cudaSuccess) {
-                uint64_t reserved = 0, used = 0;
-                cudaMemPoolGetAttribute(pool, cudaMemPoolAttrReservedMemCurrent, &reserved);
-                cudaMemPoolGetAttribute(pool, cudaMemPoolAttrUsedMemCurrent, &used);
-                pool_held = reserved > used ? reserved - used : 0;
-            }
-        }
-        if (need + ((uint64_t)2 << 30) > (uint64_t)free_b + pool_held) rp.rounds = 0;
-    }
+// How many batched-affine rounds pay for T entries in G buckets, in how many slices of the bucket range they run, and the
+// XYZZ task length after them.  slice_entries: the most entries one slice may hold (T when the rounds run in one piece).
+struct RoundPlan { uint32_t rounds, L; uint64_t max_tasks; uint64_t slice_entries; uint32_t L_plain; };
+
+// device bytes that the rounds and the XYZZ partials of T entries in G buckets hold at once: the two output buffers, the
+// prefix products and the lane totals (bounded by the first round), and one partial per bucket and per task (plan_tasks
+// cuts what is left after the rounds into tasks of at least 16 entries, and at most about 2^18 of them)
+static uint64_t round_scratch_bytes(uint64_t T, uint64_t G, size_t aff, size_t xyzz) {
+    const uint64_t t0 = std::min<uint64_t>(T, (T + G) / 2 + 1);
+    return t0 * (aff * 3 / 2 + aff / 2) + t0 / 4 + (G + std::min<uint64_t>(t0 / 16 + 1, 1u << 18)) * xyzz;
+}
+
+// task length and task bound of the XYZZ kernel for T entries in G buckets after rp.rounds rounds
+static void plan_tasks(RoundPlan& rp, uint64_t T, uint32_t G) {
+    rp.L = rp.L_plain;
+    rp.max_tasks = T / rp.L + G + 1;
     if (rp.rounds && !getenv("B2S_MSM_L")) {
         // what the XYZZ kernel sees after the rounds is 2^-R of the input: cut its tasks accordingly, otherwise the heavy
         // buckets of skewed scalars (a few thousand tasks of ~1000 points) leave most of the machine idle
@@ -655,15 +645,63 @@ static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_
         rp.L = (uint32_t)std::max<uint64_t>(16, t_after >> 18);
         rp.max_tasks = t_after / rp.L + G + 1;
     }
+}
+
+// held: bytes the caller allocates after this call and keeps while the rounds run (sorted indices, bucket sums)
+template <class F>
+static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_t L_default, uint64_t held = 0) {
+    RoundPlan rp{0, L_default, 0, T, L_default};
+    uint32_t ba_auto = 0;
+    const uint64_t per_bucket = G ? T / G : 0;
+    while ((1ull << ba_auto) < per_bucket) ba_auto++;
+    // a round has a fixed price -- one latency-bound inversion level plus a dozen small launches -- and
+    // saves 4 (G1) / 11 (G2) base multiplications on each of its T / 2^(r+1) additions: keep the rounds that pay.  Sliced
+    // rounds pay the fixed price once per slice, so a slice of t entries keeps the rounds that pay for t.
+    const double min_adds = is_g1 ? 6.0e6 : 2.5e6;
+    auto pays = [&](uint64_t t) {
+        uint32_t p = 0;
+        while (p < 16 && (double)(t >> (p + 1)) > min_adds) p++;
+        return std::min(ba_auto, p);
+    };
+    const bool forced = getenv("B2S_MSM_AFFINE_ROUNDS") != nullptr;
+    rp.rounds = forced ? env_u32("B2S_MSM_AFFINE_ROUNDS", 0) : pays(T);
+    // B2S_MSM_ROUND_BUDGET (bytes) replaces the free-memory budget, so that small problems can be made to slice
+    const char* budget_env = getenv("B2S_MSM_ROUND_BUDGET");
+    if (rp.rounds && (budget_env || !forced)) {
+        const uint64_t need = round_scratch_bytes(T, G, sizeof(Affine<F>), sizeof(XYZZ<F>));
+        uint64_t budget = 0;
+        if (budget_env) {
+            budget = strtoull(budget_env, nullptr, 10);
+        } else {
+            // free-memory queries only when the scratch is a large part of the device (they cost milliseconds of host time with
+            // a multi-GiB pool, and this runs once per MSM): anything under a third of the device is simply allocated
+            size_t free_b = (size_t)c->total_mem, total_b = 0;
+            uint64_t pool_held = 0;
+            if ((need + held) * 3 > c->total_mem) {
+                cudaMemGetInfo(&free_b, &total_b);
+                pool_held = pool_idle_bytes(c);
+            }
+            const uint64_t avail = (uint64_t)free_b + pool_held, reserve = held + ((uint64_t)2 << 30);
+            budget = avail > reserve ? avail - reserve : 0;
+        }
+        if (need > budget) {
+            // slices of the bucket range: the scratch grows with the entries, and the buckets of a slice in proportion
+            rp.slice_entries = (uint64_t)((double)T * ((double)budget / (double)need));
+            if (!forced && rp.slice_entries) rp.rounds = pays(T / ((T + rp.slice_entries - 1) / rp.slice_entries));
+            // a slice holds whole buckets: one that cannot hold the average bucket twice over is no slice
+            if (rp.slice_entries < 2 * std::max<uint64_t>(per_bucket, 1)) rp.rounds = 0;
+            if (!rp.rounds) rp.slice_entries = T;
+        }
+    }
+    plan_tasks(rp, T, G);
     return rp;
 }
 
-// bucket_acc[g] = sum of the points bases[sorted[offsets[g] .. offsets[g+1])] (sign in bit 31), for G buckets holding T
-// entries in all.  counts / offsets are the caller's (device); bucket_acc must be zeroed.  Rounds of batched-affine
-// halving first (msm_affine.cuh), then the XYZZ kernel, then the buckets that were cut into several tasks are joined.
+// One slice of bucket_sums_t (or all of it): G buckets holding T entries, sorted / counts / offsets / bucket_acc already
+// advanced to the slice's first bucket.  Without rounds the caller's offsets are rewritten from its counts (same values).
 template <class Curve, class F>
-static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sorted, uint32_t* counts, uint32_t* offsets, uint64_t T, uint32_t G,
-                             const RoundPlan& rp, XYZZ<F>* bucket_acc) {
+static int32_t bucket_slice_t(Ctx* c, const Affine<F>* bases, const uint32_t* sorted, uint32_t* counts, uint32_t* offsets, uint64_t T, uint32_t G,
+                              const RoundPlan& rp, XYZZ<F>* bucket_acc) {
     using Pt = XYZZ<F>;
     constexpr bool is_g1 = sizeof(F) == sizeof(typename Curve::Fq);
     MsmShape sh{};
@@ -781,6 +819,63 @@ static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sor
     return B2S_OK;
 }
 
+// bounds[k] = (g_k, offsets[g_k]) with g_k the first bucket whose entries start at or after k * T / S, k = 0 .. S
+__global__ void msm_slice_bounds_kernel(const uint32_t* __restrict__ offsets, uint32_t G, uint64_t T, uint32_t S, uint2* __restrict__ bounds) {
+    const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k > S) return;
+    const uint64_t e = T * k / S;
+    uint32_t lo = 0, hi = G;          // offsets[G] = T >= e
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (offsets[mid] < e) lo = mid + 1; else hi = mid;
+    }
+    bounds[k] = make_uint2(lo, offsets[lo]);
+}
+
+// bucket_acc[g] = sum of the points bases[sorted[offsets[g] .. offsets[g+1])] (sign in bit 31), for G buckets holding T
+// entries in all.  counts / offsets are the caller's (device); bucket_acc must be zeroed.  Rounds of batched-affine
+// halving first (msm_affine.cuh), then the XYZZ kernel, then the buckets that were cut into several tasks are joined.
+// When the rounds' scratch for all G buckets does not fit (rp.slice_entries < T), all of that runs once per slice of
+// whole buckets [g0, g1): buckets are independent and their entries contiguous in `sorted`, so a slice is a smaller
+// problem of the same kind.  The S + 1 bounds are read back once.
+template <class Curve, class F>
+static int32_t bucket_sums_t(Ctx* c, const Affine<F>* bases, const uint32_t* sorted, uint32_t* counts, uint32_t* offsets, uint64_t T, uint32_t G,
+                             const RoundPlan& rp, XYZZ<F>* bucket_acc) {
+    if (!rp.rounds || rp.slice_entries >= T) return bucket_slice_t<Curve, F>(c, bases, sorted, counts, offsets, T, G, rp, bucket_acc);
+    // even entry targets give slices of at most T / S entries plus the bucket that straddles a target; with skewed scalars
+    // that bucket may be large, so S doubles until every slice fits (or one bucket alone is over the budget)
+    std::vector<uint2> hb;
+    uint32_t S = (uint32_t)std::min<uint64_t>(G, (T + rp.slice_entries - 1) / rp.slice_entries);
+    for (int tries = 0;; tries++) {
+        DevBuf db;
+        B2S_TRY(db.alloc(c, ((size_t)S + 1) * sizeof(uint2)));
+        B2S_LAUNCH(c, msm_slice_bounds_kernel, cdiv(S + 1, 256), 256, 0, (const uint32_t*)offsets, G, T, S, db.as<uint2>());
+        hb.resize((size_t)S + 1);
+        B2S_CUDA(c, cudaMemcpyAsync(hb.data(), db.p, hb.size() * sizeof(uint2), cudaMemcpyDeviceToHost, c->stream));
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+        uint64_t largest = 0;
+        for (uint32_t k = 0; k < S; k++) largest = std::max<uint64_t>(largest, hb[k + 1].y - hb[k].y);
+        if (largest <= rp.slice_entries) break;
+        if (tries == 3 || S >= G) {
+            // a bucket on its own exceeds the budget: no rounds at all (the XYZZ kernel needs no scratch per entry)
+            RoundPlan plain = rp;
+            plain.rounds = 0;
+            plain.slice_entries = T;
+            plan_tasks(plain, T, G);
+            return bucket_slice_t<Curve, F>(c, bases, sorted, counts, offsets, T, G, plain, bucket_acc);
+        }
+        S = std::min<uint32_t>(G, 2 * S);
+    }
+    for (uint32_t k = 0; k < S; k++) {
+        const uint32_t g0 = hb[k].x, g1 = hb[k + 1].x, e0 = hb[k].y, e1 = hb[k + 1].y;
+        if (e1 == e0) continue;       // empty buckets keep their zeroed sums
+        RoundPlan sp = rp;
+        plan_tasks(sp, e1 - e0, g1 - g0);
+        B2S_TRY((bucket_slice_t<Curve, F>(c, bases, sorted + e0, counts + g0, offsets + g0, e1 - e0, g1 - g0, sp, bucket_acc + g0)));
+    }
+    return B2S_OK;
+}
+
 // ---- the Pippenger pipeline proper ---------------------------------------------------------------------------------
 // index_map (optional): scalar i belongs to base index_map[i] (the multiplicity-aware front end hands over a compacted
 // scalar array); nullptr: base i.
@@ -800,9 +895,12 @@ static int32_t msm_core_t(Ctx* c, const Affine<F>* bases, const typename Curve::
     if ((uint64_t)K * sh.nwin * n >= (1ull << 32) || (uint64_t)K * sh.nwin * sh.B >= (1ull << 32))
         return fail(c, B2S_ERR_INVALID_ARG, "msm: vectors * n * windows exceeds 2^32");
     if (pre && (uint64_t)pre->nwin * pre->stride >= (1ull << 31)) return fail(c, B2S_ERR_INVALID_ARG, "msm: precomputed table exceeds 2^31 points");
-    const RoundPlan rp = plan_rounds<F>(c, (uint64_t)K * sh.nwin * n, sh.G, is_g1, sh.L);
-    sh.L = rp.L; sh.max_tasks = rp.max_tasks;
     const uint32_t MSM_SEG = sh.B >= (1u << 16) ? 32u : 16u;
+    // what stays allocated beside the rounds: the u32 arrays, the sorted indices, the bucket sums and the segment sums
+    const uint64_t held = (uint64_t)sh.G * (5 * sizeof(uint32_t) + sizeof(Pt)) + (uint64_t)K * sh.nwin * n * sizeof(uint32_t) +
+                          (uint64_t)K * (pre ? 1u : sh.nwin) * ((sh.B + MSM_SEG - 1) / MSM_SEG) * sizeof(Pt);
+    const RoundPlan rp = plan_rounds<F>(c, (uint64_t)K * sh.nwin * n, sh.G, is_g1, sh.L, held);
+    sh.L = rp.L; sh.max_tasks = rp.max_tasks;
     const uint32_t ntiles = (sh.G + SCAN_TILE - 1) / SCAN_TILE;
     DevBuf ibuf, sorted, bucket_acc, segs, wins, tiles;
     B2S_TRY(tiles.alloc(c, (size_t)ntiles * sizeof(Scan3)));
@@ -1205,6 +1303,18 @@ uint64_t msm_batch_bytes(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint6
     return G * (pt + 5 * sizeof(uint32_t)) + T * (sizeof(uint32_t) * 2 + sizeof(uint16_t)) + (T / 16 + G) * pt + T * (3 * fe + fe) / 2;
 }
 
+// Device bytes of one msm_run over n points beside its inputs: *sort_bytes while it sorts (u32 arrays, sorted and partitioned
+// entries, bucket and segment sums), *round_bytes more while its batched-affine rounds run in one piece.
+void msm_working_set(Ctx* c, int group, uint64_t n, const MsmPre* pre, uint64_t* sort_bytes, uint64_t* round_bytes) {
+    const Sizes z = sizes(c);
+    const size_t pt = z.xyzz(group);
+    const MsmShape sh = msm_shape(std::max<uint64_t>(n, 1), fr_bits(c), pt, pre);
+    const uint64_t T = (uint64_t)sh.nwin * n, G = sh.G;
+    const uint64_t segs = (uint64_t)(pre ? 1u : sh.nwin) * (sh.B / 16 + 1);
+    *sort_bytes = G * (5 * sizeof(uint32_t) + pt) + segs * pt + T * (2 * sizeof(uint32_t) + sizeof(uint16_t));
+    *round_bytes = round_scratch_bytes(T, G, z.aff(group), pt);
+}
+
 // ---- fixed-base window precomputation for a resident key ----------------------------------------------------------------
 // table[w * n + i] = 2^(c w) * P_i, normalised to affine: c doublings per window step, one inversion per output (a one-off at
 // key upload).  With it the digits of ALL windows of an MSM over these bases share one set of 2^(c-1) buckets: nwin times
@@ -1225,7 +1335,8 @@ __global__ void __launch_bounds__(128) msm_precompute_kernel(const Affine<F>* __
 }
 
 uint32_t msm_precompute_windows(Ctx* c, uint64_t n, uint32_t* c_out) {
-    // one bucket set whatever the number of windows: c = 20 balances n * nwin additions against 2^(c-1) buckets from 2^18 points up
+    // one bucket set whatever the number of windows: c = 20 balances n * nwin additions against 2^(c-1) buckets from 2^18
+    // points up, and beat c = 22 at 2^24 (DESIGN.md section 4)
     (void)n;
     const uint32_t bits = fr_bits(c);
     const uint32_t cc = env_u32("B2S_MSM_PRE_C", 20);
