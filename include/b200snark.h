@@ -29,8 +29,9 @@
  *   - z = instance_assignment || witness_assignment, z[0] == 1 (relations/src/sr1cs/mod.rs:199-200).
  *
  * OWNERSHIP: caller-owned buffers are only read/written during the call.  `mem` says where a buffer
- * lives: B2S_MEM_HOST (any host pointer; copied through the ctx's pinned staging) or B2S_MEM_DEVICE
- * (a device pointer on the ctx's GPU, e.g. torch tensor storage).  Handles are freed by b2s_*_free.
+ * lives: B2S_MEM_HOST (any host pointer, pageable or pinned; copied to and from device scratch with stream-ordered copies,
+ * and batches in bounded chunks) or B2S_MEM_DEVICE (a device pointer on the ctx's GPU, e.g. torch tensor storage, used
+ * in place).  Any `mem` other than B2S_MEM_DEVICE means the host.  Handles are freed by b2s_*_free.
  *
  * THREADING: one in-flight call per ctx (calls on one ctx are serialised by an internal mutex).
  * ERRORS: never unwinds (reference builds with panic=abort for FFI, Cargo.toml:33); int32 status.

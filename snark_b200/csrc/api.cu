@@ -145,15 +145,10 @@ int32_t b2s_ntt(b2s_ctx* ctx, void* data, uint32_t log_n, int32_t inverse, int32
     LOCK(ctx);
     if (!data) return fail(ctx, B2S_ERR_INVALID_ARG, "ntt: null data");
     if (log_n > 27) return fail(ctx, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "ntt: 2^%u exceeds the backend limit 2^27", log_n);
-    const size_t bytes = (size_t)32 << log_n;
-    if (mem == B2S_MEM_DEVICE) return ntt_run(ctx, data, log_n, inverse != 0, coset != 0);
-    DevBuf d;
-    B2S_TRY(d.alloc(ctx, bytes));
-    B2S_CUDA(ctx, cudaMemcpyAsync(d.p, data, bytes, cudaMemcpyHostToDevice, ctx->stream));
-    B2S_TRY(ntt_run(ctx, d.p, log_n, inverse != 0, coset != 0));
-    B2S_CUDA(ctx, cudaMemcpyAsync(data, d.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    OutBuf d;
+    B2S_TRY(d.bind(ctx, data, (size_t)32 << log_n, mem, true));
+    B2S_TRY(ntt_run(ctx, d.dptr, log_n, inverse != 0, coset != 0));
+    return d.finish(ctx);
 }
 
 // ---- MSM ----------------------------------------------------------------------------------------
@@ -166,18 +161,13 @@ static int32_t msm_common(b2s_ctx* ctx, int group, const void* bases, const void
     InBuf b, s;
     B2S_TRY(b.bind(ctx, bases, n * pt, mem));
     B2S_TRY(s.bind(ctx, scalars, n * 32, mem));
-    DevBuf res, aff;
-    B2S_TRY(res.alloc(ctx, xyzz));
-    B2S_TRY(msm_run(ctx, group, b.dptr, s.dptr, n, mont != 0, res.p));
-    if (affine) {
-        B2S_TRY(aff.alloc(ctx, pt));
-        B2S_TRY(group_sum_to_affine(ctx, group, res.p, 1, aff.p));
-        B2S_CUDA(ctx, cudaMemcpyAsync(out, aff.p, pt, cudaMemcpyDeviceToHost, ctx->stream));
-    } else {
-        B2S_CUDA(ctx, cudaMemcpyAsync(out, res.p, xyzz, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    OutBuf o;   // the result goes to the host whatever `mem` says
+    DevBuf res;
+    B2S_TRY(o.bind(ctx, out, affine ? pt : xyzz, B2S_MEM_HOST));
+    if (affine) B2S_TRY(res.alloc(ctx, xyzz));
+    B2S_TRY(msm_run(ctx, group, b.dptr, s.dptr, n, mont != 0, affine ? res.p : o.dptr));
+    if (affine) B2S_TRY(group_sum_to_affine(ctx, group, res.p, 1, o.dptr));
+    return o.finish(ctx);
 }
 
 int32_t b2s_msm_g1(b2s_ctx* ctx, const void* bases, const void* scalars, uint64_t n, int32_t scalars_mont, int32_t mem,
@@ -205,13 +195,11 @@ static int32_t sum_common(b2s_ctx* ctx, int group, const void* xyzz, uint32_t co
     if (!xyzz || !out_affine || count == 0) return fail(ctx, B2S_ERR_INVALID_ARG, "group sum: bad arguments");
     const Sizes z = sizes(ctx);
     InBuf in;
+    OutBuf aff;
     B2S_TRY(in.bind(ctx, xyzz, (size_t)count * z.xyzz(group), B2S_MEM_HOST));
-    DevBuf aff;
-    B2S_TRY(aff.alloc(ctx, z.aff(group)));
-    B2S_TRY(group_sum_to_affine(ctx, group, in.dptr, count, aff.p));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_affine, aff.p, z.aff(group), cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    B2S_TRY(aff.bind(ctx, out_affine, z.aff(group), B2S_MEM_HOST));
+    B2S_TRY(group_sum_to_affine(ctx, group, in.dptr, count, aff.dptr));
+    return aff.finish(ctx);
 }
 int32_t b2s_g1_sum(b2s_ctx* ctx, const void* xyzz, uint32_t count, void* out_affine) {
     LOCK(ctx);
@@ -255,14 +243,11 @@ static int32_t fixed_base_common(b2s_ctx* ctx, int group, const void* scalars, u
     if ((!scalars || !out) && n) return fail(ctx, B2S_ERR_INVALID_ARG, "fixed_base: null buffer");
     const size_t pt = sizes(ctx).aff(group);
     InBuf s;
+    OutBuf o;
     B2S_TRY(s.bind(ctx, scalars, n * 32, mem));
-    if (mem == B2S_MEM_DEVICE) return fixed_base_run(ctx, group, s.dptr, n, mont != 0, out);
-    DevBuf o;
-    B2S_TRY(o.alloc(ctx, n * pt));
-    B2S_TRY(fixed_base_run(ctx, group, s.dptr, n, mont != 0, o.p));
-    if (n) B2S_CUDA(ctx, cudaMemcpyAsync(out, o.p, n * pt, cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    B2S_TRY(o.bind(ctx, out, n * pt, mem));
+    B2S_TRY(fixed_base_run(ctx, group, s.dptr, n, mont != 0, o.dptr));
+    return o.finish(ctx);
 }
 int32_t b2s_fixed_base_g1(b2s_ctx* ctx, const void* scalars, uint64_t n, int32_t scalars_mont, int32_t mem, void* out) {
     LOCK(ctx);
@@ -360,20 +345,16 @@ int32_t b2s_spmv(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, vo
     if (!m) return fail(ctx, B2S_ERR_MISSING_CS, "spmv: null matrices");
     if (!z || !out_a || !out_b || !out_c) return fail(ctx, B2S_ERR_INVALID_ARG, "spmv: null buffer");
     const size_t nz = (m->n_instance + m->n_witness) * 32, no = m->n_rows * 32;
-    if (mem == B2S_MEM_DEVICE) return spmv_run(ctx, m, z, out_a, out_b, out_c);
     InBuf zi;
+    OutBuf a, b, c;
     B2S_TRY(zi.bind(ctx, z, nz, mem));
-    DevBuf o;
-    B2S_TRY(o.alloc(ctx, 3 * no));
-    char* p = o.as<char>();
-    B2S_TRY(spmv_run(ctx, m, zi.dptr, p, p + no, p + 2 * no));
-    if (no) {
-        B2S_CUDA(ctx, cudaMemcpyAsync(out_a, p, no, cudaMemcpyDeviceToHost, ctx->stream));
-        B2S_CUDA(ctx, cudaMemcpyAsync(out_b, p + no, no, cudaMemcpyDeviceToHost, ctx->stream));
-        B2S_CUDA(ctx, cudaMemcpyAsync(out_c, p + 2 * no, no, cudaMemcpyDeviceToHost, ctx->stream));
-    }
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    B2S_TRY(a.bind(ctx, out_a, no, mem));
+    B2S_TRY(b.bind(ctx, out_b, no, mem));
+    B2S_TRY(c.bind(ctx, out_c, no, mem));
+    B2S_TRY(spmv_run(ctx, m, zi.dptr, a.dptr, b.dptr, c.dptr));
+    B2S_TRY(a.copy_back(ctx));
+    B2S_TRY(b.copy_back(ctx));
+    return c.finish(ctx);
 }
 
 static int32_t witness_map_common(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, int32_t qap, void* out_h) {
@@ -381,15 +362,12 @@ static int32_t witness_map_common(b2s_ctx* ctx, const b2s_r1cs* m, const void* z
     if (!z || !out_h) return fail(ctx, B2S_ERR_INVALID_ARG, "witness_map: null buffer");
     B2S_TRY(check_qap(ctx, qap, "witness_map"));
     const size_t nz = (m->n_instance + m->n_witness) * 32, nh = (size_t)32 << m->log_domain;
-    if (mem == B2S_MEM_DEVICE) return witness_map_run(ctx, m, z, out_h, qap);
     InBuf zi;
+    OutBuf h;
     B2S_TRY(zi.bind(ctx, z, nz, mem));
-    DevBuf h;
-    B2S_TRY(h.alloc(ctx, nh));
-    B2S_TRY(witness_map_run(ctx, m, zi.dptr, h.p, qap));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_h, h.p, nh, cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    B2S_TRY(h.bind(ctx, out_h, nh, mem));
+    B2S_TRY(witness_map_run(ctx, m, zi.dptr, h.dptr, qap));
+    return h.finish(ctx);
 }
 
 int32_t b2s_witness_map(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int32_t mem, void* out_h) {
@@ -409,15 +387,12 @@ int32_t b2s_witness_map_sim(b2s_ctx* ctx, const b2s_r1cs* m, const void* z, int3
     if (!dist_supported(m->log_domain, log_ranks))
         return fail(ctx, B2S_ERR_INVALID_ARG, "witness_map_sim: domain 2^%u cannot be cut over 2^%u ranks", m->log_domain, log_ranks);
     const size_t nz = (m->n_instance + m->n_witness) * 32, nh = (size_t)32 << m->log_domain;
-    if (mem == B2S_MEM_DEVICE) return witness_map_sim(ctx, m, z, log_ranks, out_h);
     InBuf zi;
+    OutBuf h;
     B2S_TRY(zi.bind(ctx, z, nz, mem));
-    DevBuf h;
-    B2S_TRY(h.alloc(ctx, nh));
-    B2S_TRY(witness_map_sim(ctx, m, zi.dptr, log_ranks, h.p));
-    B2S_CUDA(ctx, cudaMemcpyAsync(out_h, h.p, nh, cudaMemcpyDeviceToHost, ctx->stream));
-    B2S_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    return B2S_OK;
+    B2S_TRY(h.bind(ctx, out_h, nh, mem));
+    B2S_TRY(witness_map_sim(ctx, m, zi.dptr, log_ranks, h.dptr));
+    return h.finish(ctx);
 }
 
 int32_t b2s_gr1cs_upload(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_desc* preds,

@@ -7,6 +7,7 @@
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -133,12 +134,17 @@ struct DevBuf {
     T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// Where a caller buffer lives (`mem` of the C ABI): B2S_MEM_DEVICE is the ctx's GPU, any other value the host.
+inline bool on_host(int32_t mem) { return mem != B2S_MEM_DEVICE; }
+// the copy kind that brings a caller buffer in `mem` to the device
+inline cudaMemcpyKind to_device(int32_t mem) { return on_host(mem) ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice; }
+
 // Bring a caller buffer onto the device (copy if it lives on the host, alias if already there).
 struct InBuf {
     DevBuf own;
     const void* dptr = nullptr;
     int32_t bind(Ctx* c, const void* src, size_t bytes, int32_t mem) {
-        if (mem == B2S_MEM_DEVICE) { dptr = src; return B2S_OK; }
+        if (!on_host(mem)) { dptr = src; return B2S_OK; }
         B2S_TRY(own.alloc(c, bytes));
         if (bytes) B2S_CUDA(c, cudaMemcpyAsync(own.p, src, bytes, cudaMemcpyHostToDevice, c->stream));
         dptr = own.p;
@@ -146,6 +152,102 @@ struct InBuf {
     }
     template <class T>
     const T* as() const { return reinterpret_cast<const T*>(dptr); }
+};
+
+// A caller buffer the call writes, or with `in` reads and rewrites in place.  Device: dptr is the caller's pointer and
+// finish() does nothing.  Host: dptr is stream-ordered scratch (with `in`, filled from the caller); finish() copies it to
+// the caller and synchronises the stream, and copy_back() only queues the copy.
+struct OutBuf {
+    DevBuf own;
+    void* dst = nullptr;
+    void* dptr = nullptr;
+    bool host = false;
+    int32_t bind(Ctx* c, void* out, size_t bytes, int32_t mem, bool in = false) {
+        dst = dptr = out;
+        host = on_host(mem);
+        if (!host) return B2S_OK;
+        B2S_TRY(own.alloc(c, bytes));
+        if (in && bytes) B2S_CUDA(c, cudaMemcpyAsync(own.p, out, bytes, cudaMemcpyHostToDevice, c->stream));
+        dptr = own.p;
+        return B2S_OK;
+    }
+    int32_t copy_back(Ctx* c) {
+        if (host && own.bytes) B2S_CUDA(c, cudaMemcpyAsync(dst, own.p, own.bytes, cudaMemcpyDeviceToHost, c->stream));
+        return B2S_OK;
+    }
+    int32_t finish(Ctx* c) {
+        B2S_TRY(copy_back(c));
+        if (host) B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+        return B2S_OK;
+    }
+    template <class T>
+    T* as() const { return reinterpret_cast<T*>(dptr); }
+};
+
+// One caller column of a batch: `bytes` per row, read by the work (`in`) or written by it (`out`).  A column with a null
+// pointer or no bytes is absent: its device pointer is null and it takes no scratch.
+struct Col {
+    const void* in;
+    void* out;
+    size_t bytes;
+};
+inline Col col_in(const void* p, size_t bytes) { return {p, nullptr, bytes}; }
+inline Col col_out(void* p, size_t bytes) { return {nullptr, p, bytes}; }
+
+// The caller columns of a batch of rows, brought to the device one chunk at a time; the caller picks the chunk size.
+// Device (staged == false): the pointers of chunk [base, base + m) are the caller's, `base` rows in, and row_bytes() is 0.
+// Host: alloc(ch) takes one scratch allocation of ch * row_bytes() for chunks of up to ch rows, load(base, m) copies the
+// chunk's rows of every input column into it, store() copies the output columns' rows back to the caller, one copy per
+// column.  Copies are queued on the ctx stream; nothing synchronises.  Per-row scratch that is not a caller column is the
+// caller's own.
+struct RowStager {
+    static constexpr int MAX_COLS = 5;
+    Ctx* c;
+    const bool staged;
+    int n = 0;
+    Col col[MAX_COLS];
+    char* dev[MAX_COLS] = {};
+    DevBuf scratch;
+    uint64_t ch = 0, base = 0;
+    uint32_t m = 0;
+    RowStager(Ctx* ctx, int32_t mem, std::initializer_list<Col> cols) : c(ctx), staged(on_host(mem)) {
+        for (const Col& k : cols) col[n++] = k;
+    }
+    static bool present(const Col& k) { return (k.in || k.out) && k.bytes; }
+    size_t row_bytes() const {
+        size_t r = 0;
+        for (int k = 0; k < n; k++)
+            if (staged && present(col[k])) r += col[k].bytes;
+        return r;
+    }
+    int32_t alloc(uint64_t rows) {
+        ch = rows;
+        return scratch.alloc(c, ch * row_bytes());
+    }
+    int32_t load(uint64_t b, uint32_t rows) {
+        base = b;
+        m = rows;
+        char* s = scratch.as<char>();
+        for (int k = 0; k < n; k++) {
+            const Col& q = col[k];
+            if (!present(q)) { dev[k] = nullptr; continue; }
+            const char* caller = static_cast<const char*>(q.in ? q.in : q.out) + base * q.bytes;
+            if (!staged) { dev[k] = const_cast<char*>(caller); continue; }
+            dev[k] = s;
+            s += ch * q.bytes;
+            if (q.in) B2S_CUDA(c, cudaMemcpyAsync(dev[k], caller, m * q.bytes, cudaMemcpyHostToDevice, c->stream));
+        }
+        return B2S_OK;
+    }
+    int32_t store() {
+        for (int k = 0; k < n; k++)
+            if (staged && present(col[k]) && col[k].out)
+                B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(col[k].out) + base * col[k].bytes, dev[k], m * col[k].bytes,
+                                            cudaMemcpyDeviceToHost, c->stream));
+        return B2S_OK;
+    }
+    template <class T = char>
+    T* ptr(int k) const { return reinterpret_cast<T*>(dev[k]); }
 };
 
 // Kernels that need more than 48 KiB of dynamic shared memory: the attribute is per device, so it is (re)applied

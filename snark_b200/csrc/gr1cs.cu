@@ -119,34 +119,21 @@ int32_t check_t(Ctx* c, const std::vector<PredView>& views, const void* pool, ui
     if (n_assign == 0) return B2S_OK;
     const uint64_t P = views.size(), row_bytes = n_vars * sizeof(Fr);
     if (P == 0) return B2S_OK;
-    const bool host = mem != B2S_MEM_DEVICE;
+    const size_t out_row = P * sizeof(uint64_t);
+    RowStager io(c, mem, {col_in(z, row_bytes), col_out(first, out_row), col_out(count, out_row)});
+    // host: the z rows and the outputs of a chunk each within the scratch bound; scratch stands in for a null count
     uint64_t ch = std::min(CHECK_MAX_ASSIGN, n_assign);
-    if (host) ch = std::min(ch, std::max<uint64_t>(1, CHECK_SCRATCH_BYTES / row_bytes));
-    if (host || !count) ch = std::min(ch, std::max<uint64_t>(1, CHECK_SCRATCH_BYTES / (2 * sizeof(uint64_t) * P)));
-    // host: a chunk's z rows, and its outputs as [first | count] for one read-back; device: the caller's arrays take the outputs
-    // directly, scratch stands in for a null count
-    DevBuf zb, ob;
-    if (host) {
-        B2S_TRY(zb.alloc(c, ch * row_bytes));
-        B2S_TRY(ob.alloc(c, 2 * ch * P * sizeof(uint64_t)));
-    } else if (!count) {
-        B2S_TRY(ob.alloc(c, ch * P * sizeof(uint64_t)));
-    }
-    std::vector<uint64_t> hb(host ? 2 * ch * P : 0);
+    if (io.staged) ch = std::min(ch, std::max<uint64_t>(1, CHECK_SCRATCH_BYTES / row_bytes));
+    if (io.staged || !count) ch = std::min(ch, std::max<uint64_t>(1, CHECK_SCRATCH_BYTES / (2 * out_row)));
+    B2S_TRY(io.alloc(ch));
+    DevBuf ob;
+    if (!count) B2S_TRY(ob.alloc(c, ch * out_row));
     for (uint64_t a0 = 0; a0 < n_assign; a0 += ch) {
         const uint64_t K = std::min(ch, n_assign - a0), n_out = K * P;
-        const Fr* zc;
-        uint64_t *fo, *co;
-        if (host) {
-            B2S_CUDA(c, cudaMemcpyAsync(zb.p, static_cast<const char*>(z) + a0 * row_bytes, K * row_bytes, cudaMemcpyHostToDevice, c->stream));
-            zc = zb.as<Fr>();
-            fo = ob.as<uint64_t>();
-            co = fo + n_out;
-        } else {
-            zc = static_cast<const Fr*>(z) + a0 * n_vars;
-            fo = first + a0 * P;
-            co = count ? count + a0 * P : ob.as<uint64_t>();
-        }
+        B2S_TRY(io.load(a0, (uint32_t)K));
+        const Fr* zc = io.ptr<const Fr>(0);
+        uint64_t* fo = io.ptr<uint64_t>(1);
+        uint64_t* co = count ? io.ptr<uint64_t>(2) : ob.as<uint64_t>();
         B2S_CUDA(c, cudaMemsetAsync(fo, 0xFF, n_out * sizeof(uint64_t), c->stream));
         B2S_CUDA(c, cudaMemsetAsync(co, 0, n_out * sizeof(uint64_t), c->stream));
         for (uint64_t p = 0; p < P; p++) {
@@ -155,12 +142,7 @@ int32_t check_t(Ctx* c, const std::vector<PredView>& views, const void* pool, ui
                        reinterpret_cast<const Fr*>(pool), zc, n_vars, reinterpret_cast<unsigned long long*>(fo + p),
                        reinterpret_cast<unsigned long long*>(co + p), (uint32_t)P);
         }
-        if (host) {
-            B2S_CUDA(c, cudaMemcpyAsync(hb.data(), fo, 2 * n_out * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
-            B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-            std::copy(hb.begin(), hb.begin() + n_out, first + a0 * P);
-            if (count) std::copy(hb.begin() + n_out, hb.begin() + 2 * n_out, count + a0 * P);
-        }
+        B2S_TRY(io.store());
     }
     B2S_CUDA(c, cudaStreamSynchronize(c->stream));
     return B2S_OK;

@@ -169,7 +169,7 @@ int32_t pk_upload(Ctx* c, const b2s_pk_desc* d, int32_t mem, int32_t qap, b2s_pk
     b2s_pk* pk = new b2s_pk();
     pk->n_instance = d->n_instance; pk->n_witness = d->n_witness; pk->domain_size = d->domain_size; pk->qap = qap;
     for (int w = 0; w < PK_QUERIES; w++) { pk->q[w].off = src[w].off; pk->q[w].len = src[w].len; }
-    const cudaMemcpyKind kind = mem == B2S_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const cudaMemcpyKind kind = to_device(mem);
     auto body = [&]() -> int32_t {
         const size_t g1 = z.g1, g2 = z.g2;
         B2S_TRY(pk->consts_g1.alloc(c, 3 * g1));
@@ -323,13 +323,13 @@ static int32_t prove_batch_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, uint64
     B2S_CUDA(c, cudaMemGetInfo(&free_b, &total_b));
     max_k = std::max<uint64_t>(1, std::min<uint64_t>(max_k, free_b / 2 / per_proof));
     const uint32_t ch = (uint32_t)std::min<uint64_t>(max_k, n_proofs);
-    const bool host = mem != B2S_MEM_DEVICE;
-    const cudaMemcpyKind kind = host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-    DevBuf zb, h, sums1, sums2, outs;
+    const cudaMemcpyKind kind = to_device(mem);
+    DevBuf zb, h, sums1, sums2;
     B2S_TRY(zb.alloc(c, (size_t)ch * row * sizeof(Fr)));
     B2S_TRY(sums1.alloc(c, (size_t)4 * ch * sizeof(P1)));
     B2S_TRY(sums2.alloc(c, (size_t)ch * sizeof(P2)));
-    if (host) B2S_TRY(outs.alloc(c, (size_t)ch * (2 * sizeof(A1) + sizeof(A2))));
+    RowStager outs(c, mem, {col_out(out_a, sizeof(A1)), col_out(out_b, sizeof(A2)), col_out(out_c, sizeof(A1))});
+    B2S_TRY(outs.alloc(ch));
     Fr* zd = zb.as<Fr>();
     const size_t fr = sizeof(Fr);
     for (uint64_t p0 = 0; p0 < n_proofs; p0 += ch) {
@@ -355,17 +355,11 @@ static int32_t prove_batch_t(Ctx* c, const b2s_pk* pk, const b2s_r1cs* m, uint64
             else B2S_TRY(msm(Q_H, g1, hs, N));
             h.release();
         }
-        char* oa = host ? outs.as<char>() : static_cast<char*>(out_a) + p0 * sizeof(A1);
-        char* oc = host ? outs.as<char>() + (size_t)K * sizeof(A1) : static_cast<char*>(out_c) + p0 * sizeof(A1);
-        char* ob = host ? outs.as<char>() + (size_t)2 * K * sizeof(A1) : static_cast<char*>(out_b) + p0 * sizeof(A2);
+        B2S_TRY(outs.load(p0, K));
         B2S_LAUNCH(c, groth16_epilogue_g1_kernel<Curve>, K, 128, 0, pk->consts_g1.as<A1>(), (const P1*)g1, (const Fr*)(zd + n_vars), row,
-                   reinterpret_cast<A1*>(oa), reinterpret_cast<A1*>(oc));
-        B2S_LAUNCH(c, groth16_epilogue_g2_kernel<Curve>, K, 32, 0, pk->consts_g2.as<A2>(), sums2.as<P2>(), reinterpret_cast<A2*>(ob));
-        if (host) {
-            B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(out_a) + p0 * sizeof(A1), oa, K * sizeof(A1), cudaMemcpyDeviceToHost, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(out_c) + p0 * sizeof(A1), oc, K * sizeof(A1), cudaMemcpyDeviceToHost, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync(static_cast<char*>(out_b) + p0 * sizeof(A2), ob, K * sizeof(A2), cudaMemcpyDeviceToHost, c->stream));
-        }
+                   outs.ptr<A1>(0), outs.ptr<A1>(2));
+        B2S_LAUNCH(c, groth16_epilogue_g2_kernel<Curve>, K, 32, 0, pk->consts_g2.as<A2>(), sums2.as<P2>(), outs.ptr<A2>(1));
+        B2S_TRY(outs.store());
     }
     B2S_CUDA(c, cudaStreamSynchronize(c->stream));
     return B2S_OK;

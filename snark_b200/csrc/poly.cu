@@ -144,20 +144,16 @@ static int32_t poly_op_t(Ctx* c, int op, const void* a, const void* b, const voi
     InBuf A, B;
     B2S_TRY(A.bind(c, a, n * sizeof(Fr), mem));
     if (two) B2S_TRY(B.bind(c, b, n * sizeof(Fr), mem));
-    DevBuf O;
-    Fr* o = reinterpret_cast<Fr*>(out);
-    if (mem != B2S_MEM_DEVICE) { B2S_TRY(O.alloc(c, n * sizeof(Fr))); o = O.as<Fr>(); }
+    OutBuf O;
+    B2S_TRY(O.bind(c, out, n * sizeof(Fr), mem));
+    Fr* o = O.as<Fr>();
     if (op == 5) {
         if (o == A.as<Fr>()) return fail(c, B2S_ERR_INVALID_ARG, "poly_op: the batched inversion does not run in place");
         B2S_LAUNCH(c, poly_inv0_kernel<Fr>, cdiv(cdiv(n, INV_RUN), 128), 128, 0, A.as<Fr>(), o, n);
     } else {
         B2S_LAUNCH(c, poly_op_kernel<Fr>, cdiv(n, 256), 256, 0, op, A.as<Fr>(), two ? B.as<Fr>() : A.as<Fr>(), host_scalar<Fr>(s_host), o, n);
     }
-    if (mem != B2S_MEM_DEVICE) {
-        B2S_CUDA(c, cudaMemcpyAsync(out, o, n * sizeof(Fr), cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-    }
-    return B2S_OK;
+    return O.finish(c);
 }
 
 int32_t poly_op_run(Ctx* c, int op, const void* a, const void* b, const void* s_host, void* out, uint64_t n, int32_t mem) {
@@ -170,15 +166,10 @@ static int32_t poly_geom_t(Ctx* c, const void* c_host, const void* s_host, uint6
     using Fr = typename Curve::Fr;
     if (n == 0) return B2S_OK;
     if (!c_host || !s_host || !out) return fail(c, B2S_ERR_INVALID_ARG, "poly_geom: null argument");
-    DevBuf O;
-    Fr* o = reinterpret_cast<Fr*>(out);
-    if (mem != B2S_MEM_DEVICE) { B2S_TRY(O.alloc(c, n * sizeof(Fr))); o = O.as<Fr>(); }
-    B2S_LAUNCH(c, poly_geom_kernel<Fr>, cdiv(cdiv(n, GEOM_RUN), 128), 128, 0, host_scalar<Fr>(c_host), host_scalar<Fr>(s_host), o, n);
-    if (mem != B2S_MEM_DEVICE) {
-        B2S_CUDA(c, cudaMemcpyAsync(out, o, n * sizeof(Fr), cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-    }
-    return B2S_OK;
+    OutBuf O;
+    B2S_TRY(O.bind(c, out, n * sizeof(Fr), mem));
+    B2S_LAUNCH(c, poly_geom_kernel<Fr>, cdiv(cdiv(n, GEOM_RUN), 128), 128, 0, host_scalar<Fr>(c_host), host_scalar<Fr>(s_host), O.as<Fr>(), n);
+    return O.finish(c);
 }
 
 int32_t poly_geom_run(Ctx* c, const void* c_host, const void* s_host, uint64_t n, int32_t mem, void* out) {

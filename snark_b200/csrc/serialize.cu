@@ -88,17 +88,15 @@ int32_t serialize_points_ex(Ctx* c, int group, const void* affine, int32_t mem, 
     const size_t in_bytes = z.aff(group), out_bytes = z.enc(group, compressed);
     if (count * out_bytes > cap) return fail(c, B2S_ERR_INVALID_ARG, "serialize: output buffer too small");
     const uint64_t CH = 1u << 18;
-    DevBuf d, stage;
+    DevBuf d;
+    RowStager io(c, mem, {col_in(affine, in_bytes)});
     B2S_TRY(d.alloc(c, (size_t)std::min<uint64_t>(count, CH) * sizeof(CanonPoint)));
-    if (mem != B2S_MEM_DEVICE && count) B2S_TRY(stage.alloc(c, (size_t)std::min<uint64_t>(count, CH) * in_bytes));
+    B2S_TRY(io.alloc(std::min<uint64_t>(count, CH)));
     std::vector<CanonPoint> h((size_t)std::min<uint64_t>(count, CH));
     for (uint64_t base = 0; base < count; base += CH) {
         const uint32_t n = (uint32_t)std::min<uint64_t>(CH, count - base);
-        const char* src = reinterpret_cast<const char*>(affine) + base * in_bytes;
-        if (mem != B2S_MEM_DEVICE) {
-            B2S_CUDA(c, cudaMemcpyAsync(stage.p, src, (size_t)n * in_bytes, cudaMemcpyHostToDevice, c->stream));
-            src = stage.as<char>();
-        }
+        B2S_TRY(io.load(base, n));
+        const char* src = io.ptr(0);
         int32_t st = dispatch_curve(c, [&](auto curve) {
             using C = decltype(curve);
             if (group == 1) B2S_LAUNCH(c, canon_points_kernel<typename C::Fq>, cdiv(n, 64), 64, 0, reinterpret_cast<const Affine<typename C::Fq>*>(src), n, d.as<CanonPoint>());

@@ -131,50 +131,29 @@ int32_t groth16_verify_batch(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void*
                     (unsigned long long)(pvk->n_abc - 1));
     if (n == 0) return B2S_OK;
     if (!a || !b || !cc || !ok || (ni && !inputs)) return fail(c, B2S_ERR_INVALID_ARG, "verify_batch: null buffer");
-    const bool host = mem != B2S_MEM_DEVICE;
     return dispatch_curve(c, [&](auto curve) -> int32_t {
         using C = decltype(curve);
         using F12 = Fp12<typename C::FqP>;
-        const size_t g1 = sizeof(typename C::G1Affine), g2 = sizeof(typename C::G2Affine), fr = sizeof(typename C::Fr);
-        const size_t in_row = ni * fr, f12 = sizeof(F12);
-        const size_t per_proof = g1 + f12 + (host ? in_row + 2 * g1 + g2 + 1 : 0);
-        const uint64_t ch = chunk_size(n, per_proof);
+        using G1A = typename C::G1Affine;
+        const size_t g1 = sizeof(G1A), g2 = sizeof(typename C::G2Affine), f12 = sizeof(F12);
+        RowStager io(c, mem, {col_in(inputs, ni * sizeof(typename C::Fr)), col_in(a, g1), col_in(b, g2), col_in(cc, g1), col_out(ok, 1)});
+        const uint64_t ch = chunk_size(n, g1 + f12 + io.row_bytes());
         DevBuf scratch;
-        B2S_TRY(scratch.alloc(c, ch * per_proof));
-        char* sp = scratch.as<char>();
-        auto* ic = reinterpret_cast<typename C::G1Affine*>(sp);
-        auto* f = reinterpret_cast<F12*>(sp + ch * g1);
-        char* stage = sp + ch * (g1 + f12);   // host mode: inputs, a, b, c, ok
+        B2S_TRY(scratch.alloc(c, ch * (g1 + f12)));
+        auto* ic = scratch.as<G1A>();
+        auto* f = reinterpret_cast<F12*>(scratch.as<char>() + ch * g1);
+        B2S_TRY(io.alloc(ch));
         for (uint64_t base = 0; base < n; base += ch) {
             const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
-            const char *xi, *ai, *bi, *ci;
-            uint8_t* oki;
-            if (host) {
-                char* q = stage;
-                xi = q; q += ch * in_row;
-                ai = q; q += ch * g1;
-                bi = q; q += ch * g2;
-                ci = q; q += ch * g1;
-                oki = reinterpret_cast<uint8_t*>(q);
-                if (ni) B2S_CUDA(c, cudaMemcpyAsync((void*)xi, static_cast<const char*>(inputs) + base * in_row, m * in_row, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)ai, static_cast<const char*>(a) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)bi, static_cast<const char*>(b) + base * g2, m * g2, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)ci, static_cast<const char*>(cc) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-            } else {
-                xi = ni ? static_cast<const char*>(inputs) + base * in_row : nullptr;
-                ai = static_cast<const char*>(a) + base * g1;
-                bi = static_cast<const char*>(b) + base * g2;
-                ci = static_cast<const char*>(cc) + base * g1;
-                oki = ok + base;
-            }
+            B2S_TRY(io.load(base, m));
             const unsigned grid = cdiv(m, VERIFY_THREADS);
-            B2S_LAUNCH_N(c, "verify_ic", verify_ic_kernel<C>, grid, VERIFY_THREADS, 0, reinterpret_cast<const typename C::Fr*>(xi), m,
-                         (uint32_t)ni, pvk->abc0.as<typename C::G1Affine>(), pvk->table.as<typename C::G1Affine>(), ic);
-            B2S_LAUNCH_N(c, "verify_miller", verify_miller_kernel<C>, grid, VERIFY_THREADS, 0, reinterpret_cast<const typename C::G1Affine*>(ai),
-                         reinterpret_cast<const typename C::G2Affine*>(bi), ic, reinterpret_cast<const typename C::G1Affine*>(ci),
-                         pvk->prep.as<G2Prepared<C>>(), m, f);
-            B2S_LAUNCH_N(c, "verify_final_exp", final_exp_kernel<C>, grid, VERIFY_THREADS, 0, f, m, pvk->ab.as<F12>(), oki, (F12*)nullptr);
-            if (host) B2S_CUDA(c, cudaMemcpyAsync(ok + base, oki, m, cudaMemcpyDeviceToHost, c->stream));
+            B2S_LAUNCH_N(c, "verify_ic", verify_ic_kernel<C>, grid, VERIFY_THREADS, 0, io.ptr<const typename C::Fr>(0), m,
+                         (uint32_t)ni, pvk->abc0.as<G1A>(), pvk->table.as<G1A>(), ic);
+            B2S_LAUNCH_N(c, "verify_miller", verify_miller_kernel<C>, grid, VERIFY_THREADS, 0, io.ptr<const G1A>(1),
+                         io.ptr<const typename C::G2Affine>(2), ic, io.ptr<const G1A>(3), pvk->prep.as<G2Prepared<C>>(), m, f);
+            B2S_LAUNCH_N(c, "verify_final_exp", final_exp_kernel<C>, grid, VERIFY_THREADS, 0, f, m, pvk->ab.as<F12>(), io.ptr<uint8_t>(4),
+                         (F12*)nullptr);
+            B2S_TRY(io.store());
         }
         B2S_CUDA(c, cudaStreamSynchronize(c->stream));
         return (int32_t)B2S_OK;
@@ -183,37 +162,24 @@ int32_t groth16_verify_batch(Ctx* c, const b2s_pvk* pvk, uint64_t n, const void*
 
 int32_t pairing_batch(Ctx* c, const void* p, const void* q, uint64_t n, int32_t mem, void* out) {
     if (n == 0) return B2S_OK;
-    const bool host = mem != B2S_MEM_DEVICE;
     return dispatch_curve(c, [&](auto curve) -> int32_t {
         using C = decltype(curve);
         using F12 = Fp12<typename C::FqP>;
-        const size_t g1 = sizeof(typename C::G1Affine), g2 = sizeof(typename C::G2Affine), f12 = sizeof(F12);
-        const size_t per_proof = f12 + (host ? g1 + g2 + f12 : 0);
-        const uint64_t ch = chunk_size(n, per_proof);
-        DevBuf scratch;
-        B2S_TRY(scratch.alloc(c, ch * per_proof));
-        char* sp = scratch.as<char>();
-        auto* f = reinterpret_cast<F12*>(sp);
+        const size_t f12 = sizeof(F12);
+        RowStager io(c, mem, {col_in(p, sizeof(typename C::G1Affine)), col_in(q, sizeof(typename C::G2Affine)), col_out(out, f12)});
+        const uint64_t ch = chunk_size(n, f12 + io.row_bytes());
+        DevBuf f;
+        B2S_TRY(f.alloc(c, ch * f12));
+        B2S_TRY(io.alloc(ch));
         for (uint64_t base = 0; base < n; base += ch) {
             const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
-            const char *pi, *qi;
-            F12* oi;
-            if (host) {
-                char* s = sp + ch * f12;
-                pi = s; qi = s + ch * g1;
-                oi = reinterpret_cast<F12*>(s + ch * (g1 + g2));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)pi, static_cast<const char*>(p) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync((void*)qi, static_cast<const char*>(q) + base * g2, m * g2, cudaMemcpyHostToDevice, c->stream));
-            } else {
-                pi = static_cast<const char*>(p) + base * g1;
-                qi = static_cast<const char*>(q) + base * g2;
-                oi = static_cast<F12*>(out) + base;
-            }
+            B2S_TRY(io.load(base, m));
             const unsigned grid = cdiv(m, VERIFY_THREADS);
-            B2S_LAUNCH_N(c, "pairing_miller", pairing_miller_kernel<C>, grid, VERIFY_THREADS, 0, reinterpret_cast<const typename C::G1Affine*>(pi),
-                         reinterpret_cast<const typename C::G2Affine*>(qi), m, f);
-            B2S_LAUNCH_N(c, "pairing_final_exp", final_exp_kernel<C>, grid, VERIFY_THREADS, 0, f, m, (const F12*)nullptr, (uint8_t*)nullptr, oi);
-            if (host) B2S_CUDA(c, cudaMemcpyAsync(static_cast<F12*>(out) + base, oi, m * f12, cudaMemcpyDeviceToHost, c->stream));
+            B2S_LAUNCH_N(c, "pairing_miller", pairing_miller_kernel<C>, grid, VERIFY_THREADS, 0, io.ptr<const typename C::G1Affine>(0),
+                         io.ptr<const typename C::G2Affine>(1), m, f.as<F12>());
+            B2S_LAUNCH_N(c, "pairing_final_exp", final_exp_kernel<C>, grid, VERIFY_THREADS, 0, f.as<F12>(), m, (const F12*)nullptr,
+                         (uint8_t*)nullptr, io.ptr<F12>(2));
+            B2S_TRY(io.store());
         }
         B2S_CUDA(c, cudaStreamSynchronize(c->stream));
         return (int32_t)B2S_OK;

@@ -75,36 +75,27 @@ __global__ void verify_bytes_veto_kernel(const uint8_t* bad, uint8_t* ok) {
 
 namespace {
 
-// The chunk scratch both paths share: the proof bytes of host batches, the decoded points and the status bytes.
+// The chunk scratch both paths share: the decoded points and the status bytes.
 struct Decoded {
     DevBuf buf;
-    size_t pb = 0;   // bytes of one serialized proof
-    uint8_t* bytes = nullptr;
     void *a = nullptr, *b = nullptr, *c = nullptr;
     uint8_t* status = nullptr;
-    static size_t per_proof(Ctx* ctx, bool compressed, bool host) {
+    static size_t per_proof(Ctx* ctx) {
         const Sizes z = sizes(ctx);
-        return (host ? 2 * z.enc(1, compressed) + z.enc(2, compressed) : 0) + 2 * z.g1 + z.g2 + 3;
+        return 2 * z.g1 + z.g2 + 3;
     }
-    int32_t alloc(Ctx* ctx, uint64_t ch, bool compressed, bool host) {
+    int32_t alloc(Ctx* ctx, uint64_t ch) {
         const Sizes z = sizes(ctx);
-        pb = 2 * z.enc(1, compressed) + z.enc(2, compressed);
-        B2S_TRY(buf.alloc(ctx, ch * per_proof(ctx, compressed, host)));
+        B2S_TRY(buf.alloc(ctx, ch * per_proof(ctx)));
         char* q = buf.as<char>();
         a = q; q += ch * z.g1;
         b = q; q += ch * z.g2;
         c = q; q += ch * z.g1;
-        status = reinterpret_cast<uint8_t*>(q); q += ch * 3;
-        if (host) bytes = reinterpret_cast<uint8_t*>(q);
+        status = reinterpret_cast<uint8_t*>(q);
         return B2S_OK;
     }
-    // the proofs [base, base + m) -> a, b, c, status; `proofs` is HOST (copied through `bytes`) or DEVICE
-    int32_t decode(Ctx* ctx, const uint8_t* proofs, bool host, uint64_t base, uint32_t m, bool compressed) {
-        const uint8_t* in = proofs + base * pb;
-        if (host) {
-            B2S_CUDA(ctx, cudaMemcpyAsync(bytes, in, (size_t)m * pb, cudaMemcpyHostToDevice, ctx->stream));
-            in = bytes;
-        }
+    // the proof bytes of a chunk of m proofs, on the device -> a, b, c, status
+    int32_t decode(Ctx* ctx, const uint8_t* in, uint32_t m, bool compressed) {
         return dispatch_curve(ctx, [&](auto curve) -> int32_t {
             using C = decltype(curve);
             B2S_LAUNCH_N(ctx, "verify_decode_g1", verify_decode_g1_kernel<C>, cdiv(2ull * m, VERIFY_THREADS), VERIFY_THREADS, 0, in, m,
@@ -116,14 +107,19 @@ struct Decoded {
     }
 };
 
+// bytes of one serialized proof
+size_t proof_bytes(Ctx* c, bool compressed) {
+    const Sizes z = sizes(c);
+    return 2 * z.enc(1, compressed) + z.enc(2, compressed);
+}
+
 // the checks both entry points share, in the order of the points entry points; then the length of `proofs`
 int32_t check_args(Ctx* c, const char* name, const b2s_pvk* pvk, uint64_t n, uint64_t ni, uint64_t len, bool compressed) {
     if (pvk->curve != c->curve) return fail(c, B2S_ERR_INVALID_ARG, "%s: the prepared key belongs to another curve", name);
     if (ni + 1 != pvk->n_abc)
         return fail(c, B2S_ERR_MALFORMED_VK, "%s: %llu public inputs, the key expects %llu", name, (unsigned long long)ni,
                     (unsigned long long)(pvk->n_abc - 1));
-    const Sizes z = sizes(c);
-    const size_t pb = 2 * z.enc(1, compressed) + z.enc(2, compressed);
+    const size_t pb = proof_bytes(c, compressed);
     if (n > len / pb || n * pb != len)
         return fail(c, B2S_ERR_INVALID_DATA, "%s: %llu bytes are not %llu proofs of %zu bytes", name, (unsigned long long)len,
                     (unsigned long long)n, pb);
@@ -138,38 +134,20 @@ int32_t groth16_verify_batch_bytes(Ctx* c, const b2s_pvk* pvk, uint64_t n, const
     B2S_TRY(check_args(c, name, pvk, n, ni, len, compressed));
     if (n == 0) return B2S_OK;
     if (!proofs || !ok || (ni && !inputs)) return fail(c, B2S_ERR_INVALID_ARG, "%s: null buffer", name);
-    const bool host = mem != B2S_MEM_DEVICE;
-    const size_t in_row = ni * sizes(c).fr;
-    // per proof: the decode scratch, and for host batches the staged inputs, ok and reason
-    const size_t per_proof = Decoded::per_proof(c, compressed, host) + (host ? in_row + 2 : 0);
-    const uint64_t ch = chunk_size(n, per_proof);
+    RowStager io(c, mem, {col_in(inputs, ni * sizes(c).fr), col_in(proofs, proof_bytes(c, compressed)), col_out(ok, 1), col_out(reason, 1)});
+    const uint64_t ch = chunk_size(n, Decoded::per_proof(c) + io.row_bytes());
     Decoded d;
-    B2S_TRY(d.alloc(c, ch, compressed, host));
-    DevBuf stage;   // host mode: inputs, ok, reason
-    B2S_TRY(stage.alloc(c, host ? ch * (in_row + 2) : 0));
+    B2S_TRY(d.alloc(c, ch));
+    B2S_TRY(io.alloc(ch));
     for (uint64_t base = 0; base < n; base += ch) {
         const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
-        const char* xi;
-        uint8_t *oki, *rsi;
-        if (host) {
-            char* q = stage.as<char>();
-            xi = q;
-            oki = reinterpret_cast<uint8_t*>(q + ch * in_row);
-            rsi = reason ? oki + ch : nullptr;
-            if (ni) B2S_CUDA(c, cudaMemcpyAsync((void*)xi, static_cast<const char*>(inputs) + base * in_row, m * in_row, cudaMemcpyHostToDevice, c->stream));
-        } else {
-            xi = ni ? static_cast<const char*>(inputs) + base * in_row : nullptr;
-            oki = ok + base;
-            rsi = reason ? reason + base : nullptr;
-        }
-        B2S_TRY(d.decode(c, proofs, host, base, m, compressed));
-        B2S_TRY(groth16_verify_batch(c, pvk, m, xi, ni, d.a, d.b, d.c, B2S_MEM_DEVICE, oki));
+        B2S_TRY(io.load(base, m));
+        uint8_t *oki = io.ptr<uint8_t>(2), *rsi = io.ptr<uint8_t>(3);
+        B2S_TRY(d.decode(c, io.ptr<uint8_t>(1), m, compressed));
+        B2S_TRY(groth16_verify_batch(c, pvk, m, io.ptr(0), ni, d.a, d.b, d.c, B2S_MEM_DEVICE, oki));
         B2S_LAUNCH_N(c, "verify_bytes_fold", verify_bytes_fold_kernel, cdiv(m, VERIFY_THREADS), VERIFY_THREADS, 0, d.status, m, oki, rsi,
                      (uint8_t*)nullptr);
-        if (host) {
-            B2S_CUDA(c, cudaMemcpyAsync(ok + base, oki, m, cudaMemcpyDeviceToHost, c->stream));
-            if (reason) B2S_CUDA(c, cudaMemcpyAsync(reason + base, rsi, m, cudaMemcpyDeviceToHost, c->stream));
-        }
+        B2S_TRY(io.store());
     }
     B2S_CUDA(c, cudaStreamSynchronize(c->stream));
     return B2S_OK;
@@ -183,42 +161,27 @@ int32_t groth16_verify_batch_rlc_bytes(Ctx* c, const b2s_pvk* pvk, uint64_t n, c
     B2S_TRY(check_args(c, name, pvk, n, ni, len, compressed));
     if (n == 0) { *ok = 1; return B2S_OK; }
     if (!proofs || !rho || (ni && !inputs)) return fail(c, B2S_ERR_INVALID_ARG, "%s: null buffer", name);
-    const bool host = mem != B2S_MEM_DEVICE;
-    const size_t in_row = ni * sizes(c).fr;
-    // per proof: the check's own scratch, the decode scratch, and for host batches the staged inputs, rho and reason
-    const size_t stage_row = host ? in_row + RLC_RHO + (reason ? 1 : 0) : 0;
-    const uint64_t ch = chunk_size(n, rlc_per_proof(c) + Decoded::per_proof(c, compressed, host) + stage_row);
+    RowStager io(c, mem, {col_in(inputs, ni * sizes(c).fr), col_in(proofs, proof_bytes(c, compressed)), col_in(rho, RLC_RHO),
+                          col_out(reason, 1)});
+    const uint64_t ch = chunk_size(n, rlc_per_proof(c) + Decoded::per_proof(c) + io.row_bytes());
     RlcRun r;
     B2S_TRY(rlc_begin(c, pvk, ni, ch, name, r));
     Decoded d;
-    B2S_TRY(d.alloc(c, ch, compressed, host));
-    DevBuf stage;   // host mode: inputs, rho, reason; then the decode-failure flag
-    B2S_TRY(stage.alloc(c, ch * stage_row + 1));
-    uint8_t* bad = stage.as<uint8_t>() + ch * stage_row;
-    B2S_CUDA(c, cudaMemsetAsync(bad, 0, 1, c->stream));
+    B2S_TRY(d.alloc(c, ch));
+    B2S_TRY(io.alloc(ch));
+    DevBuf bad;   // the decode-failure flag
+    B2S_TRY(bad.alloc(c, 1));
+    B2S_CUDA(c, cudaMemsetAsync(bad.p, 0, 1, c->stream));
     for (uint64_t base = 0; base < n; base += ch) {
         const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
-        const char *xi, *ri;
-        uint8_t* rsi;
-        if (host) {
-            char* q = stage.as<char>();
-            xi = q; q += ch * in_row;
-            ri = q; q += ch * RLC_RHO;
-            rsi = reason ? reinterpret_cast<uint8_t*>(q) : nullptr;
-            if (ni) B2S_CUDA(c, cudaMemcpyAsync((void*)xi, static_cast<const char*>(inputs) + base * in_row, m * in_row, cudaMemcpyHostToDevice, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync((void*)ri, static_cast<const char*>(rho) + base * RLC_RHO, m * RLC_RHO, cudaMemcpyHostToDevice, c->stream));
-        } else {
-            xi = ni ? static_cast<const char*>(inputs) + base * in_row : nullptr;
-            ri = static_cast<const char*>(rho) + base * RLC_RHO;
-            rsi = reason ? reason + base : nullptr;
-        }
-        B2S_TRY(d.decode(c, proofs, host, base, m, compressed));
+        B2S_TRY(io.load(base, m));
+        B2S_TRY(d.decode(c, io.ptr<uint8_t>(1), m, compressed));
         B2S_LAUNCH_N(c, "verify_bytes_fold", verify_bytes_fold_kernel, cdiv(m, VERIFY_THREADS), VERIFY_THREADS, 0, d.status, m,
-                     (uint8_t*)nullptr, rsi, bad);
-        B2S_TRY(rlc_chunk(r, xi, d.a, d.b, d.c, ri, m, base, base + m == n));
-        if (host && reason) B2S_CUDA(c, cudaMemcpyAsync(reason + base, rsi, m, cudaMemcpyDeviceToHost, c->stream));
+                     (uint8_t*)nullptr, io.ptr<uint8_t>(3), bad.as<uint8_t>());
+        B2S_TRY(rlc_chunk(r, io.ptr(0), d.a, d.b, d.c, io.ptr(2), m, base, base + m == n));
+        B2S_TRY(io.store());
     }
-    B2S_LAUNCH_N(c, "verify_bytes_veto", verify_bytes_veto_kernel, 1, 1, 0, (const uint8_t*)bad, r.ok_dev);
+    B2S_LAUNCH_N(c, "verify_bytes_veto", verify_bytes_veto_kernel, 1, 1, 0, bad.as<const uint8_t>(), r.ok_dev);
     return rlc_read(r, ok);
 }
 

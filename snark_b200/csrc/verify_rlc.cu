@@ -226,39 +226,16 @@ int32_t groth16_verify_batch_rlc(Ctx* c, const b2s_pvk* pvk, uint64_t n, const v
     *ok = 0;
     if (n == 0) { *ok = 1; return B2S_OK; }
     if (!a || !b || !cc || !rho || (ni && !inputs)) return fail(c, B2S_ERR_INVALID_ARG, "verify_batch_rlc: null buffer");
-    const bool host = mem != B2S_MEM_DEVICE;
     const Sizes z = sizes(c);
-    const size_t g1 = z.g1, g2 = z.g2, in_row = ni * z.fr;
-    // per proof: the check's own scratch, and the staged inputs of host batches
-    const size_t stage_row = host ? in_row + 2 * g1 + g2 + RLC_RHO : 0;
-    const uint64_t ch = chunk_size(n, rlc_per_proof(c) + stage_row);
+    RowStager io(c, mem, {col_in(inputs, ni * z.fr), col_in(a, z.g1), col_in(b, z.g2), col_in(cc, z.g1), col_in(rho, RLC_RHO)});
+    const uint64_t ch = chunk_size(n, rlc_per_proof(c) + io.row_bytes());
     RlcRun r;
     B2S_TRY(rlc_begin(c, pvk, ni, ch, "verify_batch_rlc", r));
-    DevBuf stage;   // host mode: inputs, a, b, c, rho
-    B2S_TRY(stage.alloc(c, ch * stage_row));
+    B2S_TRY(io.alloc(ch));
     for (uint64_t base = 0; base < n; base += ch) {
         const uint32_t m = (uint32_t)std::min<uint64_t>(ch, n - base);
-        const char *xi, *ai, *bi, *ci, *ri;
-        if (host) {
-            char* s = stage.as<char>();
-            xi = s; s += ch * in_row;
-            ai = s; s += ch * g1;
-            bi = s; s += ch * g2;
-            ci = s; s += ch * g1;
-            ri = s;
-            if (ni) B2S_CUDA(c, cudaMemcpyAsync((void*)xi, static_cast<const char*>(inputs) + base * in_row, m * in_row, cudaMemcpyHostToDevice, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync((void*)ai, static_cast<const char*>(a) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync((void*)bi, static_cast<const char*>(b) + base * g2, m * g2, cudaMemcpyHostToDevice, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync((void*)ci, static_cast<const char*>(cc) + base * g1, m * g1, cudaMemcpyHostToDevice, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync((void*)ri, static_cast<const char*>(rho) + base * RLC_RHO, m * RLC_RHO, cudaMemcpyHostToDevice, c->stream));
-        } else {
-            xi = ni ? static_cast<const char*>(inputs) + base * in_row : nullptr;
-            ai = static_cast<const char*>(a) + base * g1;
-            bi = static_cast<const char*>(b) + base * g2;
-            ci = static_cast<const char*>(cc) + base * g1;
-            ri = static_cast<const char*>(rho) + base * RLC_RHO;
-        }
-        B2S_TRY(rlc_chunk(r, xi, ai, bi, ci, ri, m, base, base + m == n));
+        B2S_TRY(io.load(base, m));
+        B2S_TRY(rlc_chunk(r, io.ptr(0), io.ptr(1), io.ptr(2), io.ptr(3), io.ptr(4), m, base, base + m == n));
     }
     return rlc_read(r, ok);
 }

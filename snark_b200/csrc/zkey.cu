@@ -429,17 +429,13 @@ int32_t wtns_read(Ctx* c, const uint8_t* in, uint64_t len, uint64_t n_vars, int3
         return fail(c, B2S_ERR_INVALID_DATA, "wtns: data section holds %llu bytes, %llu values need %llu", (unsigned long long)s[2].size,
                     (unsigned long long)n_wit, (unsigned long long)(n_wit * FR_BYTES));
     if (n_wit == 0) return fail(c, B2S_ERR_INVALID_DATA, "wtns: no values (z[0] = 1 is required)");
-    DevBuf own;
-    void* dst = out_z;
-    if (mem != B2S_MEM_DEVICE) {
-        B2S_TRY(own.alloc(c, n_wit * FR_BYTES));
-        dst = own.p;
-    }
+    OutBuf z;
+    B2S_TRY(z.bind(c, out_z, n_wit * FR_BYTES, mem));
     Stager st(c);
     B2S_TRY(st.chunks(in + s[2].off, n_wit, FR_BYTES, [&](const uint8_t* src, uint32_t n, uint64_t base) {
         return dispatch_curve(c, [&](auto curve) {
             using C = decltype(curve);
-            B2S_LAUNCH(c, wtns_kernel<C>, cdiv(n, 256), 256, 0, src, n, base, reinterpret_cast<typename C::Fr*>(dst),
+            B2S_LAUNCH(c, wtns_kernel<C>, cdiv(n, 256), 256, 0, src, n, base, z.as<typename C::Fr>(),
                        st.err.as<unsigned long long>());
             return (int32_t)B2S_OK;
         });
@@ -448,11 +444,7 @@ int32_t wtns_read(Ctx* c, const uint8_t* in, uint64_t len, uint64_t n_vars, int3
     B2S_TRY(st.read_err(&word));
     if (word != ~0ull)
         return fail(c, B2S_ERR_INVALID_DATA, "wtns[%llu]: %s", word >> 3, (word & 7) == 1 ? "value not below r" : "z[0] is not 1");
-    if (mem != B2S_MEM_DEVICE) {
-        B2S_CUDA(c, cudaMemcpyAsync(out_z, own.p, n_wit * FR_BYTES, cudaMemcpyDeviceToHost, c->stream));
-        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-    }
-    return B2S_OK;
+    return z.finish(c);
 }
 
 }  // namespace b2s

@@ -228,6 +228,43 @@ def _ptr(x):
     return x.data_ptr(), (MEM_DEVICE if x.is_cuda else MEM_HOST)
 
 
+def _ptrs(*bufs, same=True):
+    """_ptr of several buffers -> ([addresses], the memory kind of the first).  With `same`, asserts that the buffers other
+    than None share one memory kind."""
+    got = [_ptr(x) for x in bufs]
+    assert not same or len({m for x, (_, m) in zip(bufs, got) if x is not None}) <= 1
+    return [p for p, _ in got], got[0][1]
+
+
+def _nbytes(x):
+    """byte size of a numpy array or torch tensor"""
+    return x.nbytes if isinstance(x, np.ndarray) else x.numel() * x.element_size()
+
+
+def _draw_rho(n, mem, like):
+    """random_rho(n) in `mem`: a numpy array, or an int32 tensor on the device of the tensor `like`"""
+    rho = random_rho(n)
+    if mem == MEM_DEVICE:
+        import torch
+
+        rho = torch.from_numpy(rho.view(np.int32)).to(like.device)
+    return rho
+
+
+def _zeros(shapes, dtype, mem, like):
+    """Zero-filled output arrays of one shape each: numpy `dtype` (np.uint32 / np.uint64) on the host, or torch tensors of
+    the signed type of the same width on the device of the tensor `like`.  torch's stream is synchronised after a device
+    fill, so that the zeros are in place before the library's stream writes."""
+    if mem == MEM_HOST:
+        return [np.zeros(s, dtype=dtype) for s in shapes]
+    import torch
+
+    tdtype = torch.int64 if np.dtype(dtype).itemsize == 8 else torch.int32
+    out = [torch.zeros(s, dtype=tdtype, device=like.device) for s in shapes]
+    torch.cuda.current_stream(like.device).synchronize()
+    return out
+
+
 class Backend:
     """One `b2s_ctx`: a curve bound to one GPU.  Buffers are numpy uint32/uint64 arrays (host) or
     CUDA torch tensors (device), already in the C-ABI layout (Montgomery limbs)."""
@@ -279,9 +316,7 @@ class Backend:
         return data
 
     def _msm(self, fn, out_bytes, bases, scalars, n, mont):
-        pb, mem = _ptr(bases)
-        ps, mem2 = _ptr(scalars)
-        assert n == 0 or mem == mem2
+        (pb, ps), mem = _ptrs(bases, scalars, same=n != 0)
         out = np.zeros(out_bytes // 4, dtype=np.uint32)
         self._ck(fn(self.h, pb, ps, n, int(mont), mem, out.ctypes.data))
         return out
@@ -309,13 +344,11 @@ class Backend:
         return out
 
     def fixed_base(self, group, scalars, n, mont=True, out=None):
-        ps, mem = _ptr(scalars)
         nbytes = (self.g1_bytes if group == 1 else self.g2_bytes) * n
         if out is None:
-            assert mem == MEM_HOST
+            assert _ptr(scalars)[1] == MEM_HOST
             out = np.zeros(nbytes // 4, dtype=np.uint32)
-        po, mem_o = _ptr(out)
-        assert mem_o == mem
+        (ps, po), mem = _ptrs(scalars, out)
         fn = self.lib.b2s_fixed_base_g1 if group == 1 else self.lib.b2s_fixed_base_g2
         self._ck(fn(self.h, ps, n, int(mont), mem, po))
         return out
@@ -428,15 +461,8 @@ class Backend:
             raise ValueError(f"z must be (n_assign, {8 * n_vars}) 32-bit limbs for {n_vars} variables, got shape {tuple(z.shape)}")
         pz, mem = _ptr(z)
         n = z.shape[0]
-        if mem == MEM_HOST:
-            first = np.zeros((n, n_pred), dtype=np.uint64)
-            count = np.zeros((n, n_pred), dtype=np.uint64) if counts else None
-        else:
-            import torch
-
-            first = torch.zeros((n, n_pred), dtype=torch.int64, device=z.device)
-            count = torch.zeros((n, n_pred), dtype=torch.int64, device=z.device) if counts else None
-            torch.cuda.current_stream(z.device).synchronize()
+        first, *count = _zeros([(n, n_pred)] * (2 if counts else 1), np.uint64, mem, z)
+        count = count[0] if counts else None
         self._ck(fn(self.h, handle, n, pz, mem, _ptr(first)[0], _ptr(count)[0] if counts else None))
         if mem == MEM_DEVICE:
             first = first.cpu().numpy().view(np.uint64)
@@ -479,16 +505,20 @@ class Backend:
         """trapdoor: uint32[5*8] Montgomery (tau, alpha, beta, gamma, delta) -> (pk handle, vk dict of numpy arrays).
         qap: the key's reduction (QAP_CIRCOM: the N-point circom h query)."""
         h = c_void_p()
-        vk = {"alpha_g1": np.zeros(self.g1_bytes // 4, dtype=np.uint32), "beta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
-              "gamma_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32), "delta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
-              "gamma_abc_g1": np.zeros(max(n_instance, 1) * self.g1_bytes // 4, dtype=np.uint32)}
-        outs = (vk["alpha_g1"].ctypes.data, vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data, vk["delta_g2"].ctypes.data,
-                vk["gamma_abc_g1"].ctypes.data)
+        vk = self._vk_bufs(n_instance)
+        outs = [v.ctypes.data for v in vk.values()]
         if qap == QAP_LIBSNARK:
             self._ck(self.lib.b2s_groth16_setup(self.h, m, trapdoor.ctypes.data, ctypes.byref(h), *outs))
         else:
             self._ck(self.lib.b2s_groth16_setup_qap(self.h, m, trapdoor.ctypes.data, qap, ctypes.byref(h), *outs))
         return h, vk
+
+    def _vk_bufs(self, n_abc):
+        """A zeroed verifying key: the dict of HOST arrays groth16_setup returns, with room for max(n_abc, 1) gamma_abc_g1
+        points; the values are in the order of the C ABI's vk arguments."""
+        g1, g2 = (np.zeros(n // 4, dtype=np.uint32) for n in (self.g1_bytes, self.g2_bytes))
+        return {"alpha_g1": g1, "beta_g2": g2, "gamma_g2": g2.copy(), "delta_g2": g2.copy(),
+                "gamma_abc_g1": np.zeros(max(n_abc, 1) * self.g1_bytes // 4, dtype=np.uint32)}
 
     def pk_query(self, pk, which, count):
         per = self.g2_bytes if which in (2, 6) else self.g1_bytes
@@ -548,12 +578,9 @@ class Backend:
         n, used = c_uint64(), c_uint64()
         self._ck(self.lib.b2s_vk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), None, None, None, None,
                                              None, 0, ctypes.byref(n), ctypes.byref(used)))
-        vk = {"alpha_g1": np.zeros(self.g1_bytes // 4, dtype=np.uint32), "beta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
-              "gamma_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32), "delta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
-              "gamma_abc_g1": np.zeros(max(n.value, 1) * self.g1_bytes // 4, dtype=np.uint32)}
-        self._ck(self.lib.b2s_vk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate), vk["alpha_g1"].ctypes.data,
-                                             vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data, vk["delta_g2"].ctypes.data,
-                                             vk["gamma_abc_g1"].ctypes.data, n.value, ctypes.byref(n), ctypes.byref(used)))
+        vk = self._vk_bufs(n.value)
+        self._ck(self.lib.b2s_vk_deserialize(self.h, buf.ctypes.data, len(buf), int(compressed), int(validate),
+                                             *(v.ctypes.data for v in vk.values()), n.value, ctypes.byref(n), ctypes.byref(used)))
         vk["gamma_abc_g1"] = vk["gamma_abc_g1"][: n.value * self.g1_bytes // 4]
         return vk, used.value
 
@@ -594,13 +621,10 @@ class Backend:
         buf = self._file_bytes(data)
         info = self.zkey_info(buf)
         n_abc = info["n_public"] + 1
-        vk = {"alpha_g1": np.zeros(self.g1_bytes // 4, dtype=np.uint32), "beta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
-              "gamma_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32), "delta_g2": np.zeros(self.g2_bytes // 4, dtype=np.uint32),
-              "gamma_abc_g1": np.zeros(n_abc * self.g1_bytes // 4, dtype=np.uint32)}
+        vk = self._vk_bufs(n_abc)
         pk, m = c_void_p(), c_void_p()
         self._ck(self.lib.b2s_zkey_load(self.h, buf.ctypes.data, buf.nbytes, int(validate), ctypes.byref(pk), ctypes.byref(m),
-                                        vk["alpha_g1"].ctypes.data, vk["beta_g2"].ctypes.data, vk["gamma_g2"].ctypes.data,
-                                        vk["delta_g2"].ctypes.data, vk["gamma_abc_g1"].ctypes.data, n_abc))
+                                        *(v.ctypes.data for v in vk.values()), n_abc))
         self._r1cs_vars[m.value] = info["n_vars"]
         return pk, m, vk
 
@@ -631,13 +655,9 @@ class Backend:
         """One verdict per proof.  inputs: n_proofs x n_inputs Montgomery Fr (None when n_inputs == 0); a, b, c: affine
         arrays; all HOST numpy or all CUDA torch tensors.  Returns a bool numpy array (host), or fills the uint8 tensor
         `ok` (device) and returns it."""
-        pa, mem = _ptr(a)
-        pb, mem_b = _ptr(b)
-        pc, mem_c = _ptr(c)
-        px, mem_x = _ptr(inputs)
-        assert mem == mem_b == mem_c and (inputs is None or mem_x == mem)
+        (pa, pb, pc, px), mem = _ptrs(a, b, c, inputs)
         if n_proofs is None:
-            n_proofs = (a.nbytes if isinstance(a, np.ndarray) else a.numel() * a.element_size()) // self.g1_bytes
+            n_proofs = _nbytes(a) // self.g1_bytes
         if mem == MEM_HOST:
             out = np.zeros(max(n_proofs, 1), dtype=np.uint8)
             self._ck(self.lib.b2s_groth16_verify_batch(self.h, pvk, n_proofs, px, n_inputs, pa, pb, pc, mem, out.ctypes.data))
@@ -650,19 +670,11 @@ class Backend:
         """True when every proof is accepted, by one random linear combination of the batch (b2s_groth16_verify_batch_rlc).
         Buffers as for groth16_verify_batch.  rho: n_proofs x 4 uint32 words (little-endian 128-bit, nonzero) in the same
         memory as the proofs; None draws them with `secrets`.  On False, groth16_verify_batch tells which proofs failed."""
-        pa, mem = _ptr(a)
-        pb, mem_b = _ptr(b)
-        pc, mem_c = _ptr(c)
-        px, mem_x = _ptr(inputs)
-        assert mem == mem_b == mem_c and (inputs is None or mem_x == mem)
+        (pa, pb, pc, px), mem = _ptrs(a, b, c, inputs)
         if n_proofs is None:
-            n_proofs = (a.nbytes if isinstance(a, np.ndarray) else a.numel() * a.element_size()) // self.g1_bytes
+            n_proofs = _nbytes(a) // self.g1_bytes
         if rho is None:
-            rho = random_rho(n_proofs)
-            if mem == MEM_DEVICE:
-                import torch
-
-                rho = torch.from_numpy(rho.view(np.int32)).to(a.device)
+            rho = _draw_rho(n_proofs, mem, a)
         pr, mem_r = _ptr(rho)
         assert n_proofs == 0 or mem_r == mem
         ok = ctypes.c_uint8(0)
@@ -673,7 +685,7 @@ class Backend:
         """serialized proofs (bytes / numpy uint8 on the HOST, or a CUDA torch uint8 tensor) -> (address, mem, len, n_proofs)"""
         if isinstance(proofs, (bytes, bytearray, memoryview)):
             proofs = np.frombuffer(bytes(proofs), dtype=np.uint8)
-        ln = proofs.nbytes if isinstance(proofs, np.ndarray) else proofs.numel() * proofs.element_size()
+        ln = _nbytes(proofs)
         pp, mem = _ptr(proofs)
         if n_proofs is None:
             n_proofs = ln // (4 * self.fq_bytes * (1 if compressed else 2))
@@ -706,11 +718,7 @@ class Backend:
         px, mem_x = _ptr(inputs)
         assert inputs is None or mem_x == mem
         if rho is None:
-            rho = random_rho(n_proofs)
-            if mem == MEM_DEVICE:
-                import torch
-
-                rho = torch.from_numpy(rho.view(np.int32)).to(proofs.device)
+            rho = _draw_rho(n_proofs, mem, proofs)
         pr, mem_r = _ptr(rho)
         assert n_proofs == 0 or mem_r == mem
         if mem == MEM_HOST:
@@ -724,16 +732,12 @@ class Backend:
     def pairing(self, p, q, n=None, out=None):
         """e(P_i, Q_i) element-wise.  p, q: affine G1 / G2 arrays (HOST numpy, or CUDA torch tensors with `out` a device
         tensor of n * 12 Fq).  Returns GT elements as uint32 limbs (ark's Fp12 layout, Montgomery)."""
-        pp, mem = _ptr(p)
-        pq, mem_q = _ptr(q)
-        assert mem == mem_q
         if n is None:
-            n = (p.nbytes if isinstance(p, np.ndarray) else p.numel() * p.element_size()) // self.g1_bytes
+            n = _nbytes(p) // self.g1_bytes
         if out is None:
-            assert mem == MEM_HOST
+            assert _ptr(p)[1] == MEM_HOST
             out = np.zeros(n * 12 * self.fq_bytes // 4, dtype=np.uint32)
-        po, mem_o = _ptr(out)
-        assert mem_o == mem
+        (pp, pq, po), mem = _ptrs(p, q, out)
         self._ck(self.lib.b2s_pairing(self.h, pp, pq, n, mem, po))
         return out
 
@@ -758,19 +762,10 @@ class Backend:
         Montgomery Fr (row i = proof i's instance || witness); r, s: n_proofs Montgomery Fr each; all HOST numpy arrays or all
         CUDA torch tensors.  Returns (a, b, c): n_proofs x (G1 / G2 / G1 affine) uint32 numpy arrays, or int32 tensors on the
         device of the inputs (the library's stream is synchronised before return)."""
-        pz, mem = _ptr(z)
-        pr, mem_r = _ptr(r)
-        ps, mem_s = _ptr(s)
-        assert mem == mem_r == mem_s
-        n = (r.nbytes if isinstance(r, np.ndarray) else r.numel() * r.element_size()) // self.fr_bytes
+        (pz, pr, ps), mem = _ptrs(z, r, s)
+        n = _nbytes(r) // self.fr_bytes
         w1, w2 = self.g1_bytes // 4, self.g2_bytes // 4
-        if mem == MEM_HOST:
-            a, b, c = (np.zeros((n, w), dtype=np.uint32) for w in (w1, w2, w1))
-        else:
-            import torch
-
-            a, b, c = (torch.zeros((n, w), dtype=torch.int32, device=r.device) for w in (w1, w2, w1))
-            torch.cuda.current_stream(r.device).synchronize()
+        a, b, c = _zeros([(n, w1), (n, w2), (n, w1)], np.uint32, mem, r)
         self._ck(self.lib.b2s_groth16_prove_batch(self.h, pk, m, n, pz, pr, ps, mem, _ptr(a)[0], _ptr(b)[0], _ptr(c)[0]))
         return a, b, c
 
