@@ -65,7 +65,7 @@ extern "C" {
  *                     writes it).  The rest of the key and the proof are unchanged; the verifiers below take circom proofs as
  *                     they are.  Not provided: the distributed witness map (b2s_groth16_prove_group* refuse circom keys with
  *                     B2S_ERR_INVALID_ARG; b2s_groth16_prove_shard + b2s_groth16_finish work).  snarkjs .zkey and circom
- *                     .wtns files load directly: b2s_zkey_load / b2s_wtns_read below.
+ *                     .wtns and .r1cs files load directly: b2s_zkey_load / b2s_wtns_read / b2s_r1cs_file_load below.
  * Any other value is B2S_ERR_INVALID_ARG. */
 #define B2S_QAP_LIBSNARK 0
 #define B2S_QAP_CIRCOM 1
@@ -391,7 +391,8 @@ int32_t b2s_pk_deserialize_qap(b2s_ctx* ctx, const uint8_t* in, uint64_t len, in
  *                       build from the same points and matrices: a full circom key (n_instance = nPublic + 1, the h query
  *                       table built as by b2s_pk_deserialize) and a matrix handle of A and B over the circuit's constraints
  *                       with an EMPTY C (snarkjs's trailing input rows are checked and left to the witness map).  On such a
- *                       handle b2s_r1cs_check checks A z o B z = 0, which is not the circuit's satisfaction.  The verifying key
+ *                       handle b2s_r1cs_check checks A z o B z = 0, which is not the circuit's satisfaction: load the
+ *                       circuit's .r1cs with b2s_r1cs_file_load for that (its handle proves under this key too).  The verifying key
  *                       goes to the HOST in the form b2s_vk_prepare takes: alpha_g1, beta_g2, gamma_g2, delta_g2 and
  *                       nPublic + 1 gamma_abc_g1 points (cap_gamma_abc = room in out_gamma_abc_g1).
  *   b2s_wtns_read       a .wtns -> z = instance || witness, n_vars Montgomery Fr in `mem` (HOST or DEVICE), for
@@ -411,6 +412,32 @@ int32_t b2s_zkey_load(b2s_ctx* ctx, const uint8_t* in, uint64_t len, int32_t val
                       void* out_alpha_g1, void* out_beta_g2, void* out_gamma_g2, void* out_delta_g2, void* out_gamma_abc_g1,
                       uint64_t cap_gamma_abc);
 int32_t b2s_wtns_read(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t n_vars, int32_t mem, void* out_z);
+
+/* ---- circom .r1cs files (ark-circom R1CSFile + to_matrices + b2s_r1cs_upload, in one call) -------------------------------
+ * The format (iden3 r1cs binfile, version 1) is restated in snark_b200/csrc/zkey.cu; it is NOT pinned against bytes written
+ * by circom.  Bytes on the HOST.  The host walks the 3 mConstraints count words only; every entry is decoded and checked on
+ * the device.  There is no validate flag: every check is always on.
+ *   b2s_r1cs_file_read_info  the framing and the header (section 1) only; allocates nothing.  domain_size =
+ *                            next_pow2(nConstraints + 1 + nPubOut + nPubIn).
+ *   b2s_r1cs_file_load       the circuit -> the handle b2s_r1cs_upload builds from the same matrices: n_rows = mConstraints,
+ *                            n_instance = 1 + nPubOut + nPubIn, n_witness = nWires - n_instance, A, B and C filled (duplicate
+ *                            wires in one linear combination are summed).  Every entry point that takes a b2s_r1cs works on
+ *                            it: b2s_r1cs_check checks the circuit's own constraints, b2s_groth16_setup[_qap] makes keys under
+ *                            either reduction, and it proves under the key of b2s_zkey_load (the circom witness map reads
+ *                            A and B only; snarkjs's input rows stay implicit, as for the zkey's handle).
+ * Errors (b2s_last_error names the section, or the constraint, matrix and entry, with the reason, e.g.
+ * "r1cs constraint 17 C[2]: wire 900 not below nWires 512"):
+ *   B2S_ERR_INVALID_DATA    bad magic, version or framing; truncation; a duplicate, missing or wrongly sized section; PLONK
+ *                           custom-gate sections (4, 5); nWires < 1 + nPubOut + nPubIn + nPrvIn; a count that overruns
+ *                           section 2, or bytes after its mConstraints constraints; a wire >= nWires; a coefficient >= r
+ *   B2S_ERR_INVALID_ARG     a prime other than the ctx curve's r; a null pointer
+ *   B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE  a domain past the limits of b2s_r1cs_upload (decided from the header, before the walk
+ *                           or any allocation); 2^32 or more nonzeros in one matrix */
+typedef struct b2s_r1cs_file_info {
+    uint64_t n_wires, n_pub_out, n_pub_in, n_prv_in, n_labels, n_constraints, domain_size;
+} b2s_r1cs_file_info;
+int32_t b2s_r1cs_file_read_info(b2s_ctx* ctx, const uint8_t* in, uint64_t len, b2s_r1cs_file_info* out);
+int32_t b2s_r1cs_file_load(b2s_ctx* ctx, const uint8_t* in, uint64_t len, b2s_r1cs** out);
 
 /* ---- verification: pairings and batched Groth16 verify ----------------------------------------------------------------
  * The optimal ate pairing in CUDA (snark_b200/csrc/pairing.cuh): BLS12-381 loops over |x| and conjugates, BN254 over the

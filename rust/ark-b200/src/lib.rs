@@ -34,6 +34,13 @@ pub struct B2sPredicateDesc {
 pub struct B2sZkeyInfo { pub n_vars: u64, pub n_public: u64, pub domain_size: u64, pub n_coeffs: u64 }
 
 #[repr(C)]
+#[derive(Default)]
+pub struct B2sR1csFileInfo {
+    pub n_wires: u64, pub n_pub_out: u64, pub n_pub_in: u64, pub n_prv_in: u64, pub n_labels: u64, pub n_constraints: u64,
+    pub domain_size: u64,
+}
+
+#[repr(C)]
 pub struct B2sPkDesc {
     pub n_instance: u64, pub n_witness: u64, pub domain_size: u64,
     pub alpha_g1: *const c_void, pub beta_g1: *const c_void, pub delta_g1: *const c_void,
@@ -96,6 +103,9 @@ extern "C" {
                          out_alpha_g1: *mut c_void, out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void, out_delta_g2: *mut c_void,
                          out_gamma_abc_g1: *mut c_void, cap_gamma_abc: u64) -> i32;
     pub fn b2s_wtns_read(ctx: *mut B2sCtx, inp: *const u8, len: u64, n_vars: u64, mem: i32, out_z: *mut c_void) -> i32;
+    // circom .r1cs files (ark-circom R1CSFile + to_matrices + b2s_r1cs_upload), walked on the host and decoded on the GPU
+    pub fn b2s_r1cs_file_read_info(ctx: *mut B2sCtx, inp: *const u8, len: u64, out: *mut B2sR1csFileInfo) -> i32;
+    pub fn b2s_r1cs_file_load(ctx: *mut B2sCtx, inp: *const u8, len: u64, out: *mut *mut B2sR1cs) -> i32;
     pub fn b2s_groth16_setup_qap(ctx: *mut B2sCtx, m: *const B2sR1cs, trapdoor: *const c_void, qap: i32, out_pk: *mut *mut B2sPk,
                                  out_alpha_g1: *mut c_void, out_beta_g2: *mut c_void, out_gamma_g2: *mut c_void,
                                  out_delta_g2: *mut c_void, out_gamma_abc_g1: *mut c_void) -> i32;
@@ -306,6 +316,17 @@ impl<E: Pairing + B200Curve> Groth16B200<E> {
             gamma_abc_g1: abc.chunks(g1).map(unpack_point::<E::G1Affine>).collect(),
         };
         Ok((Resident { ctx, pk, mat }, vk))
+    }
+
+    /// The circuit's A, B and C from the bytes of its circom `.r1cs`, loaded into `res`'s context (b2s_r1cs_file_load: the
+    /// count words are walked on the host, every entry is decoded and range-checked on the GPU).  Unlike the zkey's matrix
+    /// handle it has C, so b2s_r1cs_check on it checks the circuit's own constraints, and it proves under `res.pk` with the
+    /// same proofs.  The caller frees it with `b2s_r1cs_free(res.ctx, m)` before `res` is dropped.  The format is restated
+    /// from the iden3 r1cs spec, not pinned against bytes circom wrote.
+    pub fn load_r1cs(res: &Resident, r1cs: &[u8]) -> Result<*mut B2sR1cs, B200Error> {
+        let mut mat: *mut B2sR1cs = core::ptr::null_mut();
+        check(res.ctx, unsafe { b2s_r1cs_file_load(res.ctx, r1cs.as_ptr(), r1cs.len() as u64, &mut mat) })?;
+        Ok(mat)
     }
 
     /// `prove` for many circuits of one shape under one resident key, in one GPU call (b2s_groth16_prove_batch): each

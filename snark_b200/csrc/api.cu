@@ -39,6 +39,8 @@ int32_t zkey_read_info(Ctx* c, const uint8_t* in, uint64_t len, b2s_zkey_info* o
 int32_t zkey_load(Ctx* c, const uint8_t* in, uint64_t len, bool validate, b2s_pk** out_pk, b2s_r1cs** out_m, void* alpha_g1,
                   void* beta_g2, void* gamma_g2, void* delta_g2, void* gamma_abc, uint64_t cap_abc);
 int32_t wtns_read(Ctx* c, const uint8_t* in, uint64_t len, uint64_t n_vars, int32_t mem, void* out_z);
+int32_t r1cs_file_read_info(Ctx* c, const uint8_t* in, uint64_t len, b2s_r1cs_file_info* out);
+int32_t r1cs_file_load(Ctx* c, const uint8_t* in, uint64_t len, b2s_r1cs** out);
 // verify.cu
 int32_t vk_prepare(Ctx* c, const void* alpha, const void* beta, const void* gamma, const void* delta, const void* abc, uint64_t n_abc,
                    b2s_pvk** out);
@@ -685,6 +687,17 @@ int32_t b2s_wtns_read(b2s_ctx* ctx, const uint8_t* in, uint64_t len, uint64_t n_
     LOCK(ctx);
     if (!in || !out_z) return fail(ctx, B2S_ERR_INVALID_ARG, "wtns_read: null argument");
     return wtns_read(ctx, in, len, n_vars, mem, out_z);
+}
+int32_t b2s_r1cs_file_read_info(b2s_ctx* ctx, const uint8_t* in, uint64_t len, b2s_r1cs_file_info* out) {
+    LOCK(ctx);
+    if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_file_read_info: null argument");
+    return r1cs_file_read_info(ctx, in, len, out);
+}
+int32_t b2s_r1cs_file_load(b2s_ctx* ctx, const uint8_t* in, uint64_t len, b2s_r1cs** out) {
+    LOCK(ctx);
+    if (!in || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_file_load: null argument");
+    *out = nullptr;
+    return r1cs_file_load(ctx, in, len, out);
 }
 
 int32_t b2s_vk_prepare(b2s_ctx* ctx, const void* alpha_g1, const void* beta_g2, const void* gamma_g2, const void* delta_g2,

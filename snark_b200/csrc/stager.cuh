@@ -6,6 +6,7 @@
 
 #include <algorithm>
 #include <cstring>
+#include <utility>
 
 #include "common.cuh"
 #include "deserialize.cuh"
@@ -83,17 +84,36 @@ struct Stager {
     template <class Launch>
     int32_t chunks(const uint8_t* in, uint64_t count, size_t pb, Launch&& launch) {
         B2S_TRY(reserve((size_t)std::min<uint64_t>(count, CH) * pb));
+        return copy_loop<true>(in, (count + CH - 1) / CH, pb,
+                               [&](uint64_t k) { return std::make_pair(k * CH * pb, std::min<uint64_t>(CH, count - k * CH) * pb); }, launch);
+    }
+    // Variable-length items from the HOST: span j is bytes [cut[j], cut[j + 1]) of `in`, j < n_spans, chosen by the caller
+    // (runs of whole items, about a chunk's worth each).  The buffers are reserved for the longest span, so one item longer
+    // than a chunk still goes in one piece.  launch(src_dev, j) queues the kernel that consumes span j, staged at src_dev.
+    // The error word `err` is set to ~0 first.
+    template <class Launch>
+    int32_t spans(const uint8_t* in, const uint64_t* cut, uint64_t n_spans, Launch&& launch) {
+        uint64_t longest = 0;
+        for (uint64_t j = 0; j < n_spans; j++) longest = std::max(longest, cut[j + 1] - cut[j]);
+        B2S_TRY(reserve((size_t)longest));
+        return copy_loop<false>(in, n_spans, 0, [&](uint64_t j) { return std::make_pair(cut[j], cut[j + 1] - cut[j]); }, launch);
+    }
+    // the copy / launch pipeline of chunks and spans: piece k is span(k) = (offset, bytes) of `in`, at most cap bytes, consumed
+    // by launch(src_dev, items, first item) of pb-byte items (ITEMS) or by launch(src_dev, k)
+    template <bool ITEMS, class Span, class Launch>
+    int32_t copy_loop(const uint8_t* in, uint64_t n_pieces, size_t pb, Span&& span, Launch&& launch) {
         B2S_CUDA(c, cudaMemsetAsync(err.p, 0xFF, sizeof(unsigned long long), c->stream));
-        for (uint64_t base = 0, k = 0; base < count; base += CH, k++) {
+        for (uint64_t k = 0; k < n_pieces; k++) {
             const int s = (int)(k & 1);
-            const uint32_t n = (uint32_t)std::min<uint64_t>(CH, count - base);
+            const auto [off, n] = span(k);
             if (k >= 2) B2S_CUDA(c, cudaEventSynchronize(copied[s]));   // pinned[s] is free again
-            memcpy(pinned[s], in + base * pb, (size_t)n * pb);
+            memcpy(pinned[s], in + off, (size_t)n);
             if (k >= 2) B2S_CUDA(c, cudaStreamWaitEvent(c->side, consumed[s], 0));   // dev[s] has been consumed
-            B2S_CUDA(c, cudaMemcpyAsync(dev[s].p, pinned[s], (size_t)n * pb, cudaMemcpyHostToDevice, c->side));
+            B2S_CUDA(c, cudaMemcpyAsync(dev[s].p, pinned[s], (size_t)n, cudaMemcpyHostToDevice, c->side));
             B2S_CUDA(c, cudaEventRecord(copied[s], c->side));
             B2S_CUDA(c, cudaStreamWaitEvent(c->stream, copied[s], 0));
-            B2S_TRY(launch(dev[s].as<const uint8_t>(), n, base));
+            if constexpr (ITEMS) B2S_TRY(launch(dev[s].as<const uint8_t>(), (uint32_t)(n / pb), off / pb));
+            else B2S_TRY(launch(dev[s].as<const uint8_t>(), k));
             B2S_CUDA(c, cudaEventRecord(consumed[s], c->stream));
         }
         return B2S_OK;

@@ -1,13 +1,15 @@
-// Readers of the two files a circom user has: the Groth16 .zkey written by `snarkjs groth16 setup` / `zkey contribute`, and
-// the .wtns written by circom's witness generator.  They stand in for ark-circom's `read_zkey` and snarkjs's
-// `zkey_utils.js` / `wtns_utils.js`, and give the handles b2s_pk_upload_qap(.., B2S_QAP_CIRCOM, ..) and b2s_r1cs_upload would
-// build from the same points and matrices.
+// Readers of the three files a circom user has: the Groth16 .zkey written by `snarkjs groth16 setup` / `zkey contribute`,
+// the .wtns written by circom's witness generator and the circuit's .r1cs written by the circom compiler.  They stand in for
+// ark-circom's `read_zkey` / `R1CSFile` and snarkjs's `zkey_utils.js` / `wtns_utils.js`, and give the handles
+// b2s_pk_upload_qap(.., B2S_QAP_CIRCOM, ..) and b2s_r1cs_upload would build from the same points and matrices.
 //
-// The formats, restated from snarkjs and ark-circom (neither is in the reference tree, and no file written by snarkjs is
-// available here, so byte parity with them is NOT pinned -- tests/zkey_oracle.py restates the same writers):
-//   binfile framing (both files): 4-byte magic "zkey" / "wtns", u32 LE version (zkey 1, wtns 2), u32 LE section count, then per
-//     section a u32 type, a u64 size and `size` bytes.  Sections may come in any order and are indexed by type; unknown types
-//     and zkey section 10 (contributions) are skipped; a required section that appears twice is malformed.
+// The formats, restated from snarkjs, ark-circom and the iden3 r1cs binfile spec (none is in the reference tree, and no file
+// written by snarkjs or circom is available here, so byte parity with them is NOT pinned -- tests/zkey_oracle.py and
+// tests/r1cs_file_oracle.py restate the same writers):
+//   binfile framing (all three files): 4-byte magic "zkey" / "wtns" / "r1cs", u32 LE version (zkey 1, wtns 2, r1cs 1), u32 LE
+//     section count, then per section a u32 type, a u64 size and `size` bytes.  Sections may come in any order and are indexed
+//     by type; unknown types and zkey section 10 (contributions) are skipped; a section this reader indexes that appears twice
+//     is malformed.
 //   zkey  1  u32 protocol: 1 = Groth16 (2 PLONK and 10 FFLONK are rejected)
 //         2  n8q, q (n8q bytes LE), n8r, r, nVars, nPublic, domainSize (u32 each), then alpha1 (G1), beta1 (G1), beta2 (G2),
 //            gamma2 (G2), delta1 (G1), delta2 (G2)
@@ -26,14 +28,27 @@
 //     entry there, keeps rows [0, n_constraints) and requires domainSize = next_pow2(n_constraints + nPublic + 1).
 //   wtns  1  n8, prime (n8 bytes LE), u32 nWitness
 //         2  nWitness values, canonical LE (not Montgomery); nWitness = nVars and z[0] = 1
+//   r1cs  1  header, exactly n8 + 32 bytes: u32 n8, the prime (n8 bytes LE), u32 nWires, nPubOut, nPubIn, nPrvIn, u64 nLabels,
+//            u32 mConstraints
+//         2  constraints: per constraint, for A, then B, then C, a u32 count and `count` x (u32 wire, n8-byte coefficient);
+//            coefficients canonical LE (not Montgomery), each below r.  Constraint i: <A_i, z> <B_i, z> - <C_i, z> = 0 with z
+//            in wire order (One, public outputs, public inputs, private inputs, internal wires).  Duplicate wires in one
+//            linear combination are summed; empty combinations are allowed.
+//         3  wire -> label map (optional): nWires u64, not read
+//         4 / 5  PLONK custom gates: rejected
+//     The handle: n_rows = mConstraints, n_instance = 1 + nPubOut + nPubIn, n_witness = nWires - n_instance, A, B, C filled.
 //
-// The host reads the file headers and section offsets only.  Points are checked in place by the decode kernel (stager.cuh,
+// The host reads the file headers and section offsets only (for an .r1cs also the 3 m count words, the one sequential
+// dependency of the file: they give each constraint's offset).  Points are checked in place by the decode kernel (stager.cuh,
 // decode_point_mont); coefficient records are parsed, range-checked and reduced by one kernel per chunk, then sorted into CSR
 // by row counts, a scan and a placement pass, which also checks the input rows.  Non-ONE coefficients get one pool entry each,
-// compacted by a scan (no host-side interning: the sums are exact, whatever the order and the duplication).
+// compacted by a scan (no host-side interning: the sums are exact, whatever the order and the duplication).  An .r1cs is
+// already in CSR order: its row pointers come from a scan of the walk's counts, and one kernel per run of whole constraints
+// decodes, checks and places every entry.
 #include <cuda_runtime.h>
 
 #include <cstring>
+#include <vector>
 
 #include "common.cuh"
 #include "deserialize.cuh"
@@ -56,9 +71,11 @@ uint64_t rd64(const uint8_t* p) { return (uint64_t)rd32(p) | (uint64_t)rd32(p + 
 
 struct Section { uint64_t off = 0, size = 0; bool seen = false; };
 
-// Indexes a binfile: sections 1..n_types kept in sec[type] (each at most once), any other type skipped.  Every section must
-// lie inside the `len` bytes and the last one must end there.
-int32_t bin_sections(Ctx* c, const char* magic, const uint8_t* in, uint64_t len, uint32_t version, int n_types, Section* sec) {
+// Indexes a binfile: sections 1..n_types kept in sec[type] (each at most once), any other type skipped; sections
+// 1..n_required must be present (n_required < 0: all n_types).  Every section must lie inside the `len` bytes and the last one
+// must end there.
+int32_t bin_sections(Ctx* c, const char* magic, const uint8_t* in, uint64_t len, uint32_t version, int n_types, Section* sec,
+                     int n_required = -1) {
     if (len < 12 || memcmp(in, magic, 4) != 0) return fail(c, B2S_ERR_INVALID_DATA, "%s: bad magic (not a .%s file)", magic, magic);
     const uint32_t ver = rd32(in + 4), n = rd32(in + 8);
     if (ver != version) return fail(c, B2S_ERR_INVALID_DATA, "%s: version %u, expected %u", magic, ver, version);
@@ -78,7 +95,7 @@ int32_t bin_sections(Ctx* c, const char* magic, const uint8_t* in, uint64_t len,
         at += size;
     }
     if (at != len) return fail(c, B2S_ERR_INVALID_DATA, "%s: %llu trailing bytes after the last section", magic, (unsigned long long)(len - at));
-    for (int t = 1; t <= n_types; t++)
+    for (int t = 1; t <= (n_required < 0 ? n_types : n_required); t++)
         if (!sec[t].seen) return fail(c, B2S_ERR_INVALID_DATA, "%s: section %d missing", magic, t);
     return B2S_OK;
 }
@@ -351,6 +368,275 @@ __global__ void wtns_kernel(const uint8_t* __restrict__ src, uint32_t n, uint64_
     out[e] = v.to_mont();
 }
 
+// ---- circom .r1cs ----------------------------------------------------------------------------------------------------
+constexpr uint32_t R1CS_ENTRY = 4 + FR_BYTES;   // u32 wire, then the coefficient
+enum R1csSection { R_HEADER = 1, R_CONSTRAINTS, R_WIRE_MAP, R_GATES_USED, R_GATES_APPLIED, R_SECTIONS = R_GATES_APPLIED };
+enum EntryReason : uint32_t { EN_WIRE = 1, EN_VALUE };
+const char MATRIX_NAME[3] = {'A', 'B', 'C'};
+
+struct R1csFile {
+    Section s[R_SECTIONS + 1];
+    b2s_r1cs_file_info info{};
+    uint64_t n_instance = 0;
+    uint32_t log_domain = 0;
+};
+
+// framing, curve and dimensions, the domain limits included: every check that needs no per-constraint data
+int32_t r1cs_parse(Ctx* c, const uint8_t* in, uint64_t len, R1csFile& f) {
+    B2S_TRY(bin_sections(c, "r1cs", in, len, 1, R_SECTIONS, f.s, R_CONSTRAINTS));
+    for (int t : {R_GATES_USED, R_GATES_APPLIED})
+        if (f.s[t].seen) return fail(c, B2S_ERR_INVALID_DATA, "r1cs: section %d (PLONK custom gates) is not supported", t);
+    const Section& h = f.s[R_HEADER];
+    const uint8_t* b = in + h.off;
+    const uint32_t n8 = h.size >= 4 ? rd32(b) : 0;
+    if (h.size < 4 || h.size != 32ull + n8)
+        return fail(c, B2S_ERR_INVALID_DATA, "r1cs: header section holds %llu bytes, n8 = %u needs %llu", (unsigned long long)h.size, n8,
+                    32ull + n8);
+    const bool same_field = dispatch_curve(c, [&](auto curve) { return (int32_t)is_modulus<typename decltype(curve)::FrP>(b + 4, n8); }) == 1;
+    if (!same_field) return fail(c, B2S_ERR_INVALID_ARG, "r1cs: the prime (%u bytes) is not the scalar field of the ctx's curve", n8);
+    const uint8_t* d = b + 4 + n8;
+    b2s_r1cs_file_info& i = f.info;
+    i.n_wires = rd32(d);
+    i.n_pub_out = rd32(d + 4);
+    i.n_pub_in = rd32(d + 8);
+    i.n_prv_in = rd32(d + 12);
+    i.n_labels = rd64(d + 16);
+    i.n_constraints = rd32(d + 24);
+    if (i.n_wires < 1 + i.n_pub_out + i.n_pub_in + i.n_prv_in)
+        return fail(c, B2S_ERR_INVALID_DATA, "r1cs: nWires %llu < 1 + nPubOut %llu + nPubIn %llu + nPrvIn %llu", (unsigned long long)i.n_wires,
+                    (unsigned long long)i.n_pub_out, (unsigned long long)i.n_pub_in, (unsigned long long)i.n_prv_in);
+    const Section& wm = f.s[R_WIRE_MAP];
+    if (wm.seen && wm.size != 8 * i.n_wires)
+        return fail(c, B2S_ERR_INVALID_DATA, "r1cs: section 3 (wire map) holds %llu bytes, nWires %llu need %llu", (unsigned long long)wm.size,
+                    (unsigned long long)i.n_wires, (unsigned long long)(8 * i.n_wires));
+    f.n_instance = 1 + i.n_pub_out + i.n_pub_in;
+    uint32_t logd = 0;
+    while ((1ull << logd) < i.n_constraints + f.n_instance) logd++;
+    const uint32_t two_adicity = (uint32_t)dispatch_curve(c, [](auto curve) { return (int32_t)decltype(curve)::FrP::TWO_ADICITY; });
+    if (logd > two_adicity || logd > 27)   // the limits of b2s_r1cs_upload
+        return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "r1cs: %llu constraints and %llu instance variables need domain 2^%u, unsupported",
+                    (unsigned long long)i.n_constraints, (unsigned long long)f.n_instance, logd);
+    f.log_domain = logd;
+    i.domain_size = 1ull << logd;
+    return B2S_OK;
+}
+
+// The host's part of the constraint section: its 3 m count words, each checked against the bytes that remain (64-bit), and
+// the walk must end at the section's end.  counts[k m + i] = the entries of matrix k in constraint i.  The section is cut
+// into spans of whole constraints of at most a chunk's bytes (one longer constraint makes a span of its own): span j holds
+// constraints [row[j], row[j + 1]), bytes [cut[j], cut[j + 1]) of the section, and matrix k's entries from first[3 j + k].
+struct R1csWalk {
+    std::vector<uint32_t> counts;
+    uint64_t nnz[3] = {0, 0, 0};
+    std::vector<uint64_t> cut, row, first;
+};
+
+int32_t r1cs_walk(Ctx* c, const uint8_t* p, uint64_t size, uint64_t m, R1csWalk& w) {
+    const uint64_t span_max = Stager::CH * R1CS_ENTRY;
+    w.counts.resize(3 * m);
+    auto close_span = [&](uint64_t at, uint64_t i) {
+        w.cut.push_back(at);
+        w.row.push_back(i);
+        w.first.insert(w.first.end(), w.nnz, w.nnz + 3);
+    };
+    close_span(0, 0);
+    uint64_t at = 0;
+    for (uint64_t i = 0; i < m; i++) {
+        const uint64_t start = at;
+        for (int k = 0; k < 3; k++) {
+            if (size - at < 4)
+                return fail(c, B2S_ERR_INVALID_DATA, "r1cs constraint %llu %c: the count word overruns section 2 (%llu bytes)", (unsigned long long)i,
+                            MATRIX_NAME[k], (unsigned long long)size);
+            const uint64_t n = rd32(p + at);
+            at += 4;
+            if (n > (size - at) / R1CS_ENTRY)
+                return fail(c, B2S_ERR_INVALID_DATA, "r1cs constraint %llu %c: %llu entries overrun section 2 (%llu bytes remain)",
+                            (unsigned long long)i, MATRIX_NAME[k], (unsigned long long)n, (unsigned long long)(size - at));
+            at += n * R1CS_ENTRY;
+            w.counts[k * m + i] = (uint32_t)n;
+        }
+        if (start > w.cut.back() && at - w.cut.back() > span_max) close_span(start, i);
+        for (int k = 0; k < 3; k++) w.nnz[k] += w.counts[k * m + i];
+    }
+    if (at != size)
+        return fail(c, B2S_ERR_INVALID_DATA, "r1cs: section 2 holds %llu bytes after its %llu constraints", (unsigned long long)(size - at),
+                    (unsigned long long)m);
+    if (m) close_span(at, m);
+    for (int k = 0; k < 3; k++)
+        if (w.nnz[k] >= (1ull << 32))
+            return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "r1cs: matrix %c has %llu nonzeros, 2^32 or more", MATRIX_NAME[k],
+                        (unsigned long long)w.nnz[k]);
+    return B2S_OK;
+}
+
+struct R1csMats {
+    uint64_t* row_ptr[3];
+    uint32_t* col[3];
+    uint32_t* cid[3];
+    uint64_t base[3];   // matrix k's entries start at base[k] in the arrays of all entries (val, nonone, pool_off)
+};
+// member k of three, without indexing a kernel parameter by a runtime k (which would copy it to local memory)
+template <class T>
+__device__ __forceinline__ T pick3(const T (&a)[3], uint32_t k) { return k == 0 ? a[0] : k == 1 ? a[1] : a[2]; }
+struct R1csSpan {
+    uint64_t row0, row1, byte0;   // constraints [row0, row1), staged from section byte byte0 on
+    uint64_t first[3];            // the span's first entry of each matrix
+    uint32_t n[3];                // and its entries of each matrix
+};
+
+// row_ptr[k][r] = offsets[k (M + 1) + r] (the three per-matrix scans of the counts, widened)
+__global__ void r1cs_rows_kernel(const uint32_t* __restrict__ offsets, uint64_t M, R1csMats o) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= 3 * (M + 1)) return;
+    const uint32_t k = (uint32_t)(t / (M + 1));
+    pick3(o.row_ptr, k)[t - k * (M + 1)] = offsets[t];
+}
+
+// One thread per entry of a span, A's entries first, then B's, then C's.  Entry e of matrix k lies in the row i whose range
+// [row_ptr[k][i], row_ptr[k][i + 1]) holds it (binary search over the span's rows), at section byte
+// 12 i + 4 (k + 1) + R1CS_ENTRY (e + sum_{k' < k} row_ptr[k'][i + 1] + sum_{k' > k} row_ptr[k'][i]).  Range checks (the
+// lowest bad entry, in file order, into err with its EntryReason), then the wire into col and the Montgomery value with its
+// ONE flag at base[k] + e.
+template <class Curve>
+__global__ void __launch_bounds__(256) r1cs_entry_kernel(const uint8_t* __restrict__ src, R1csSpan sp, R1csMats o, uint32_t n_wires,
+                                                         typename Curve::Fr* __restrict__ val, uint32_t* __restrict__ nonone,
+                                                         unsigned long long* err) {
+    using Fr = typename Curve::Fr;
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= sp.n[0] + sp.n[1] + sp.n[2]) return;
+    const uint32_t k = t < sp.n[0] ? 0 : t < sp.n[0] + sp.n[1] ? 1 : 2;
+    const uint64_t e = pick3(sp.first, k) + t - (k > 0 ? sp.n[0] : 0) - (k > 1 ? sp.n[1] : 0);
+    const uint64_t* rp = pick3(o.row_ptr, k);
+    uint64_t lo = sp.row0, hi = sp.row1 - 1;   // the last row i of the span with rp[i] <= e
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi + 1) >> 1;
+        if (rp[mid] <= e) lo = mid;
+        else hi = mid - 1;
+    }
+    const uint64_t i = lo;
+    uint64_t before = e;
+#pragma unroll
+    for (uint32_t q = 0; q < 3; q++)
+        if (q != k) before += o.row_ptr[q][q < k ? i + 1 : i];   // q unrolled: no runtime index into o
+    const uint64_t at = 12 * i + 4 * (k + 1) + (uint64_t)R1CS_ENTRY * before - sp.byte0;
+    const uint32_t* w = reinterpret_cast<const uint32_t*>(src + at);
+    const uint32_t wire = w[0];
+    Fr v;
+#pragma unroll
+    for (int j = 0; j < Fr::N; j++) v.v[j] = w[1 + j];
+    const uint32_t bad = wire >= n_wires ? EN_WIRE : !dec::below_p(v) ? EN_VALUE : 0;
+    if (bad) {   // (3 i + k) < 2^29 and the index in the row < 2^32: the key sorts in file order
+        atomicMin(err, ((3 * i + k) << 32 | (e - rp[i])) << 2 | bad);
+        return;
+    }
+    v = v.to_mont();
+    const uint64_t g = pick3(o.base, k) + e;
+    pick3(o.col, k)[e] = wire;
+    val[g] = v;
+    nonone[g] = v != Fr::one();
+}
+
+// coefficient ids over all N entries: 0 for ONE, 1 + pool_off otherwise (that pool slot receives the value); pool[0] = ONE
+template <class Fr>
+__global__ void r1cs_place_kernel(uint64_t N, R1csMats o, const Fr* __restrict__ val, const uint32_t* __restrict__ nonone,
+                                  const uint32_t* __restrict__ pool_off, Fr* pool) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g == 0) pool[0] = Fr::one();
+    if (g >= N) return;
+    const uint32_t k = g >= o.base[2] ? 2 : g >= o.base[1] ? 1 : 0;
+    uint32_t id = 0;
+    if (nonone[g]) {
+        id = 1 + pool_off[g];
+        pool[id] = val[g];
+    }
+    pick3(o.cid, k)[g - pick3(o.base, k)] = id;
+}
+
+template <class Curve>
+int32_t r1cs_matrices(Ctx* c, const uint8_t* sec, const R1csFile& f, const R1csWalk& w, b2s_r1cs* m) {
+    using Fr = typename Curve::Fr;
+    const uint64_t M = f.info.n_constraints, N = w.nnz[0] + w.nnz[1] + w.nnz[2];
+    if (N >= UINT32_MAX)
+        return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "r1cs: %llu nonzeros in all, more than the coefficient pool's 2^32 - 2",
+                    (unsigned long long)N);
+    m->n_rows = M;
+    m->n_instance = f.n_instance;
+    m->n_witness = f.info.n_wires - f.n_instance;
+    m->log_domain = f.log_domain;
+    R1csMats o{};
+    for (int k = 0; k < 3; k++) {
+        m->nnz[k] = w.nnz[k];
+        B2S_TRY(m->row_ptr[k].alloc(c, (M + 1) * 8));
+        B2S_TRY(m->col[k].alloc(c, w.nnz[k] * 4));
+        B2S_TRY(m->coeff_id[k].alloc(c, w.nnz[k] * 4));
+        o.row_ptr[k] = m->row_ptr[k].as<uint64_t>();
+        o.col[k] = m->col[k].as<uint32_t>();
+        o.cid[k] = m->coeff_id[k].as<uint32_t>();
+        o.base[k] = k == 0 ? 0 : o.base[k - 1] + w.nnz[k - 1];
+    }
+    // row pointers: the counts of each matrix scanned on the device
+    DevBuf counts, offsets, task, val, nonone, pool_off, task2;
+    if (M) {
+        B2S_TRY(counts.alloc(c, 3 * M * 4));
+        B2S_TRY(offsets.alloc(c, 3 * (M + 1) * 4));
+        B2S_TRY(task.alloc(c, 3 * (M + 1) * 4));
+        B2S_CUDA(c, cudaMemcpyAsync(counts.p, w.counts.data(), 3 * M * 4, cudaMemcpyHostToDevice, c->stream));
+        for (uint64_t k = 0; k < 3; k++)
+            B2S_TRY(scan_counts(c, counts.as<uint32_t>() + k * M, (uint32_t)M, 1u, offsets.as<uint32_t>() + k * (M + 1),
+                                task.as<uint32_t>() + k * (M + 1)));
+        B2S_LAUNCH(c, r1cs_rows_kernel, cdiv(3 * (M + 1), 256), 256, 0, (const uint32_t*)offsets.as<uint32_t>(), M, o);
+    } else {
+        for (int k = 0; k < 3; k++) B2S_CUDA(c, cudaMemsetAsync(m->row_ptr[k].p, 0, 8, c->stream));
+    }
+    // every entry decoded, checked and placed, one span of whole constraints at a time
+    B2S_TRY(val.alloc(c, N * sizeof(Fr)));
+    B2S_TRY(nonone.alloc(c, N * 4));
+    Stager st(c);
+    const uint64_t n_spans = w.cut.size() - 1;
+    B2S_TRY(st.spans(sec, w.cut.data(), n_spans, [&](const uint8_t* src, uint64_t j) -> int32_t {
+        R1csSpan sp{w.row[j], w.row[j + 1], w.cut[j], {}, {}};
+        for (int k = 0; k < 3; k++) {
+            sp.first[k] = w.first[3 * j + k];
+            sp.n[k] = (uint32_t)(w.first[3 * (j + 1) + k] - sp.first[k]);
+        }
+        const uint64_t n = (uint64_t)sp.n[0] + sp.n[1] + sp.n[2];
+        if (n)
+            B2S_LAUNCH(c, r1cs_entry_kernel<Curve>, cdiv(n, 256), 256, 0, src, sp, o, (uint32_t)f.info.n_wires, val.as<Fr>(),
+                       nonone.as<uint32_t>(), st.err.as<unsigned long long>());
+        return B2S_OK;
+    }));
+    unsigned long long word = ~0ull;
+    B2S_TRY(st.read_err(&word));
+    if (word != ~0ull) {
+        const uint64_t i = (word >> 34) / 3, j = (word >> 2) & 0xFFFFFFFFull;
+        const uint32_t k = (uint32_t)((word >> 34) % 3);
+        if ((word & 3) == EN_VALUE)
+            return fail(c, B2S_ERR_INVALID_DATA, "r1cs constraint %llu %c[%llu]: coefficient not below r", (unsigned long long)i, MATRIX_NAME[k],
+                        (unsigned long long)j);
+        uint64_t at = 0;   // the entry's byte in the section, for the wire in the message
+        for (uint64_t q = 0; q < i; q++) at += 12 + (uint64_t)R1CS_ENTRY * (w.counts[q] + w.counts[M + q] + w.counts[2 * M + q]);
+        for (uint32_t q = 0; q < k; q++) at += 4 + (uint64_t)R1CS_ENTRY * w.counts[q * M + i];
+        at += 4 + (uint64_t)R1CS_ENTRY * j;
+        return fail(c, B2S_ERR_INVALID_DATA, "r1cs constraint %llu %c[%llu]: wire %u not below nWires %llu", (unsigned long long)i, MATRIX_NAME[k],
+                    (unsigned long long)j, rd32(sec + at), (unsigned long long)f.info.n_wires);
+    }
+    // pool slots of the entries other than ONE, compacted by a scan
+    uint32_t n_pool = 0;
+    if (N) {
+        B2S_TRY(pool_off.alloc(c, (N + 1) * 4));
+        B2S_TRY(task2.alloc(c, (N + 1) * 4));
+        B2S_TRY(scan_counts(c, nonone.as<uint32_t>(), (uint32_t)N, 1u, pool_off.as<uint32_t>(), task2.as<uint32_t>()));
+        B2S_CUDA(c, cudaMemcpyAsync(&n_pool, pool_off.as<uint32_t>() + N, 4, cudaMemcpyDeviceToHost, c->stream));
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+    }
+    m->pool_size = n_pool + 1;
+    B2S_TRY(m->pool.alloc(c, (size_t)m->pool_size * sizeof(Fr)));
+    B2S_LAUNCH(c, r1cs_place_kernel<Fr>, cdiv(std::max<uint64_t>(N, 1), 256), 256, 0, N, o, (const Fr*)val.as<Fr>(),
+               (const uint32_t*)nonone.as<uint32_t>(), (const uint32_t*)pool_off.as<uint32_t>(), m->pool.as<Fr>());
+    B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+    return B2S_OK;
+}
+
 }  // namespace
 
 int32_t zkey_read_info(Ctx* c, const uint8_t* in, uint64_t len, b2s_zkey_info* out) {
@@ -445,6 +731,29 @@ int32_t wtns_read(Ctx* c, const uint8_t* in, uint64_t len, uint64_t n_vars, int3
     if (word != ~0ull)
         return fail(c, B2S_ERR_INVALID_DATA, "wtns[%llu]: %s", word >> 3, (word & 7) == 1 ? "value not below r" : "z[0] is not 1");
     return z.finish(c);
+}
+
+int32_t r1cs_file_read_info(Ctx* c, const uint8_t* in, uint64_t len, b2s_r1cs_file_info* out) {
+    R1csFile f;
+    B2S_TRY(r1cs_parse(c, in, len, f));
+    *out = f.info;
+    return B2S_OK;
+}
+
+int32_t r1cs_file_load(Ctx* c, const uint8_t* in, uint64_t len, b2s_r1cs** out) {
+    R1csFile f;
+    B2S_TRY(r1cs_parse(c, in, len, f));
+    R1csWalk w;
+    const Section& sec = f.s[R_CONSTRAINTS];
+    B2S_TRY(r1cs_walk(c, in + sec.off, sec.size, f.info.n_constraints, w));
+    b2s_r1cs* m = new b2s_r1cs();
+    const int32_t s = dispatch_curve(c, [&](auto curve) { return r1cs_matrices<decltype(curve)>(c, in + sec.off, f, w, m); });
+    if (s != B2S_OK) {
+        delete m;
+        return s;
+    }
+    *out = m;
+    return B2S_OK;
 }
 
 }  // namespace b2s

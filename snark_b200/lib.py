@@ -49,6 +49,10 @@ class ZkeyInfo(ctypes.Structure):
     _fields_ = [("n_vars", c_uint64), ("n_public", c_uint64), ("domain_size", c_uint64), ("n_coeffs", c_uint64)]
 
 
+class R1csFileInfo(ctypes.Structure):
+    _fields_ = [(n, c_uint64) for n in ("n_wires", "n_pub_out", "n_pub_in", "n_prv_in", "n_labels", "n_constraints", "domain_size")]
+
+
 class PredicateDesc(ctypes.Structure):
     _fields_ = [
         ("arity", c_uint32), ("n_terms", c_uint32),
@@ -152,6 +156,8 @@ SIGNATURES = {
     "b2s_zkey_read_info": (c_int32, [c_void_p, c_void_p, c_uint64, POINTER(ZkeyInfo)]),
     "b2s_zkey_load": (c_int32, [c_void_p, c_void_p, c_uint64, c_int32, POINTER(c_void_p), POINTER(c_void_p)] + [c_void_p] * 5 + [c_uint64]),
     "b2s_wtns_read": (c_int32, [c_void_p, c_void_p, c_uint64, c_uint64, c_int32, c_void_p]),
+    "b2s_r1cs_file_read_info": (c_int32, [c_void_p, c_void_p, c_uint64, POINTER(R1csFileInfo)]),
+    "b2s_r1cs_file_load": (c_int32, [c_void_p, c_void_p, c_uint64, POINTER(c_void_p)]),
     "b2s_vk_prepare": (c_int32, [c_void_p] * 6 + [c_uint64, POINTER(c_void_p)]),
     "b2s_pvk_free": (None, [c_void_p, c_void_p]),
     "b2s_groth16_verify_batch": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p, c_int32,
@@ -599,7 +605,7 @@ class Backend:
     def pk_free(self, pk):
         self.lib.b2s_pk_free(self.h, pk)
 
-    # ---- snarkjs files (.zkey / .wtns) --------------------------------------------------------------------------------
+    # ---- snarkjs and circom files (.zkey / .wtns / .r1cs) ------------------------------------------------------------
     @staticmethod
     def _file_bytes(data):
         """bytes-like or numpy array (an np.memmap of the file included) -> a uint8 view of the same memory, not a copy"""
@@ -637,6 +643,24 @@ class Backend:
         po, mem = _ptr(out)
         self._ck(self.lib.b2s_wtns_read(self.h, buf.ctypes.data, buf.nbytes, n_vars, mem, po))
         return out
+
+    def r1cs_file_info(self, data):
+        """Header of a circom .r1cs (bytes, or a numpy array / np.memmap of the file): {n_wires, n_pub_out, n_pub_in, n_prv_in,
+        n_labels, n_constraints, domain_size}."""
+        buf = self._file_bytes(data)
+        info = R1csFileInfo()
+        self._ck(self.lib.b2s_r1cs_file_read_info(self.h, buf.ctypes.data, buf.nbytes, ctypes.byref(info)))
+        return {name: int(getattr(info, name)) for name, _ in R1csFileInfo._fields_}
+
+    def r1cs_file_load(self, data):
+        """A circom .r1cs (bytes, or a numpy array / np.memmap of the file) -> the matrix handle r1cs_upload builds from the
+        same A, B, C (n_instance = 1 + n_pub_out + n_pub_in), checked and decoded on the GPU."""
+        buf = self._file_bytes(data)
+        info = self.r1cs_file_info(buf)
+        m = c_void_p()
+        self._ck(self.lib.b2s_r1cs_file_load(self.h, buf.ctypes.data, buf.nbytes, ctypes.byref(m)))
+        self._r1cs_vars[m.value] = info["n_wires"]
+        return m
 
     # ---- verification (pairings in CUDA) ----------------------------------------------------------------------------
     def vk_prepare(self, vk):
