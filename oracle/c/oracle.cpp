@@ -10,6 +10,7 @@
 //   ntt           ark-poly Radix2EvaluationDomain::{fft,ifft}_in_place, coset                        A.3
 //   spmv          relations/src/utils/matrix.rs:26-36 (mat_vec_mul), sr1cs/mod.rs:24-56 (skip coeff == 1)
 //   witness_map   ark-groth16 LibsnarkReduction                                                       A.2
+//   witness_map_circom  ark-circom CircomReduction (odd-coset evaluations)                      DESIGN.md §3.6
 //   prove         ark-groth16 create_proof_with_assignment                                            A.1
 // It is validated against the pure-Python oracle (tests/test_oracle_c.py) which in turn is pinned by
 // the definitions (naive DFT, double-and-add) and the known-trapdoor Groth16 check.
@@ -149,9 +150,11 @@ static void init_params(Params<N>& P, const u64* modulus) {
     }
 }
 
-template <class B>
+// Fp2 = B[u] / (u^2 + K): u^2 = -1 (K = 1) for BLS12-381 and BN254, u^2 = -5 (K = 5) for BLS12-377.  Schoolbook product.
+template <class B, int K = 1>
 struct Fp2 {
     B c0, c1;
+    static B times_k(const B& x) { B r = x; for (int i = 1; i < K; i++) r = r + x; return r; }
     static Fp2 zero() { return {B::zero(), B::zero()}; }
     static Fp2 one() { return {B::one(), B::zero()}; }
     bool is_zero() const { return c0.is_zero() && c1.is_zero(); }
@@ -159,11 +162,11 @@ struct Fp2 {
     bool operator!=(const Fp2& o) const { return !(*this == o); }
     Fp2 operator+(const Fp2& o) const { return {c0 + o.c0, c1 + o.c1}; }
     Fp2 operator-(const Fp2& o) const { return {c0 - o.c0, c1 - o.c1}; }
-    Fp2 operator*(const Fp2& o) const { return {c0 * o.c0 - c1 * o.c1, c0 * o.c1 + c1 * o.c0}; }  // u^2 = -1
+    Fp2 operator*(const Fp2& o) const { return {c0 * o.c0 - times_k(c1 * o.c1), c0 * o.c1 + c1 * o.c0}; }
     Fp2 sqr() const { return *this * *this; }
     Fp2 neg() const { return {c0.neg(), c1.neg()}; }
     Fp2 dbl() const { return {c0.dbl(), c1.dbl()}; }
-    Fp2 inverse() const { B n = (c0.sqr() + c1.sqr()).inverse(); return {c0 * n, (c1 * n).neg()}; }
+    Fp2 inverse() const { B n = (c0.sqr() + times_k(c1.sqr())).inverse(); return {c0 * n, (c1 * n).neg()}; }
 };
 
 // ------------------------------------------------------------------------------------------------
@@ -338,26 +341,36 @@ static void ntt_inplace(Fr* a, int log_n, const Fr& w_n, int threads) {
     }
 }
 
+// a[i] *= c0 * base^i, i < n
+template <class Fr>
+static void scale_pow(Fr* a, size_t n, const Fr& base, const Fr& c0, int threads) {
+    const int T = (int)std::max<size_t>(1, std::min<size_t>(threads, n / 4096 + 1));
+    run_parallel(T, T, [&](int t) {
+        size_t lo = n * t / T, hi = n * (t + 1) / T;
+        Fr cur = c0 * base.pow64(lo);
+        for (size_t i = lo; i < hi; i++) { a[i] = a[i] * cur; cur = cur * base; }
+    });
+}
+
+// primitive 2^log_n-th root of unity
+template <class Fr>
+static Fr root_of_unity(const FrConsts<Fr>& K, int log_n) {
+    Fr w = K.root;
+    for (int i = log_n; i < K.two_adicity; i++) w = w.sqr();
+    return w;
+}
+
 template <class Fr>
 static void ntt_full(Fr* a, int log_n, bool inverse, bool coset, const FrConsts<Fr>& K, int threads) {
     const size_t n = (size_t)1 << log_n;
-    Fr w = K.root;
-    for (int i = log_n; i < K.two_adicity; i++) w = w.sqr();
-    auto scale_pow = [&](const Fr& base, const Fr& c0) {
-        const int T = (int)std::max<size_t>(1, std::min<size_t>(threads, n / 4096 + 1));
-        run_parallel(T, T, [&](int t) {
-            size_t lo = n * t / T, hi = n * (t + 1) / T;
-            Fr cur = c0 * base.pow64(lo);
-            for (size_t i = lo; i < hi; i++) { a[i] = a[i] * cur; cur = cur * base; }
-        });
-    };
+    const Fr w = root_of_unity(K, log_n);
     if (!inverse) {
-        if (coset) scale_pow(K.gen, Fr::one());
+        if (coset) scale_pow(a, n, K.gen, Fr::one(), threads);
         ntt_inplace(a, log_n, w, threads);
     } else {
         ntt_inplace(a, log_n, w.inverse(), threads);
         Fr ninv = Fr::from_u64(n).inverse();
-        scale_pow(coset ? K.gen.inverse() : Fr::one(), ninv);
+        scale_pow(a, n, coset ? K.gen.inverse() : Fr::one(), ninv, threads);
     }
 }
 
@@ -400,6 +413,28 @@ static void witness_map(const Csr mats[3], size_t n_rows, size_t n_inst, const F
     ntt_full(h, log_dom, true, true, K, threads);
 }
 
+// ark-circom CircomReduction::witness_map_from_matrices (DESIGN.md §3.6): a = A z with the instance rows copied in, b = B z,
+// c = a o b on H; each of a, b, c interpolated, its k-th coefficient multiplied by w2^k (w2 the primitive 2N-th root, so
+// that the next transform evaluates at x_j = w2 w^j, the odd coset) and transformed; h = a b - c there.  C is not read.
+template <class Fr>
+static void witness_map_circom(const Csr mats[3], size_t n_rows, size_t n_inst, const Fr* z, int log_dom, Fr* h,
+                               const FrConsts<Fr>& K, int threads) {
+    const size_t N = (size_t)1 << log_dom;
+    std::vector<Fr> b(N, Fr::zero()), c(N);
+    for (size_t i = 0; i < N; i++) h[i] = Fr::zero();
+    spmv(mats[0], z, h, n_rows, threads);
+    spmv(mats[1], z, b.data(), n_rows, threads);
+    for (size_t i = 0; i < n_inst; i++) h[n_rows + i] = z[i];
+    for (size_t i = 0; i < N; i++) c[i] = h[i] * b[i];
+    const Fr w2 = root_of_unity(K, log_dom + 1);
+    for (Fr* p : {h, b.data(), c.data()}) {
+        ntt_full(p, log_dom, true, false, K, threads);
+        scale_pow(p, N, w2, Fr::one(), threads);
+        ntt_full(p, log_dom, false, false, K, threads);
+    }
+    for (size_t i = 0; i < N; i++) h[i] = h[i] * b[i] - c[i];
+}
+
 // ------------------------------------------------------------------------------------------------
 static void run_parallel(int threads, int jobs, const std::function<void(int)>& fn) {
     if (threads <= 1 || jobs <= 1) { for (int j = 0; j < jobs; j++) fn(j); return; }
@@ -425,9 +460,23 @@ typedef Fp<6, 0> BlsFq;
 typedef Fp<4, 1> BlsFr;
 typedef Fp<4, 2> BnFq;
 typedef Fp<4, 3> BnFr;
+typedef Fp<6, 4> Bls377Fq;
+typedef Fp<4, 5> Bls377Fr;
 static FrConsts<BlsFr> g_bls_fr;
 static FrConsts<BnFr> g_bn_fr;
+static FrConsts<Bls377Fr> g_bls377_fr;
 static bool g_init = false;
+
+// K.root = gen^((r-1)/2^S), S the two-adicity of r - 1 (S < 64)
+template <class Fr>
+static void init_fr_consts(FrConsts<Fr>& K, const u64* r, u64 gen, int S) {
+    K.gen = Fr::from_u64(gen);
+    K.two_adicity = S;
+    u64 e[4], one[4] = {1, 0, 0, 0};
+    sub_n<4>(e, r, one);
+    for (int i = 0; i < 4; i++) e[i] = (e[i] >> S) | (i + 1 < 4 ? e[i + 1] << (64 - S) : 0);
+    K.root = K.gen.pow(e, 4);
+}
 
 static void init_all() {
     if (g_init) return;
@@ -435,29 +484,45 @@ static void init_all() {
     const u64 bls_r[4] = {0xffffffff00000001ull, 0x53bda402fffe5bfeull, 0x3339d80809a1d805ull, 0x73eda753299d7d48ull};
     const u64 bn_p[4] = {0x3c208c16d87cfd47ull, 0x97816a916871ca8dull, 0xb85045b68181585dull, 0x30644e72e131a029ull};
     const u64 bn_r[4] = {0x43e1f593f0000001ull, 0x2833e84879b97091ull, 0xb85045b68181585dull, 0x30644e72e131a029ull};
+    // BLS12-377: the published moduli, p = (x - 1)^2 r / 3 + x and r = x^4 - x^2 + 1 for x = 0x8508c00000000001
+    const u64 bls377_p[6] = {0x8508c00000000001ull, 0x170b5d4430000000ull, 0x1ef3622fba094800ull, 0x1a22d9f300f5138full, 0xc63b05c06ca1493bull, 0x01ae3a4617c510eaull};
+    const u64 bls377_r[4] = {0x0a11800000000001ull, 0x59aa76fed0000001ull, 0x60b44d1e5c37b001ull, 0x12ab655e9a2ca556ull};
     init_params<6>(BlsFq::P, bls_p);
     init_params<4>(BlsFr::P, bls_r);
     init_params<4>(BnFq::P, bn_p);
     init_params<4>(BnFr::P, bn_r);
-    {   // root = gen^((r-1)/2^S)
-        g_bls_fr.gen = BlsFr::from_u64(7); g_bls_fr.two_adicity = 32;
-        u64 e[4], one[4] = {1, 0, 0, 0};
-        sub_n<4>(e, bls_r, one);
-        for (int i = 0; i < 4; i++) e[i] = (e[i] >> 32) | (i + 1 < 4 ? e[i + 1] << 32 : 0);
-        g_bls_fr.root = g_bls_fr.gen.pow(e, 4);
-        g_bn_fr.gen = BnFr::from_u64(5); g_bn_fr.two_adicity = 28;
-        sub_n<4>(e, bn_r, one);
-        for (int i = 0; i < 4; i++) e[i] = (e[i] >> 28) | (i + 1 < 4 ? e[i + 1] << 36 : 0);
-        g_bn_fr.root = g_bn_fr.gen.pow(e, 4);
-    }
+    init_params<6>(Bls377Fq::P, bls377_p);
+    init_params<4>(Bls377Fr::P, bls377_r);
+    init_fr_consts(g_bls_fr, bls_r, 7, 32);
+    init_fr_consts(g_bn_fr, bn_r, 5, 28);
+    init_fr_consts(g_bls377_fr, bls377_r, 22, 47);
     g_init = true;
 }
 
-template <class Fq, class Fr>
-static void prove_t(const FrConsts<Fr>& K, int num_bits, const Csr mats[3], size_t n_rows, size_t n_inst, size_t n_wit,
-                    const void* const* pk, const Fr* z_inst, const Fr* z_wit, const Fr* r, const Fr* s, void* out_a,
-                    void* out_b, void* out_c, void* out_h, int threads) {
-    typedef Fp2<Fq> Fq2;
+// One struct per curve id, for the dispatch of the exported functions
+struct Bls12_381 { typedef BlsFq Fq; typedef Fp2<BlsFq> Fq2; typedef BlsFr Fr; static constexpr int bits = 255; static const FrConsts<Fr>& K() { return g_bls_fr; } };
+struct Bn254 { typedef BnFq Fq; typedef Fp2<BnFq> Fq2; typedef BnFr Fr; static constexpr int bits = 254; static const FrConsts<Fr>& K() { return g_bn_fr; } };
+struct Bls12_377 { typedef Bls377Fq Fq; typedef Fp2<Bls377Fq, 5> Fq2; typedef Bls377Fr Fr; static constexpr int bits = 253; static const FrConsts<Fr>& K() { return g_bls377_fr; } };
+
+// fn(curve struct) for curve id 0 / 1 / 2 -> 0, or 1 for an unknown id
+template <class Fn>
+static int with_curve(int curve, Fn&& fn) {
+    init_all();
+    switch (curve) {
+        case 0: fn(Bls12_381()); return 0;
+        case 1: fn(Bn254()); return 0;
+        case 2: fn(Bls12_377()); return 0;
+        default: return 1;
+    }
+}
+
+template <class C>
+static void prove_t(const Csr mats[3], size_t n_rows, size_t n_inst, size_t n_wit, const void* const* pk,
+                    const typename C::Fr* z_inst, const typename C::Fr* z_wit, const typename C::Fr* r, const typename C::Fr* s,
+                    void* out_a, void* out_b, void* out_c, void* out_h, int threads) {
+    typedef typename C::Fq Fq; typedef typename C::Fq2 Fq2; typedef typename C::Fr Fr;
+    const FrConsts<Fr>& K = C::K();
+    const int num_bits = C::bits;
     typedef Aff<Fq> A1; typedef Aff<Fq2> A2; typedef Jac<Fq> J1; typedef Jac<Fq2> J2;
     // pk pointers: alpha_g1, beta_g1, delta_g1, beta_g2, delta_g2, a_query, b_g1_query, b_g2_query, h_query, l_query
     const A1 *alpha = (const A1*)pk[0], *beta1 = (const A1*)pk[1], *delta1 = (const A1*)pk[2];
@@ -512,31 +577,29 @@ int orc_threads_default() { unsigned h = std::thread::hardware_concurrency(); re
 
 // group: 1 / 2; scalars Montgomery (mont = 1) or canonical; out: one affine point
 int orc_msm(int curve, int group, const void* bases, const void* scalars, uint64_t n, int mont, int threads, void* out) {
-    init_all();
-    if (curve == 0 && group == 1) { auto r = msm<BlsFq, BlsFr>((const Aff<BlsFq>*)bases, (const BlsFr*)scalars, n, mont, threads, 255).to_affine(); memcpy(out, &r, sizeof(r)); }
-    else if (curve == 0 && group == 2) { auto r = msm<Fp2<BlsFq>, BlsFr>((const Aff<Fp2<BlsFq>>*)bases, (const BlsFr*)scalars, n, mont, threads, 255).to_affine(); memcpy(out, &r, sizeof(r)); }
-    else if (curve == 1 && group == 1) { auto r = msm<BnFq, BnFr>((const Aff<BnFq>*)bases, (const BnFr*)scalars, n, mont, threads, 254).to_affine(); memcpy(out, &r, sizeof(r)); }
-    else if (curve == 1 && group == 2) { auto r = msm<Fp2<BnFq>, BnFr>((const Aff<Fp2<BnFq>>*)bases, (const BnFr*)scalars, n, mont, threads, 254).to_affine(); memcpy(out, &r, sizeof(r)); }
-    else return 1;
-    return 0;
+    if (group != 1 && group != 2) return 1;
+    return with_curve(curve, [&](auto c) {
+        typedef decltype(c) C;
+        typedef typename C::Fr Fr;
+        if (group == 1) { auto r = msm<typename C::Fq, Fr>((const Aff<typename C::Fq>*)bases, (const Fr*)scalars, n, mont, threads, C::bits).to_affine(); memcpy(out, &r, sizeof(r)); }
+        else { auto r = msm<typename C::Fq2, Fr>((const Aff<typename C::Fq2>*)bases, (const Fr*)scalars, n, mont, threads, C::bits).to_affine(); memcpy(out, &r, sizeof(r)); }
+    });
 }
 
 int orc_ntt(int curve, void* data, int log_n, int inverse, int coset, int threads) {
-    init_all();
-    if (curve == 0) ntt_full((BlsFr*)data, log_n, inverse, coset, g_bls_fr, threads);
-    else if (curve == 1) ntt_full((BnFr*)data, log_n, inverse, coset, g_bn_fr, threads);
-    else return 1;
-    return 0;
+    return with_curve(curve, [&](auto c) {
+        typedef decltype(c) C;
+        ntt_full((typename C::Fr*)data, log_n, inverse, coset, C::K(), threads);
+    });
 }
 
 int orc_spmv(int curve, const uint64_t* row_ptr, const uint32_t* col, const void* coeff, uint64_t n_rows, const void* z,
              void* out, int threads) {
-    init_all();
     Csr m{row_ptr, col, coeff};
-    if (curve == 0) spmv(m, (const BlsFr*)z, (BlsFr*)out, n_rows, threads);
-    else if (curve == 1) spmv(m, (const BnFr*)z, (BnFr*)out, n_rows, threads);
-    else return 1;
-    return 0;
+    return with_curve(curve, [&](auto c) {
+        typedef typename decltype(c)::Fr Fr;
+        spmv(m, (const Fr*)z, (Fr*)out, n_rows, threads);
+    });
 }
 
 // pk: 10 pointers (see prove_t).  out_h may be null.
@@ -544,46 +607,61 @@ int orc_groth16_prove(int curve, const uint64_t* const row_ptr[3], const uint32_
                       uint64_t n_rows, uint64_t n_inst, uint64_t n_wit, const void* const* pk, const void* z_inst,
                       const void* z_wit, const void* r, const void* s, void* out_a, void* out_b, void* out_c, void* out_h,
                       int threads) {
-    init_all();
     Csr mats[3];
     for (int k = 0; k < 3; k++) mats[k] = Csr{row_ptr[k], col[k], coeff[k]};
-    if (curve == 0) prove_t<BlsFq, BlsFr>(g_bls_fr, 255, mats, n_rows, n_inst, n_wit, pk, (const BlsFr*)z_inst, (const BlsFr*)z_wit, (const BlsFr*)r, (const BlsFr*)s, out_a, out_b, out_c, out_h, threads);
-    else if (curve == 1) prove_t<BnFq, BnFr>(g_bn_fr, 254, mats, n_rows, n_inst, n_wit, pk, (const BnFr*)z_inst, (const BnFr*)z_wit, (const BnFr*)r, (const BnFr*)s, out_a, out_b, out_c, out_h, threads);
-    else return 1;
-    return 0;
+    return with_curve(curve, [&](auto c) {
+        typedef decltype(c) C;
+        typedef typename C::Fr Fr;
+        prove_t<C>(mats, n_rows, n_inst, n_wit, pk, (const Fr*)z_inst, (const Fr*)z_wit, (const Fr*)r, (const Fr*)s, out_a, out_b,
+                   out_c, out_h, threads);
+    });
 }
 
 // h = witness_map(A, B, C, z) alone (SpMV + 7 transforms + quotient), z = instance || witness: the full-size parity
 // tests compare the GPU's h with it element by element (2^24 / 2^25 domains take seconds on the host cores)
 int orc_witness_map(int curve, const uint64_t* const row_ptr[3], const uint32_t* const col[3], const void* const coeff[3],
                     uint64_t n_rows, uint64_t n_inst, const void* z, int log_dom, void* out_h, int threads) {
-    init_all();
     Csr mats[3];
     for (int k = 0; k < 3; k++) mats[k] = Csr{row_ptr[k], col[k], coeff[k]};
-    if (curve == 0) witness_map(mats, n_rows, n_inst, (const BlsFr*)z, log_dom, (BlsFr*)out_h, g_bls_fr, threads);
-    else if (curve == 1) witness_map(mats, n_rows, n_inst, (const BnFr*)z, log_dom, (BnFr*)out_h, g_bn_fr, threads);
-    else return 1;
-    return 0;
+    return with_curve(curve, [&](auto c) {
+        typedef decltype(c) C;
+        typedef typename C::Fr Fr;
+        witness_map(mats, n_rows, n_inst, (const Fr*)z, log_dom, (Fr*)out_h, C::K(), threads);
+    });
+}
+
+// the CircomReduction's h (N odd-coset evaluations, see witness_map_circom) for the same arguments; C is not read
+int orc_witness_map_circom(int curve, const uint64_t* const row_ptr[3], const uint32_t* const col[3], const void* const coeff[3],
+                           uint64_t n_rows, uint64_t n_inst, const void* z, int log_dom, void* out_h, int threads) {
+    Csr mats[3];
+    for (int k = 0; k < 3; k++) mats[k] = Csr{row_ptr[k], col[k], coeff[k]};
+    return with_curve(curve, [&](auto c) {
+        typedef decltype(c) C;
+        typedef typename C::Fr Fr;
+        witness_map_circom(mats, n_rows, n_inst, (const Fr*)z, log_dom, (Fr*)out_h, C::K(), threads);
+    });
 }
 
 // out[i] = (start + i) * gen, affine
 int orc_multiples(int curve, int group, const void* gen, uint64_t start, uint64_t n, void* out, int threads) {
-    init_all();
-    if (curve == 0 && group == 1) multiples_t((const Aff<BlsFq>*)gen, start, n, (Aff<BlsFq>*)out, threads);
-    else if (curve == 0 && group == 2) multiples_t((const Aff<Fp2<BlsFq>>*)gen, start, n, (Aff<Fp2<BlsFq>>*)out, threads);
-    else if (curve == 1 && group == 1) multiples_t((const Aff<BnFq>*)gen, start, n, (Aff<BnFq>*)out, threads);
-    else if (curve == 1 && group == 2) multiples_t((const Aff<Fp2<BnFq>>*)gen, start, n, (Aff<Fp2<BnFq>>*)out, threads);
-    else return 1;
-    return 0;
+    if (group != 1 && group != 2) return 1;
+    return with_curve(curve, [&](auto c) {
+        typedef decltype(c) C;
+        typedef typename C::Fq Fq; typedef typename C::Fq2 Fq2;
+        if (group == 1) multiples_t((const Aff<Fq>*)gen, start, n, (Aff<Fq>*)out, threads);
+        else multiples_t((const Aff<Fq2>*)gen, start, n, (Aff<Fq2>*)out, threads);
+    });
 }
 
 // sum_i a[i] * b[i] over Fr (Montgomery in, Montgomery out): used by full-size parity checks
 int orc_fr_dot(int curve, const void* a, const void* b, uint64_t n, void* out) {
-    init_all();
-    if (curve == 0) { BlsFr acc = BlsFr::zero(); const BlsFr *x = (const BlsFr*)a, *y = (const BlsFr*)b; for (uint64_t i = 0; i < n; i++) acc = acc + x[i] * y[i]; memcpy(out, &acc, 32); }
-    else if (curve == 1) { BnFr acc = BnFr::zero(); const BnFr *x = (const BnFr*)a, *y = (const BnFr*)b; for (uint64_t i = 0; i < n; i++) acc = acc + x[i] * y[i]; memcpy(out, &acc, 32); }
-    else return 1;
-    return 0;
+    return with_curve(curve, [&](auto c) {
+        typedef typename decltype(c)::Fr Fr;
+        Fr acc = Fr::zero();
+        const Fr *x = (const Fr*)a, *y = (const Fr*)b;
+        for (uint64_t i = 0; i < n; i++) acc = acc + x[i] * y[i];
+        memcpy(out, &acc, 32);
+    });
 }
 
 }  // extern "C"

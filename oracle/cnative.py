@@ -27,6 +27,7 @@ def load(build=True):
                                           c_uint64, POINTER(c_void_p)] + [c_void_p] * 8 + [c_int]
         lib.orc_witness_map.argtypes = [c_int, POINTER(c_void_p), POINTER(c_void_p), POINTER(c_void_p), c_uint64, c_uint64, c_void_p, c_int,
                                         c_void_p, c_int]
+        lib.orc_witness_map_circom.argtypes = lib.orc_witness_map.argtypes
         lib.orc_multiples.argtypes = [c_int, c_int, c_void_p, c_uint64, c_uint64, c_void_p, c_int]
         lib.orc_fr_dot.argtypes = [c_int, c_void_p, c_void_p, c_uint64, c_void_p]
         _lib = lib
@@ -50,8 +51,11 @@ def _p(a):
     return a.ctypes.data if a is not None else None
 
 
+FQ_WORDS = {0: 12, 1: 8, 2: 12}   # 32-bit words of one Fq element: BLS12-381, BN254, BLS12-377
+
+
 def msm(curve_id, group, bases, scalars, n, mont=True, threads=None):
-    fq = 12 if curve_id == 0 else 8
+    fq = FQ_WORDS[curve_id]
     out = np.zeros(2 * group * fq, dtype=np.uint32)
     rc = load().orc_msm(curve_id, group, _p(bases), _p(scalars), n, int(mont), threads or threads_default(), _p(out))
     assert rc == 0
@@ -73,7 +77,7 @@ def spmv(curve_id, csr, z, n_rows, threads=None):
 
 def groth16_prove(curve_id, csr3, n_rows, n_inst, n_wit, pk_arrays, z_inst, z_wit, r, s, want_h=False, threads=None):
     """pk_arrays: [alpha_g1, beta_g1, delta_g1, beta_g2, delta_g2, a_query, b_g1_query, b_g2_query, h_query, l_query]."""
-    fq = 12 if curve_id == 0 else 8
+    fq = FQ_WORDS[curve_id]
     rp = (c_void_p * 3)(*[_p(m[0]) for m in csr3])
     col = (c_void_p * 3)(*[_p(m[1]) for m in csr3])
     co = (c_void_p * 3)(*[_p(m[2]) for m in csr3])
@@ -90,20 +94,29 @@ def groth16_prove(curve_id, csr3, n_rows, n_inst, n_wit, pk_arrays, z_inst, z_wi
     return a, b, c, h
 
 
-def witness_map(curve_id, csr3, n_rows, n_inst, z, threads=None):
-    """h of the LibsnarkReduction (SURVEY App. A.2) for z = instance || witness; domain = next_pow2(n_rows + n_inst)."""
+def _witness_map(fn, curve_id, csr3, n_rows, n_inst, z, threads):
     rp = (c_void_p * 3)(*[_p(m[0]) for m in csr3])
     col = (c_void_p * 3)(*[_p(m[1]) for m in csr3])
     co = (c_void_p * 3)(*[_p(m[2]) for m in csr3])
     log_dom = max((n_rows + n_inst - 1).bit_length(), 0)
     h = np.zeros((1 << log_dom) * 8, dtype=np.uint32)
-    rc = load().orc_witness_map(curve_id, rp, col, co, n_rows, n_inst, _p(z), log_dom, _p(h), threads or threads_default())
+    rc = fn(curve_id, rp, col, co, n_rows, n_inst, _p(z), log_dom, _p(h), threads or threads_default())
     assert rc == 0
     return h
 
 
+def witness_map(curve_id, csr3, n_rows, n_inst, z, threads=None):
+    """h of the LibsnarkReduction (SURVEY App. A.2) for z = instance || witness; domain = next_pow2(n_rows + n_inst)."""
+    return _witness_map(load().orc_witness_map, curve_id, csr3, n_rows, n_inst, z, threads)
+
+
+def witness_map_circom(curve_id, csr3, n_rows, n_inst, z, threads=None):
+    """h of the CircomReduction (DESIGN.md §3.6): N evaluations on the odd coset w2 H, same arguments and domain."""
+    return _witness_map(load().orc_witness_map_circom, curve_id, csr3, n_rows, n_inst, z, threads)
+
+
 def multiples(curve_id, group, gen, start, n, threads=None):
-    fq = 12 if curve_id == 0 else 8
+    fq = FQ_WORDS[curve_id]
     out = np.zeros(n * 2 * group * fq, dtype=np.uint32)
     rc = load().orc_multiples(curve_id, group, _p(gen), start, n, _p(out), threads or threads_default())
     assert rc == 0

@@ -6,13 +6,11 @@ import random
 import numpy as np
 import pytest
 
-from oracle import cnative
 from oracle import groth16 as og
 from oracle import r1cs as orc
-from oracle.ec import groups
 from oracle.params import BLS12_381, BN254
 from tests import circom_oracle as oc
-from tests.util import csr_from_rows, make_pk_desc, pack_fr, random_fr_limbs, unpack_fr, unpack_points
+from tests.util import csr_from_rows, known_log_key, known_log_proof, make_pk_desc, pack_fr, random_fr_limbs, unpack_fr, unpack_points
 
 pytestmark = pytest.mark.gpu
 CURVES = [BLS12_381, BN254]
@@ -176,51 +174,18 @@ def test_full_size_bls12_381_known_discrete_logs():
     """Synthetic circom key k_j G at domain 2^24: A, B, C are the multiples of G predicted from z, h and the k_j; h equals
     -2 times the libsnark h evaluated on the odd coset, computed with b2s_witness_map, b2s_poly_geom, b2s_poly_op and
     b2s_ntt."""
-    import torch
-
     from snark_b200 import Backend
-    from snark_b200.lib import MEM_DEVICE, MEM_HOST, PkDesc
+    from snark_b200.lib import MEM_HOST
 
     curve, cid, log_n = BLS12_381, 0, 24
     r = curve.r
     N = 1 << log_n
     rng = random.Random(0x24C)
     csr, n_rows, n_inst, n_wit, z_inst, z_wit = dummy_2k(curve, log_n)
-    n_vars = n_inst + n_wit
     rr, ss = rng.randrange(r), rng.randrange(r)
     be = Backend(curve=cid)
-    dev = torch.device("cuda", 0)
-    gen = torch.Generator(device=dev)
-    gen.manual_seed(4321)
-
-    def query(group, n):
-        k = torch.randint(-(1 << 31), (1 << 31) - 1, (n, 8), dtype=torch.int32, device=dev, generator=gen)
-        k[:, 7] &= 0x1FFFFFFF
-        out = torch.empty(n * (be.g1_bytes if group == 1 else be.g2_bytes) // 4, dtype=torch.int32, device=dev)
-        be.fixed_base(group, k, n, mont=False, out=out)
-        be.sync()
-        return out, k.cpu().numpy().view(np.uint32).reshape(-1)
-
     consts = [rng.randrange(1, r) for _ in range(3)]
-    c1 = be.fixed_base(1, pack_fr(curve, consts, mont=False), 3, mont=False)
-    c2 = be.fixed_base(2, pack_fr(curve, consts[1:], mont=False), 2, mont=False)
-    g1w, g2w = be.g1_bytes // 4, be.g2_bytes // 4
-    c1t = torch.from_numpy(c1.view(np.int32)).to(dev)
-    c2t = torch.from_numpy(c2.view(np.int32)).to(dev)
-    d = PkDesc()
-    d.n_instance, d.n_witness, d.domain_size = n_inst, n_wit, N
-    d.alpha_g1, d.beta_g1, d.delta_g1 = c1t.data_ptr(), c1t.data_ptr() + 4 * g1w, c1t.data_ptr() + 8 * g1w
-    d.beta_g2, d.delta_g2 = c2t.data_ptr(), c2t.data_ptr() + 4 * g2w
-    keep, dl = [], {}
-    for name, ln, group, total in (("a_query", "a_len", 1, n_vars), ("b_g1_query", "b1_len", 1, n_vars), ("b_g2_query", "b2_len", 2, n_vars),
-                                   ("h_query", "h_len", 1, N), ("l_query", "l_len", 1, n_wit)):
-        t, k = query(group, total)
-        keep.append(t)
-        dl[name] = k
-        setattr(d, name, t.data_ptr())
-        setattr(d, ln, total)
-    pk = be.pk_upload(d, mem=MEM_DEVICE, qap=CIRCOM)
-    keep.clear()
+    pk, dl = known_log_key(be, curve, consts, n_inst, n_wit, N, seed=4321, qap=CIRCOM)
     m = be.r1cs_upload(n_rows, n_inst, n_wit, csr)
     z_all = np.concatenate([z_inst, z_wit])
     ga, gb, gc = be.groth16_prove(pk, m, z_inst, z_wit, pack_fr(curve, [rr]), pack_fr(curve, [ss]))
@@ -239,23 +204,10 @@ def test_full_size_bls12_381_known_discrete_logs():
     be.sync()
     assert np.array_equal(h, hl), "circom h != -2 * libsnark h on the odd coset"
 
-    def dot(k_canon, scal_mont, n):
-        return unpack_fr(curve, cnative.fr_dot(cid, k_canon, scal_mont, n), mont=False)[0]
-
-    za = dot(dl["a_query"], z_all, n_vars)
-    zb1 = dot(dl["b_g1_query"], z_all, n_vars)
-    zb2 = dot(dl["b_g2_query"], z_all, n_vars)
-    wl = dot(dl["l_query"], z_wit, n_wit)
-    hh = dot(dl["h_query"], h, N)
-    alpha, beta, delta = consts
-    a_star = (alpha + za + rr * delta) % r
-    b1_star = (beta + zb1 + ss * delta) % r
-    b2_star = (beta + zb2 + ss * delta) % r
-    c_star = (ss * a_star + rr * b1_star - rr * ss % r * delta + wl + hh) % r
-    G1, G2 = groups(curve)
-    assert unpack_points(curve, 1, ga)[0] == G1.mul(G1.gen, a_star)
-    assert unpack_points(curve, 2, gb)[0] == G2.mul(G2.gen, b2_star)
-    assert unpack_points(curve, 1, gc)[0] == G1.mul(G1.gen, c_star)
+    want = known_log_proof(be, curve, consts, dl, z_inst, z_wit, h, rr, ss)
+    assert unpack_points(curve, 1, ga)[0] == want[0]
+    assert unpack_points(curve, 2, gb)[0] == want[1]
+    assert unpack_points(curve, 1, gc)[0] == want[2]
     be.r1cs_free(m)
     be.close()
 

@@ -17,7 +17,7 @@ from oracle import groth16 as og
 from oracle import r1cs as orc
 from oracle.ec import groups
 from oracle.params import BLS12_381, BN254
-from tests.util import csr_from_rows, limbs_to_ints, pack_fr, pack_points, unpack_fr, unpack_points
+from tests.util import csr_from_rows, known_log_key, known_log_proof, limbs_to_ints, pack_fr, pack_points, unpack_fr, unpack_points
 
 pytestmark = pytest.mark.gpu
 
@@ -105,54 +105,19 @@ def test_groth16_full_size_known_discrete_logs(log_n):
     """Synthetic key k_j*G (as bench.py builds it) at domain 2^log_n -- 2^24 is the benchmarked configuration, 2^25 the
     form with 2^24+ constraints (SURVEY 8d config 4): A, B, C must be the multiples of G predicted from z, h and the k_j
     with CPU field arithmetic, and h itself must equal the CPU oracle's witness_map element by element."""
-    import torch
-
     from snark_b200 import Backend
-    from snark_b200.lib import MEM_DEVICE, PkDesc
 
     curve, cid = BLS12_381, 0
     r = curve.r
     N = 1 << log_n
     n_rows, n_inst, n_wit = N - 2, 2, N - 3
-    n_vars = n_inst + n_wit
     rng = random.Random(7)
     a, b = rng.randrange(r), rng.randrange(r)
     rr, ss = rng.randrange(r), rng.randrange(r)
     csr, z_inst, z_wit = dummy_csr(curve, n_rows, a, b, n_wit)
     be = Backend(curve=cid)
-    dev = torch.device("cuda", 0)
-    gen = torch.Generator(device=dev); gen.manual_seed(1234)
-
-    def scalars(n):
-        t = torch.randint(-(1 << 31), (1 << 31) - 1, (n, 8), dtype=torch.int32, device=dev, generator=gen)
-        t[:, 7] &= 0x1FFFFFFF
-        return t
-
-    def query(group, n):
-        k = scalars(n)
-        out = torch.empty(n * (be.g1_bytes if group == 1 else be.g2_bytes) // 4, dtype=torch.int32, device=dev)
-        be.fixed_base(group, k, n, mont=False, out=out)
-        be.sync()
-        return out, k.cpu().numpy().view(np.uint32).reshape(-1)
-
     consts = [rng.randrange(1, r) for _ in range(3)]       # alpha, beta, delta
-    c1 = be.fixed_base(1, pack_fr(curve, consts, mont=False), 3, mont=False)
-    c2 = be.fixed_base(2, pack_fr(curve, consts[1:], mont=False), 2, mont=False)
-    g1w, g2w = be.g1_bytes // 4, be.g2_bytes // 4
-    c1t = torch.from_numpy(c1.view(np.int32)).to(dev); c2t = torch.from_numpy(c2.view(np.int32)).to(dev)
-    d = PkDesc()
-    d.n_instance, d.n_witness, d.domain_size = n_inst, n_wit, N
-    d.alpha_g1, d.beta_g1, d.delta_g1 = c1t.data_ptr(), c1t.data_ptr() + 4 * g1w, c1t.data_ptr() + 8 * g1w
-    d.beta_g2, d.delta_g2 = c2t.data_ptr(), c2t.data_ptr() + 4 * g2w
-    keep, dl = [], {}
-    # b_g1 and b_g2 queries share their discrete logs in a real key; here they are independent, which the algebra allows
-    for name, ln, group, total in (("a_query", "a_len", 1, n_vars), ("b_g1_query", "b1_len", 1, n_vars), ("b_g2_query", "b2_len", 2, n_vars),
-                                   ("h_query", "h_len", 1, N - 1), ("l_query", "l_len", 1, n_wit)):
-        t, k = query(group, total)
-        keep.append(t); dl[name] = k
-        setattr(d, name, t.data_ptr()); setattr(d, ln, total)
-    pk = be.pk_upload(d, mem=MEM_DEVICE)
-    keep.clear()
+    pk, dl = known_log_key(be, curve, consts, n_inst, n_wit, N, seed=1234)
     m = be.r1cs_upload(n_rows, n_inst, n_wit, csr)
     z_all = np.concatenate([z_inst, z_wit])
     ga, gb, gc = be.groth16_prove(pk, m, z_inst, z_wit, pack_fr(curve, [rr]), pack_fr(curve, [ss]))
@@ -172,23 +137,9 @@ def test_groth16_full_size_known_discrete_logs(log_n):
         bx, cx = b * su % r, ab * su % r
         hx = sum(hc * pow(x, i, r) for i, hc in enumerate(unpack_fr(curve, h))) % r
         assert (ax * bx - cx - hx * (pow(x, N, r) - 1)) % r == 0
-    # discrete logs of the proof elements: dot products in Fr done by the C++ oracle (Montgomery in/out)
-    def dot(k_canon, scal_mont, n):
-        # k canonical -> Montgomery by multiplying with R^2 ... simpler: dot(k, s~) = R * sum k_i s_i  =>  times R^-1 twice
-        v = unpack_fr(curve, cnative.fr_dot(cid, k_canon, scal_mont, n), mont=False)[0]   # = sum k_i * s~_i * R^-1 = sum k_i s_i
-        return v
-    za = dot(dl["a_query"], z_all, n_vars)
-    zb1 = dot(dl["b_g1_query"], z_all, n_vars)
-    zb2 = dot(dl["b_g2_query"], z_all, n_vars)
-    wl = dot(dl["l_query"], z_wit, n_wit)
-    hh = dot(dl["h_query"], h, N - 1)
-    alpha, beta, delta = consts
-    a_star = (alpha + za + rr * delta) % r
-    b1_star = (beta + zb1 + ss * delta) % r
-    b2_star = (beta + zb2 + ss * delta) % r
-    c_star = (ss * a_star + rr * b1_star - rr * ss % r * delta + wl + hh) % r
-    G1, G2 = groups(curve)
-    assert unpack_points(curve, 1, ga)[0] == G1.mul(G1.gen, a_star)
-    assert unpack_points(curve, 2, gb)[0] == G2.mul(G2.gen, b2_star)
-    assert unpack_points(curve, 1, gc)[0] == G1.mul(G1.gen, c_star)
+    # the proof elements against their discrete logs: dot products in Fr done by the C++ oracle
+    want = known_log_proof(be, curve, consts, dl, z_inst, z_wit, h, rr, ss)
+    assert unpack_points(curve, 1, ga)[0] == want[0]
+    assert unpack_points(curve, 2, gb)[0] == want[1]
+    assert unpack_points(curve, 1, gc)[0] == want[2]
     be.pk_free(pk); be.r1cs_free(m); be.close()

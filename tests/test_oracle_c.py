@@ -12,12 +12,14 @@ from oracle import ntt as ontt
 from oracle import r1cs as orc
 from oracle.ec import groups
 from oracle.params import BLS12_381, BN254
+from tests import circom_oracle as oc
+from tests.bls377_oracle import BLS12_377
 from tests.util import csr_from_rows, pack_fr, pack_points, unpack_fr, unpack_points
 
-CURVES = [BLS12_381, BN254]
+CURVES = [BLS12_381, BN254, BLS12_377]
 
 
-@pytest.mark.parametrize("cid", [0, 1])
+@pytest.mark.parametrize("cid", [0, 1, 2])
 def test_c_ntt(cid):
     curve = CURVES[cid]
     rng = random.Random(cid)
@@ -29,7 +31,7 @@ def test_c_ntt(cid):
         assert unpack_fr(curve, cnative.ntt(cid, pack_fr(curve, x), log_n, inverse=True, coset=True)) == ontt.coset_intt(curve, x)
 
 
-@pytest.mark.parametrize("cid,group", [(0, 1), (0, 2), (1, 1), (1, 2)])
+@pytest.mark.parametrize("cid,group", [(0, 1), (0, 2), (1, 1), (1, 2), (2, 1), (2, 2)])
 def test_c_msm(cid, group):
     curve = CURVES[cid]
     G = groups(curve)[group - 1]
@@ -48,7 +50,7 @@ def test_c_msm(cid, group):
     assert mult == [G.mul(G.gen, 5 + i) for i in range(9)]
 
 
-@pytest.mark.parametrize("cid", [0, 1])
+@pytest.mark.parametrize("cid", [0, 1, 2])
 def test_c_groth16(cid):
     curve = CURVES[cid]
     rng = random.Random(99 + cid)
@@ -76,3 +78,25 @@ def test_c_groth16(cid):
     x = [rng.randrange(curve.r) for _ in range(50)]
     y = [rng.randrange(curve.r) for _ in range(50)]
     assert unpack_fr(curve, cnative.fr_dot(cid, pack_fr(curve, x), pack_fr(curve, y), 50))[0] == sum(p * q for p, q in zip(x, y)) % curve.r
+
+
+@pytest.mark.parametrize("cid", [0, 1, 2])
+def test_c_witness_map_circom(cid):
+    """orc_witness_map_circom against tests/circom_oracle.py, satisfying and spoiled assignments, unit and random
+    coefficients, a full domain and one that has just doubled"""
+    curve = CURVES[cid]
+    rng = random.Random(0xC1 + cid)
+    bc = orc.bench_circuit(curve, 12, seed=3)
+    bc.finalize()
+    cases = [(bc.to_matrices(), bc.instance_assignment, bc.witness_assignment)]
+    for n_rows, n_inst, n_vars in ((29, 3, 40), (14, 3, 20)):      # 29 + 3 = 2^5; 14 + 3 = 2^4 + 1
+        mats = [[[(rng.choice([1, 2, curve.r - 1, rng.randrange(curve.r)]), rng.randrange(n_vars))
+                  for _ in range(rng.randrange(5))] for _ in range(n_rows)] for _ in range(3)]
+        z = [1] + [rng.choice([0, 1, curve.r - 1, rng.randrange(curve.r)]) for _ in range(n_vars - 1)]
+        cases.append((mats, z[:n_inst], z[n_inst:]))
+    for mats, inst, wit in cases:
+        csr = [csr_from_rows(curve, m) for m in mats]
+        for w in (wit, [(v + 1) % curve.r for v in wit]):
+            z = list(inst) + list(w)
+            got = cnative.witness_map_circom(cid, csr, len(mats[0]), len(inst), pack_fr(curve, z), threads=3)
+            assert unpack_fr(curve, got) == oc.witness_map_circom(curve, mats, z, len(inst)), len(mats[0])

@@ -144,3 +144,77 @@ def pairing_verify_packed(curve, vk, n_instance, z_inst, proof_abc):
     a, b, c = proof_abc
     proof = (unpack_points(curve, 1, a)[0], unpack_points(curve, 2, b)[0], unpack_points(curve, 1, c)[0])
     return pairing.groth16_verify(vk_pts, list(z_inst[1:]), proof, curve)
+
+
+# ---- synthetic proving keys of known discrete logs (GPU tests at full size) ----------------------
+KEY_QUERIES = (("a_query", "a_len", 1), ("b_g1_query", "b1_len", 1), ("b_g2_query", "b2_len", 2), ("h_query", "h_len", 1),
+               ("l_query", "l_len", 1))
+
+
+def known_log_key(be, curve, consts, n_inst, n_wit, domain, seed, qap=0):
+    """A proving key whose points are k G for random k known to the caller, as bench.py builds it: the k are drawn on the GPU
+    (torch generator seeded with `seed`, below 2^253 and below r), multiplied by the fixed-base kernel and uploaded from
+    device memory.  consts = (alpha, beta, delta) as ints; the h query has domain - 1 points (libsnark) or domain (qap = 1,
+    circom).  The b_g1 and b_g2 queries get independent logs, which the algebra allows.  Returns (pk handle, dl) with
+    dl[query] the canonical uint32 limbs of its k."""
+    import torch
+
+    from snark_b200.lib import MEM_DEVICE, PkDesc
+
+    dev = torch.device("cuda", 0)
+    gen = torch.Generator(device=dev)
+    gen.manual_seed(seed)
+    top = (1 << (min(253, curve.r.bit_length() - 1) - 224)) - 1
+    n_vars = n_inst + n_wit
+    lens = {"a_query": n_vars, "b_g1_query": n_vars, "b_g2_query": n_vars, "h_query": domain if qap else domain - 1,
+            "l_query": n_wit}
+
+    def query(group, n):
+        k = torch.randint(-(1 << 31), (1 << 31) - 1, (n, 8), dtype=torch.int32, device=dev, generator=gen)
+        k[:, 7] &= top
+        out = torch.empty(n * (be.g1_bytes if group == 1 else be.g2_bytes) // 4, dtype=torch.int32, device=dev)
+        be.fixed_base(group, k, n, mont=False, out=out)
+        be.sync()
+        return out, k.cpu().numpy().view(np.uint32).reshape(-1)
+
+    c1 = be.fixed_base(1, pack_fr(curve, consts, mont=False), 3, mont=False)
+    c2 = be.fixed_base(2, pack_fr(curve, consts[1:], mont=False), 2, mont=False)
+    g1w, g2w = be.g1_bytes // 4, be.g2_bytes // 4
+    c1t = torch.from_numpy(c1.view(np.int32)).to(dev)
+    c2t = torch.from_numpy(c2.view(np.int32)).to(dev)
+    d = PkDesc()
+    d.n_instance, d.n_witness, d.domain_size = n_inst, n_wit, domain
+    d.alpha_g1, d.beta_g1, d.delta_g1 = c1t.data_ptr(), c1t.data_ptr() + 4 * g1w, c1t.data_ptr() + 8 * g1w
+    d.beta_g2, d.delta_g2 = c2t.data_ptr(), c2t.data_ptr() + 4 * g2w
+    keep, dl = [], {}
+    for name, ln, group in KEY_QUERIES:
+        t, k = query(group, lens[name])
+        keep.append(t)
+        dl[name] = k
+        setattr(d, name, t.data_ptr())
+        setattr(d, ln, lens[name])
+    return be.pk_upload(d, mem=MEM_DEVICE, qap=qap), dl
+
+
+def known_log_proof(be, curve, consts, dl, z_inst, z_wit, h, r, s):
+    """The proof (A, B, C) as affine oracle points that a key of known_log_key gives for z = z_inst || z_wit (Montgomery
+    limbs), the witness map's h (Montgomery limbs, as many as the h query has points) and ints r, s: the exponents by
+    dot products in Fr on the CPU (C++ oracle), the points by the oracle's scalar multiplication of the generators."""
+    from oracle import cnative
+    from oracle.ec import groups
+
+    rm = curve.r
+    z_all = np.concatenate([z_inst, z_wit])
+
+    def dot(name, scal_mont):
+        # fr_dot(k, s~) = sum k_i s~_i R^-1 = sum k_i s_i: read back as a canonical value
+        n = len(dl[name]) // 8
+        return unpack_fr(curve, cnative.fr_dot(be.curve, dl[name], scal_mont, n), mont=False)[0]
+
+    alpha, beta, delta = consts
+    a_star = (alpha + dot("a_query", z_all) + r * delta) % rm
+    b1_star = (beta + dot("b_g1_query", z_all) + s * delta) % rm
+    b2_star = (beta + dot("b_g2_query", z_all) + s * delta) % rm
+    c_star = (s * a_star + r * b1_star - r * s % rm * delta + dot("l_query", z_wit) + dot("h_query", h)) % rm
+    G1, G2 = groups(curve)
+    return G1.mul(G1.gen, a_star), G2.mul(G2.gen, b2_star), G1.mul(G1.gen, c_star)
