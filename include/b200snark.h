@@ -211,6 +211,32 @@ typedef struct b2s_predicate_desc {
 } b2s_predicate_desc;
 int32_t b2s_gr1cs_upload(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates,
                          const b2s_predicate_desc* preds, b2s_gr1cs** out);
+/* The same handle built ON THE DEVICE from the constraint system's flat storage, bypassing to_matrices() for every predicate,
+ * as b2s_r1cs_upload_lcmap does for the R1CS one: one descriptor per entry of predicate_constraint_systems (pass them in label
+ * order), each with its polynomial as in b2s_predicate_desc and, for argument j < arity, get_constraints()[j]: n_rows raw
+ * Variables.  All predicates share one LcMap and one interner pool, laid out as for b2s_r1cs_upload_lcmap; the pool is kept
+ * as it is, not re-interned.  Row i of argument j is make_row(get_lc(args[j][i])): Zero gives no terms, SymbolicLc(k) the
+ * terms of LC k, any other variable the single term (ONE, v); terms with a zero coefficient or the Zero variable are dropped,
+ * repeated columns stay.  For every z b2s_gr1cs_check then gives what it gives on the b2s_gr1cs_upload handle of
+ * to_matrices().  Rejected, with the status codes of b2s_gr1cs_upload: a descriptor it rejects (args[j] null with
+ * n_rows > 0 included), checked before anything is allocated; and with those of b2s_r1cs_upload_lcmap: an LcMap it rejects
+ * (B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE also for 2^32 or more (argument, row) slots or nonzeros over all predicates).
+ * b2s_last_error names the predicate (upload index) and, for a rejected argument, the argument and the constraint.
+ * HOST pointers; the call returns after the last copy, so the caller may free them. */
+typedef struct b2s_predicate_lcmap_desc {
+    uint32_t arity;                        /* as b2s_predicate_desc */
+    uint32_t n_terms;
+    const void* term_coeffs;
+    const uint32_t* term_offsets;
+    const uint32_t* factor_var;
+    const uint32_t* factor_pow;
+    uint64_t n_rows;                       /* this predicate's num_constraints */
+    const uint64_t* args[B2S_GR1CS_MAX_ARITY];   /* get_constraints()[j]: n_rows raw Variables, j < arity */
+} b2s_predicate_lcmap_desc;
+int32_t b2s_gr1cs_upload_lcmap(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates,
+                               const b2s_predicate_lcmap_desc* preds, uint64_t n_lcs, const uint64_t* lc_offsets,
+                               const uint64_t* lc_vars, const uint32_t* lc_coeffs, const void* pool, uint32_t pool_len,
+                               b2s_gr1cs** out);
 void b2s_gr1cs_free(b2s_ctx* ctx, b2s_gr1cs* g);
 int32_t b2s_gr1cs_check(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem,
                         uint64_t* first_unsat, uint64_t* n_unsat);

@@ -5,8 +5,9 @@ use std::os::raw::c_void;
 use ark_ec::{pairing::Pairing, AffineRepr};
 use ark_groth16::{Groth16, PreparedVerifyingKey, Proof, ProvingKey, VerifyingKey};
 use ark_ff::PrimeField;
+use ark_relations::utils::variable::{VarKind, Variable};
 use ark_relations::gr1cs::{
-    predicate::Predicate, ConstraintSynthesizer, ConstraintSystem, Label, Matrix, OptimizationGoal, SynthesisError,
+    predicate::{polynomial_constraint::PolynomialPredicate, Predicate}, ConstraintSynthesizer, ConstraintSystem, Label, Matrix, OptimizationGoal, SynthesisError,
     R1CS_PREDICATE_LABEL,
 };
 use ark_snark::{CircuitSpecificSetupSNARK, SNARK};
@@ -27,6 +28,15 @@ pub struct B2sPredicateDesc {
     pub n_rows: u64,
     pub row_ptr: [*const u64; B2S_GR1CS_MAX_ARITY], pub col: [*const u32; B2S_GR1CS_MAX_ARITY],
     pub coeff: [*const c_void; B2S_GR1CS_MAX_ARITY],
+}
+/// `b2s_predicate_lcmap_desc`: a predicate's polynomial as in `B2sPredicateDesc`, and for argument j < arity
+/// `get_constraints()[j]` as raw Variables (tag << 61 | index)
+#[repr(C)]
+pub struct B2sPredicateLcmapDesc {
+    pub arity: u32, pub n_terms: u32,
+    pub term_coeffs: *const c_void, pub term_offsets: *const u32, pub factor_var: *const u32, pub factor_pow: *const u32,
+    pub n_rows: u64,
+    pub args: [*const u64; B2S_GR1CS_MAX_ARITY],
 }
 
 #[repr(C)]
@@ -137,6 +147,9 @@ extern "C" {
     pub fn b2s_poly_eval(ctx: *mut B2sCtx, coeffs: *const c_void, n: u64, z: *const c_void, mem: i32, out: *mut c_void) -> i32;
     pub fn b2s_gr1cs_upload(ctx: *mut B2sCtx, n_instance: u64, n_witness: u64, n_predicates: u32, preds: *const B2sPredicateDesc,
                             out: *mut *mut B2sGr1cs) -> i32;
+    pub fn b2s_gr1cs_upload_lcmap(ctx: *mut B2sCtx, n_instance: u64, n_witness: u64, n_predicates: u32,
+                                  preds: *const B2sPredicateLcmapDesc, n_lcs: u64, lc_offsets: *const u64, lc_vars: *const u64,
+                                  lc_coeffs: *const u32, pool: *const c_void, pool_len: u32, out: *mut *mut B2sGr1cs) -> i32;
     pub fn b2s_gr1cs_free(ctx: *mut B2sCtx, g: *mut B2sGr1cs);
     pub fn b2s_gr1cs_check(ctx: *mut B2sCtx, g: *const B2sGr1cs, n_assign: u64, z: *const c_void, mem: i32, first_unsat: *mut u64,
                            n_unsat: *mut u64) -> i32;
@@ -563,8 +576,7 @@ impl<F: PrimeField> Gr1csB200<F> {
     /// `F`'s curve (checked by the modulus size: 255 / 254 / 253 bits).  A predicate that is not polynomial (`Predicate` is `#[non_exhaustive]`,
     /// predicate/mod.rs:19-25) is `B200Error::Backend(B2S_ERR_INVALID_ARG)`.
     pub fn upload(curve_id: i32, cs: &ConstraintSystem<F>) -> Result<Self, B200Error> {
-        let bits = match curve_id { 0 => 255, 1 => 254, 2 => 253, _ => return Err(B200Error::Backend(ERR_INVALID_ARG)) };
-        if F::MODULUS_BIT_SIZE != bits || core::mem::size_of::<F>() != 32 { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        Self::check_curve(curve_id)?;
         let mats = cs.to_matrices()?;
         let types = cs.get_all_predicate_types();
         // per predicate: (arity, coefficients, term offsets, factor variables, factor powers) and its CSR matrices
@@ -576,13 +588,7 @@ impl<F: PrimeField> Gr1csB200<F> {
                 Some(Predicate::Polynomial(p)) => p,
                 _ => return Err(B200Error::Backend(ERR_INVALID_ARG)),
             };
-            let (mut co, mut off, mut var, mut pow) = (Vec::new(), vec![0u32], Vec::new(), Vec::new());
-            for (c, term) in &p.polynomial.terms {
-                co.push(*c);
-                for (v, e) in term.iter() { var.push(*v as u32); pow.push(*e as u32); }
-                off.push(var.len() as u32);
-            }
-            terms.push((p.polynomial.num_vars as u32, co, off, var, pow));
+            terms.push(poly_terms(p));
             csrs.push(ms.iter().map(to_csr).collect::<Vec<_>>());
             labels.push(label.clone());
         }
@@ -600,14 +606,73 @@ impl<F: PrimeField> Gr1csB200<F> {
             }
             d
         }).collect();
+        Self::create(curve_id, cs, labels, |ctx, g| unsafe {
+            b2s_gr1cs_upload(ctx, cs.num_instance_variables() as u64, cs.num_witness_variables() as u64, descs.len() as u32,
+                             descs.as_ptr(), g)
+        })
+    }
+
+    /// The same handle built on the GPU from the constraint system's own storage, without `to_matrices()`: every entry of
+    /// `cs.predicate_constraint_systems` (its `get_constraints()` and `get_predicate()`, in label order) over the one
+    /// `cs.lc_map` (`#[doc(hidden)] pub`).  `cs` must be finalized (nested LCs are `B200Error::Backend(B2S_ERR_INVALID_ARG)`).
+    /// The interner is private upstream (`constraint_system.rs:88`, `gr1cs/mod.rs:9`), so its two facts come from the
+    /// caller until it has a one-line accessor: `pool` is its `vec` (pool[0] = ONE, pool[1] = -ONE) and `coeff_ids` the
+    /// index each `InternedField` of the LcMap names in it, flat in the order of `cs.lc_map.iter()`.
+    pub fn upload_lcmap(curve_id: i32, cs: &ConstraintSystem<F>, pool: &[F], coeff_ids: &[u32]) -> Result<Self, B200Error> {
+        Self::check_curve(curve_id)?;
+        let raw = |v: &Variable| -> u64 {
+            ((v.kind() as u64) << 61) | v.index().unwrap_or(0) as u64
+        };
+        // the LcMap's variables, flat: LC i's terms at offsets[i]..offsets[i + 1]
+        let (mut offsets, mut vars) = (vec![0u64], Vec::new());
+        for lc in cs.lc_map.iter() {
+            vars.extend(lc.map(|(_, v)| raw(v)));
+            offsets.push(vars.len() as u64);
+        }
+        if coeff_ids.len() != vars.len() { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        let mut terms = Vec::new();
+        let mut args: Vec<Vec<Vec<u64>>> = Vec::new();
+        let mut labels = Vec::new();
+        for (label, pcs) in &cs.predicate_constraint_systems {
+            let p = match pcs.get_predicate() {
+                Predicate::Polynomial(p) => p,
+                _ => return Err(B200Error::Backend(ERR_INVALID_ARG)),
+            };
+            terms.push(poly_terms(p));
+            args.push(pcs.get_constraints().iter().map(|a| a.iter().map(raw).collect()).collect());
+            labels.push(label.clone());
+        }
+        let descs: Vec<B2sPredicateLcmapDesc> = terms.iter().zip(&args).zip(&cs.predicate_constraint_systems)
+            .map(|(((arity, co, off, var, pow), a), (_, pcs))| {
+                let mut d = B2sPredicateLcmapDesc {
+                    arity: *arity, n_terms: co.len() as u32, term_coeffs: co.as_ptr().cast(), term_offsets: off.as_ptr(),
+                    factor_var: var.as_ptr(), factor_pow: pow.as_ptr(), n_rows: pcs.num_constraints() as u64,
+                    args: [core::ptr::null(); B2S_GR1CS_MAX_ARITY],
+                };
+                for (j, col) in a.iter().take(B2S_GR1CS_MAX_ARITY).enumerate() { d.args[j] = col.as_ptr(); }
+                d
+            }).collect();
+        Self::create(curve_id, cs, labels, |ctx, g| unsafe {
+            b2s_gr1cs_upload_lcmap(ctx, cs.num_instance_variables() as u64, cs.num_witness_variables() as u64, descs.len() as u32,
+                                   descs.as_ptr(), (offsets.len() - 1) as u64, offsets.as_ptr(), vars.as_ptr(), coeff_ids.as_ptr(),
+                                   pool.as_ptr().cast(), pool.len() as u32, g)
+        })
+    }
+
+    fn check_curve(curve_id: i32) -> Result<(), B200Error> {
+        let bits = match curve_id { 0 => 255, 1 => 254, 2 => 253, _ => return Err(B200Error::Backend(ERR_INVALID_ARG)) };
+        if F::MODULUS_BIT_SIZE != bits || core::mem::size_of::<F>() != 32 { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        Ok(())
+    }
+
+    /// a ctx on `curve_id` and the handle `upload` makes on it; the ctx is destroyed again if the upload fails
+    fn create(curve_id: i32, cs: &ConstraintSystem<F>, labels: Vec<Label>, upload: impl FnOnce(*mut B2sCtx, *mut *mut B2sGr1cs) -> i32)
+        -> Result<Self, B200Error> {
         let n_vars = cs.num_instance_variables() + cs.num_witness_variables();
         let mut ctx: *mut B2sCtx = core::ptr::null_mut();
         check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
         let mut g: *mut B2sGr1cs = core::ptr::null_mut();
-        let st = unsafe {
-            b2s_gr1cs_upload(ctx, cs.num_instance_variables() as u64, cs.num_witness_variables() as u64, descs.len() as u32,
-                             descs.as_ptr(), &mut g)
-        };
+        let st = upload(ctx, &mut g);
         if st != 0 { unsafe { b2s_ctx_destroy(ctx) }; }
         check(ctx, st)?;
         Ok(Gr1csB200 { ctx, g, labels, n_vars, _f: core::marker::PhantomData })
@@ -631,6 +696,17 @@ impl<F: PrimeField> Gr1csB200<F> {
     pub fn assignment(cs: &ConstraintSystem<F>) -> Result<Vec<F>, B200Error> {
         Ok([cs.instance_assignment()?, cs.witness_assignment()?].concat())
     }
+}
+
+/// A polynomial predicate as the C ABI takes it: (arity, coefficients, term offsets, factor variables, factor powers)
+fn poly_terms<F: PrimeField>(p: &PolynomialPredicate<F>) -> (u32, Vec<F>, Vec<u32>, Vec<u32>, Vec<u32>) {
+    let (mut co, mut off, mut var, mut pow) = (Vec::new(), vec![0u32], Vec::new(), Vec::new());
+    for (c, term) in &p.polynomial.terms {
+        co.push(*c);
+        for (v, e) in term.iter() { var.push(*v as u32); pow.push(*e as u32); }
+        off.push(var.len() as u32);
+    }
+    (p.polynomial.num_vars as u32, co, off, var, pow)
 }
 
 impl<F: PrimeField> Drop for Gr1csB200<F> {

@@ -405,6 +405,17 @@ int32_t b2s_gr1cs_upload(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, 
     return gr1cs_upload(ctx, n_instance, n_witness, n_predicates, preds, out);
 }
 
+int32_t b2s_gr1cs_upload_lcmap(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates,
+                               const b2s_predicate_lcmap_desc* preds, uint64_t n_lcs, const uint64_t* lc_offsets, const uint64_t* lc_vars,
+                               const uint32_t* lc_coeffs, const void* pool, uint32_t pool_len, b2s_gr1cs** out) {
+    LOCK(ctx);
+    if (!out || (!preds && n_predicates) || !lc_offsets || !pool) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_upload_lcmap: null argument");
+    if (n_lcs && lc_offsets[n_lcs] != 0 && (!lc_vars || !lc_coeffs)) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_upload_lcmap: null LC arrays");
+    *out = nullptr;
+    return gr1cs_upload_lcmap(ctx, n_instance, n_witness, n_predicates, preds, LcMapHost{n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len},
+                              out);
+}
+
 void b2s_gr1cs_free(b2s_ctx* ctx, b2s_gr1cs* g) {
     if (!ctx || !g) return;
     std::lock_guard<std::mutex> guard(ctx->mu);

@@ -148,34 +148,72 @@ int32_t check_t(Ctx* c, const std::vector<PredView>& views, const void* pool, ui
     return B2S_OK;
 }
 
+// The checks shared by both uploads: the variable count, and of one descriptor the arity, the row count and the polynomial
+int32_t check_vars(Ctx* c, uint64_t n_instance, uint64_t n_witness) {
+    const uint64_t n_vars = n_instance + n_witness;
+    if (n_instance == 0) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: n_instance counts the constant One and must be >= 1");
+    if (n_vars > (1ull << 32))
+        return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "gr1cs: %llu variables; columns are u32, the limit is 2^32", (unsigned long long)n_vars);
+    return B2S_OK;
+}
+
+template <class Desc>
+int32_t check_poly(Ctx* c, uint32_t p, const Desc& d) {
+    if (d.arity == 0 || d.arity > MAXA)
+        return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: arity %u outside 1..%d", p, d.arity, MAXA);
+    if (d.n_rows >= (1ull << 32))
+        return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "gr1cs: predicate %u: %llu constraints; the limit is 2^32 - 1", p,
+                    (unsigned long long)d.n_rows);
+    if (d.n_terms) {
+        if (!d.term_coeffs || !d.term_offsets) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null term arrays", p);
+        if (d.term_offsets[0] != 0) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: term_offsets[0] != 0", p);
+        for (uint32_t t = 0; t < d.n_terms; t++)
+            if (d.term_offsets[t + 1] < d.term_offsets[t])
+                return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: term_offsets not monotone at term %u", p, t);
+        const uint32_t nf = d.term_offsets[d.n_terms];
+        if (nf && (!d.factor_var || !d.factor_pow)) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null factor arrays", p);
+        for (uint32_t f = 0; f < nf; f++)
+            if (d.factor_var[f] >= d.arity)
+                return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: factor_var[%u] = %u >= arity %u", p, f, d.factor_var[f], d.arity);
+    }
+    return B2S_OK;
+}
+
+// a new predicate with the shape and the polynomial (term arrays on the device) of a checked descriptor
+template <class Desc>
+int32_t upload_poly(Ctx* c, const Desc& d, std::unique_ptr<Gr1csPredicate>& out) {
+    std::unique_ptr<Gr1csPredicate> pr(new Gr1csPredicate());
+    pr->arity = d.arity;
+    pr->n_terms = d.n_terms;
+    pr->n_rows = d.n_rows;
+    if (d.n_terms) {
+        const uint64_t nf = d.term_offsets[d.n_terms];
+        B2S_TRY(pr->term_coeff.alloc(c, (uint64_t)d.n_terms * 32));
+        B2S_TRY(pr->term_off.alloc(c, ((uint64_t)d.n_terms + 1) * 4));
+        B2S_TRY(pr->factor_var.alloc(c, nf * 4));
+        B2S_TRY(pr->factor_pow.alloc(c, nf * 4));
+        B2S_CUDA(c, cudaMemcpyAsync(pr->term_coeff.p, d.term_coeffs, (uint64_t)d.n_terms * 32, cudaMemcpyHostToDevice, c->stream));
+        B2S_CUDA(c, cudaMemcpyAsync(pr->term_off.p, d.term_offsets, ((uint64_t)d.n_terms + 1) * 4, cudaMemcpyHostToDevice, c->stream));
+        if (nf) {
+            B2S_CUDA(c, cudaMemcpyAsync(pr->factor_var.p, d.factor_var, nf * 4, cudaMemcpyHostToDevice, c->stream));
+            B2S_CUDA(c, cudaMemcpyAsync(pr->factor_pow.p, d.factor_pow, nf * 4, cudaMemcpyHostToDevice, c->stream));
+        }
+        B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+    }
+    out = std::move(pr);
+    return B2S_OK;
+}
+
 template <class Curve>
 int32_t gr1cs_upload_t(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_desc* preds,
                        b2s_gr1cs** out) {
     using FrP = typename Curve::FrP;
     const uint64_t n_vars = n_instance + n_witness;
-    if (n_instance == 0) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: n_instance counts the constant One and must be >= 1");
-    if (n_vars > (1ull << 32))
-        return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "gr1cs: %llu variables; columns are u32, the limit is 2^32", (unsigned long long)n_vars);
+    B2S_TRY(check_vars(c, n_instance, n_witness));
     // the descriptors first: nothing is interned or allocated for a malformed one
     for (uint32_t p = 0; p < n_predicates; p++) {
         const b2s_predicate_desc& d = preds[p];
-        if (d.arity == 0 || d.arity > MAXA)
-            return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: arity %u outside 1..%d", p, d.arity, MAXA);
-        if (d.n_rows >= (1ull << 32))
-            return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "gr1cs: predicate %u: %llu constraints; the limit is 2^32 - 1", p,
-                        (unsigned long long)d.n_rows);
-        if (d.n_terms) {
-            if (!d.term_coeffs || !d.term_offsets) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null term arrays", p);
-            if (d.term_offsets[0] != 0) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: term_offsets[0] != 0", p);
-            for (uint32_t t = 0; t < d.n_terms; t++)
-                if (d.term_offsets[t + 1] < d.term_offsets[t])
-                    return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: term_offsets not monotone at term %u", p, t);
-            const uint32_t nf = d.term_offsets[d.n_terms];
-            if (nf && (!d.factor_var || !d.factor_pow)) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null factor arrays", p);
-            for (uint32_t f = 0; f < nf; f++)
-                if (d.factor_var[f] >= d.arity)
-                    return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: factor_var[%u] = %u >= arity %u", p, f, d.factor_var[f], d.arity);
-        }
+        B2S_TRY(check_poly(c, p, d));
         for (uint32_t j = 0; j < d.arity; j++)
             if (!d.row_ptr[j] || ((!d.col[j] || !d.coeff[j]) && d.row_ptr[j][d.n_rows] != 0))
                 return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null CSR array for argument %u", p, j);
@@ -187,29 +225,13 @@ int32_t gr1cs_upload_t(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t
     CoeffInterner in(fr_one_key<FrP>());
     for (uint32_t p = 0; p < n_predicates; p++) {
         const b2s_predicate_desc& d = preds[p];
-        std::unique_ptr<Gr1csPredicate> pr(new Gr1csPredicate());
-        pr->arity = d.arity;
-        pr->n_terms = d.n_terms;
-        pr->n_rows = d.n_rows;
+        std::unique_ptr<Gr1csPredicate> pr;
+        B2S_TRY(upload_poly(c, d, pr));
         char who[48];
         snprintf(who, sizeof(who), "gr1cs: predicate %u", p);
         for (uint32_t j = 0; j < d.arity; j++)
             B2S_TRY(csr_intern_upload(c, in, who, (int)j, d.n_rows, n_vars, d.row_ptr[j], d.col[j], d.coeff[j], pr->row_ptr[j], pr->col[j],
                                       pr->coeff_id[j], &pr->nnz[j]));
-        if (d.n_terms) {
-            const uint64_t nf = d.term_offsets[d.n_terms];
-            B2S_TRY(pr->term_coeff.alloc(c, (uint64_t)d.n_terms * 32));
-            B2S_TRY(pr->term_off.alloc(c, ((uint64_t)d.n_terms + 1) * 4));
-            B2S_TRY(pr->factor_var.alloc(c, nf * 4));
-            B2S_TRY(pr->factor_pow.alloc(c, nf * 4));
-            B2S_CUDA(c, cudaMemcpyAsync(pr->term_coeff.p, d.term_coeffs, (uint64_t)d.n_terms * 32, cudaMemcpyHostToDevice, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync(pr->term_off.p, d.term_offsets, ((uint64_t)d.n_terms + 1) * 4, cudaMemcpyHostToDevice, c->stream));
-            if (nf) {
-                B2S_CUDA(c, cudaMemcpyAsync(pr->factor_var.p, d.factor_var, nf * 4, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync(pr->factor_pow.p, d.factor_pow, nf * 4, cudaMemcpyHostToDevice, c->stream));
-            }
-            B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-        }
         g->preds.push_back(std::move(pr));
     }
     B2S_TRY(coeff_pool_upload(c, in, "gr1cs", g->pool, &g->pool_size));
@@ -270,6 +292,45 @@ int32_t gr1cs_upload(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n
     return dispatch_curve(c, [&](auto curve) {
         return gr1cs_upload_t<decltype(curve)>(c, n_instance, n_witness, n_predicates, preds, out);
     });
+}
+
+int32_t gr1cs_upload_lcmap(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_lcmap_desc* preds,
+                           const LcMapHost& lm, b2s_gr1cs** out) {
+    B2S_TRY(check_vars(c, n_instance, n_witness));
+    uint64_t n_slots = 0;   // (argument, row) slots of all predicates, saturated at 2^32 (lcmap_validate rejects that)
+    for (uint32_t p = 0; p < n_predicates; p++) {
+        const b2s_predicate_lcmap_desc& d = preds[p];
+        B2S_TRY(check_poly(c, p, d));
+        for (uint32_t j = 0; j < d.arity; j++)
+            if (!d.args[j] && d.n_rows) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null argument array %u", p, j);
+        n_slots = std::min<uint64_t>(n_slots + d.arity * d.n_rows, 1ull << 32);
+    }
+    B2S_TRY(lcmap_validate(c, lm, n_slots));
+    std::unique_ptr<b2s_gr1cs> g(new b2s_gr1cs());
+    g->curve = c->curve;
+    g->n_instance = n_instance;
+    g->n_witness = n_witness;
+    std::vector<LcMatrix> mats;
+    std::vector<std::pair<uint32_t, uint32_t>> arg_of;   // (predicate, argument) of each matrix, for messages
+    for (uint32_t p = 0; p < n_predicates; p++) {
+        const b2s_predicate_lcmap_desc& d = preds[p];
+        std::unique_ptr<Gr1csPredicate> pr;
+        B2S_TRY(upload_poly(c, d, pr));
+        for (uint32_t j = 0; j < d.arity; j++) {
+            mats.push_back({d.args[j], d.n_rows, &pr->row_ptr[j], &pr->col[j], &pr->coeff_id[j], &pr->nnz[j]});
+            arg_of.emplace_back(p, j);
+        }
+        g->preds.push_back(std::move(pr));
+    }
+    const auto where = [&](size_t m, uint64_t row) {
+        char buf[96];
+        snprintf(buf, sizeof(buf), "gr1cs: predicate %u, argument %u, constraint %llu: ", arg_of[m].first, arg_of[m].second,
+                 (unsigned long long)row);
+        return std::string(buf);
+    };
+    B2S_TRY(lcmap_build(c, lm, n_instance, n_instance + n_witness, mats, "the arguments of all predicates", where, g->pool, &g->pool_size));
+    *out = g.release();
+    return B2S_OK;
 }
 
 int32_t gr1cs_check(Ctx* c, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat) {

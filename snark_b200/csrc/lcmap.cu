@@ -1,6 +1,8 @@
-// b2s_r1cs_upload_lcmap: build the device CSR of A, B, C from the constraint system's flat LcMap (lcmap.cuh has the
-// reference citations and the per-row logic).  Three launches per matrix set: count, scan (msm.cu's scan kernels),
-// fill; everything is HBM-bound index work and runs once per circuit.
+// Argument matrices built on the device from the constraint system's flat LcMap (lcmap.cuh has the reference citations and
+// the per-row logic): A, B, C for b2s_r1cs_upload_lcmap, every argument of every predicate for b2s_gr1cs_upload_lcmap.
+// The matrices are one flat list of (matrix, row) slots, so any number of them takes the same launches: count, scan
+// (msm.cu's scan kernels), bounds, fill; everything is HBM-bound index work and runs once per circuit.
+#include <algorithm>
 #include <cstring>
 #include <vector>
 
@@ -12,39 +14,173 @@ namespace b2s {
 
 using lcmap::View;
 
-struct LcArgs { const uint64_t* a[3]; };
-struct LcOut { uint64_t* row_ptr[3]; uint32_t* col[3]; uint32_t* coeff_id[3]; };
+// where matrix m's CSR goes (device pointers)
+struct LcOut { uint64_t* row_ptr; uint32_t* col; uint32_t* coeff_id; };
 
-// one thread per (matrix, row): counts[k * n_rows + row] = nonzeros make_row keeps
+// the matrix that holds slot t: the largest m with row0[m] <= t (row0[0] = 0; empty matrices share their row0 with the next)
+__device__ __forceinline__ uint32_t matrix_of(const uint64_t* __restrict__ row0, uint32_t n_mats, uint64_t t) {
+    uint32_t lo = 0, hi = n_mats;
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) / 2;
+        if (row0[mid] <= t) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+// one thread per slot: counts[t] = nonzeros make_row keeps for argument args[t]
 // total64: the same sum in 64 bits (one atomic per warp) -- the scan below is 32-bit and must not wrap unnoticed
-__global__ void lcmap_count_kernel(View v, LcArgs args, uint64_t n_rows, uint32_t* __restrict__ counts, uint32_t* __restrict__ err,
-                                   unsigned long long* __restrict__ total64) {
+// err_at: the lowest slot whose argument was rejected, so that the message can name it
+__global__ void lcmap_count_kernel(View v, const uint64_t* __restrict__ args, uint64_t n_slots, uint32_t* __restrict__ counts,
+                                   uint32_t* __restrict__ err, unsigned long long* __restrict__ total64,
+                                   unsigned long long* __restrict__ err_at) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= 3 * n_rows) return;
-    const uint32_t k = (uint32_t)(t / n_rows);
-    const uint64_t row = t - (uint64_t)k * n_rows;
+    if (t >= n_slots) return;
     uint32_t e = 0;
-    const uint32_t n = lcmap::count_row(v, args.a[k][row], &e);
+    const uint32_t n = lcmap::count_row(v, args[t], &e);
     counts[t] = n;
-    if (e) atomicOr(err, e);
+    if (e) {
+        atomicOr(err, e);
+        atomicMin(err_at, (unsigned long long)t);
+    }
     atomicAdd(total64, (unsigned long long)n);
 }
 
-// offsets: exclusive scan of counts over all 3 * n_rows entries (one scan for the three matrices); matrix k's entries
-// start at offsets[k * n_rows]
-__global__ void lcmap_fill_kernel(View v, LcArgs args, uint64_t n_rows, const uint32_t* __restrict__ offsets, LcOut out) {
+// bounds[m] = offsets[row0[m]], m <= n_mats: where matrix m's nonzeros start in the one scan over all slots
+__global__ void lcmap_bounds_kernel(const uint32_t* __restrict__ offsets, const uint64_t* __restrict__ row0, uint32_t n_mats,
+                                    uint32_t* __restrict__ bounds) {
+    const uint64_t m = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (m <= n_mats) bounds[m] = offsets[row0[m]];
+}
+
+// offsets: exclusive scan of counts over all n_slots slots.  Threads past the slots write the closing row_ptr entry of
+// matrix t - n_slots.
+__global__ void lcmap_fill_kernel(View v, const uint64_t* __restrict__ args, const uint64_t* __restrict__ row0, uint32_t n_mats,
+                                  uint64_t n_slots, const uint32_t* __restrict__ offsets, const LcOut* __restrict__ out) {
     const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t > 3 * n_rows) return;
-    if (t == 3 * n_rows) {      // closing entries of the three row_ptr arrays
-        for (uint32_t k = 0; k < 3; k++) out.row_ptr[k][n_rows] = (uint64_t)(offsets[(uint64_t)(k + 1) * n_rows] - offsets[(uint64_t)k * n_rows]);
+    if (t >= n_slots + n_mats) return;
+    if (t >= n_slots) {
+        const uint32_t m = (uint32_t)(t - n_slots);
+        out[m].row_ptr[row0[m + 1] - row0[m]] = (uint64_t)(offsets[row0[m + 1]] - offsets[row0[m]]);
         return;
     }
-    const uint32_t k = (uint32_t)(t / n_rows);
-    const uint64_t row = t - (uint64_t)k * n_rows;
-    const uint32_t base = offsets[(uint64_t)k * n_rows];
-    const uint32_t at = offsets[t] - base;
-    out.row_ptr[k][row] = at;
-    lcmap::fill_row(v, args.a[k][row], out.col[k] + at, out.coeff_id[k] + at);
+    const uint32_t m = matrix_of(row0, n_mats, t);
+    const uint32_t at = offsets[t] - offsets[row0[m]];
+    const LcOut o = out[m];
+    o.row_ptr[t - row0[m]] = at;
+    lcmap::fill_row(v, args[t], o.col + at, o.coeff_id + at);
+}
+
+int32_t lcmap_validate(Ctx* c, const LcMapHost& lm, uint64_t n_slots) {
+    if (lm.n_lcs == 0 || !lm.offsets || lm.offsets[0] != 0)
+        return fail(c, B2S_ERR_INVALID_ARG, "lcmap: offsets must start with 0 (LC 0 is the empty LC)");
+    if (lm.pool_len < 2 || !lm.pool) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: the interner pool holds at least ONE and -ONE");
+    if (n_slots >= (1ull << 32)) return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "lcmap: too many rows");
+    for (uint64_t j = 0; j < lm.n_lcs; j++)
+        if (lm.offsets[j + 1] < lm.offsets[j]) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: offsets not monotone at %llu", (unsigned long long)j);
+    return dispatch_curve(c, [&](auto curve) -> int32_t {
+        // pool[0] must be ONE: the SpMV and check kernels skip the multiplication for id 0 (sr1cs/mod.rs:42-46)
+        using FrP = typename decltype(curve)::FrP;
+        uint32_t one[8];
+        for (int i = 0; i < 8; i++) one[i] = FrP::r1(i);
+        if (memcmp(lm.pool, one, 32) != 0) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: pool[0] is not ONE (Montgomery form)");
+        return B2S_OK;
+    });
+}
+
+int32_t lcmap_build(Ctx* c, const LcMapHost& lm, uint64_t n_instance, uint64_t n_vars, const std::vector<LcMatrix>& mats,
+                    const char* what, const std::function<std::string(size_t, uint64_t)>& where, DevBuf& pool, uint32_t* pool_size) {
+    constexpr size_t FR_BYTES = 32;
+    const uint32_t M = (uint32_t)mats.size();
+    std::vector<uint64_t> row0(M + 1, 0);
+    for (uint32_t m = 0; m < M; m++) row0[m + 1] = row0[m] + mats[m].n_rows;
+    const uint64_t T = row0[M];                      // < 2^32: lcmap_validate
+    const uint64_t total = lm.offsets[lm.n_lcs];
+
+    // zero flags of the pool (byte comparison on the host; the pool is one entry per DISTINCT coefficient)
+    std::vector<uint8_t> is_zero(lm.pool_len);
+    {
+        const uint8_t* p = reinterpret_cast<const uint8_t*>(lm.pool);
+        static const uint8_t zeros[FR_BYTES] = {0};
+        for (uint32_t i = 0; i < lm.pool_len; i++) is_zero[i] = memcmp(p + (size_t)i * FR_BYTES, zeros, FR_BYTES) == 0;
+    }
+    B2S_TRY(pool.alloc(c, (size_t)lm.pool_len * FR_BYTES));
+    B2S_CUDA(c, cudaMemcpyAsync(pool.p, lm.pool, (size_t)lm.pool_len * FR_BYTES, cudaMemcpyHostToDevice, c->stream));
+    *pool_size = lm.pool_len;
+    if (M == 0) return B2S_OK;
+
+    DevBuf d_off, d_vars, d_coeffs, d_zero, d_args, d_row0, d_counts, d_offsets, d_task, d_err, d_bounds, d_out;
+    B2S_TRY(d_off.alloc(c, (lm.n_lcs + 1) * 8));
+    B2S_CUDA(c, cudaMemcpyAsync(d_off.p, lm.offsets, (lm.n_lcs + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    B2S_TRY(d_vars.alloc(c, total * 8));
+    B2S_TRY(d_coeffs.alloc(c, total * 4));
+    if (total) {
+        B2S_CUDA(c, cudaMemcpyAsync(d_vars.p, lm.vars, total * 8, cudaMemcpyHostToDevice, c->stream));
+        B2S_CUDA(c, cudaMemcpyAsync(d_coeffs.p, lm.coeffs, total * 4, cudaMemcpyHostToDevice, c->stream));
+    }
+    B2S_TRY(d_zero.alloc(c, lm.pool_len));
+    B2S_CUDA(c, cudaMemcpyAsync(d_zero.p, is_zero.data(), lm.pool_len, cudaMemcpyHostToDevice, c->stream));
+    B2S_TRY(d_args.alloc(c, T * 8));
+    for (uint32_t m = 0; m < M; m++) {
+        if (mats[m].n_rows)
+            B2S_CUDA(c, cudaMemcpyAsync(d_args.as<uint64_t>() + row0[m], mats[m].args, mats[m].n_rows * 8, cudaMemcpyHostToDevice, c->stream));
+        B2S_TRY(mats[m].row_ptr->alloc(c, (mats[m].n_rows + 1) * 8));
+    }
+    B2S_TRY(d_row0.alloc(c, (M + 1) * 8));
+    B2S_CUDA(c, cudaMemcpyAsync(d_row0.p, row0.data(), (M + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    View v{d_off.as<uint64_t>(), d_vars.as<uint64_t>(), d_coeffs.as<uint32_t>(), d_zero.as<uint8_t>(), lm.n_lcs, lm.pool_len, n_instance, n_vars};
+
+    B2S_TRY(d_err.alloc(c, 24));         // [0..3] error bits, [8..15] 64-bit nonzero total, [16..23] first rejected slot
+    B2S_CUDA(c, cudaMemsetAsync(d_err.p, 0, 16, c->stream));
+    B2S_CUDA(c, cudaMemsetAsync(d_err.as<uint8_t>() + 16, 0xFF, 8, c->stream));
+    unsigned long long* d_total64 = reinterpret_cast<unsigned long long*>(d_err.as<uint8_t>() + 8);
+    unsigned long long* d_err_at = reinterpret_cast<unsigned long long*>(d_err.as<uint8_t>() + 16);
+    B2S_TRY(d_offsets.alloc(c, (T + 1) * 4));
+    if (T) {
+        B2S_TRY(d_counts.alloc(c, T * 4));
+        B2S_TRY(d_task.alloc(c, (T + 1) * 4));
+        B2S_LAUNCH(c, lcmap_count_kernel, cdiv(T, 256), 256, 0, v, (const uint64_t*)d_args.as<uint64_t>(), T, d_counts.as<uint32_t>(),
+                   d_err.as<uint32_t>(), d_total64, d_err_at);
+        B2S_TRY(scan_counts(c, d_counts.as<uint32_t>(), (uint32_t)T, 1u, d_offsets.as<uint32_t>(), d_task.as<uint32_t>()));
+    } else {
+        B2S_CUDA(c, cudaMemsetAsync(d_offsets.p, 0, 4, c->stream));
+    }
+    B2S_TRY(d_bounds.alloc(c, (M + 1) * 4));
+    B2S_LAUNCH(c, lcmap_bounds_kernel, cdiv(M + 1, 256), 256, 0, (const uint32_t*)d_offsets.as<uint32_t>(),
+               (const uint64_t*)d_row0.as<uint64_t>(), M, d_bounds.as<uint32_t>());
+    std::vector<uint32_t> bounds(M + 1);
+    uint32_t h_err = 0;
+    unsigned long long h_total64 = 0, h_err_at = 0;
+    B2S_CUDA(c, cudaMemcpyAsync(bounds.data(), d_bounds.p, (M + 1) * 4, cudaMemcpyDeviceToHost, c->stream));
+    B2S_CUDA(c, cudaMemcpyAsync(&h_err, d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
+    B2S_CUDA(c, cudaMemcpyAsync(&h_total64, d_total64, 8, cudaMemcpyDeviceToHost, c->stream));
+    B2S_CUDA(c, cudaMemcpyAsync(&h_err_at, d_err_at, 8, cudaMemcpyDeviceToHost, c->stream));
+    B2S_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (h_err) {
+        const size_t m = (size_t)(std::upper_bound(row0.begin(), row0.end(), (uint64_t)h_err_at) - row0.begin()) - 1;
+        const std::string at = where ? where(m, h_err_at - row0[m]) : std::string();
+        if (h_err & lcmap::ERR_NESTED_LC)
+            return fail(c, B2S_ERR_INVALID_ARG, "%slcmap: a linear combination refers to another one -- call finalize() (inline_all_lcs) first",
+                        at.c_str());
+        if (h_err & lcmap::ERR_COLUMN)
+            return fail(c, B2S_ERR_ASSIGNMENT_MISSING, "%slcmap: a variable index is outside the %llu variables", at.c_str(),
+                        (unsigned long long)n_vars);
+        return fail(c, B2S_ERR_INVALID_ARG, "%slcmap: malformed input (error bits 0x%x: 1 tag, 2 lc index, 16 coefficient id)", at.c_str(), h_err);
+    }
+    if (h_total64 >> 32)
+        return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "lcmap: %llu nonzeros in %s together; the limit is 2^32 - 1", h_total64, what);
+    std::vector<LcOut> lo(M);
+    for (uint32_t m = 0; m < M; m++) {
+        *mats[m].nnz = (uint64_t)(bounds[m + 1] - bounds[m]);
+        B2S_TRY(mats[m].col->alloc(c, *mats[m].nnz * 4));
+        B2S_TRY(mats[m].coeff_id->alloc(c, *mats[m].nnz * 4));
+        lo[m] = {mats[m].row_ptr->as<uint64_t>(), mats[m].col->as<uint32_t>(), mats[m].coeff_id->as<uint32_t>()};
+    }
+    B2S_TRY(d_out.alloc(c, M * sizeof(LcOut)));
+    B2S_CUDA(c, cudaMemcpyAsync(d_out.p, lo.data(), M * sizeof(LcOut), cudaMemcpyHostToDevice, c->stream));
+    B2S_LAUNCH(c, lcmap_fill_kernel, cdiv(T + M, 256), 256, 0, v, (const uint64_t*)d_args.as<uint64_t>(), (const uint64_t*)d_row0.as<uint64_t>(),
+               M, T, (const uint32_t*)d_offsets.as<uint32_t>(), (const LcOut*)d_out.as<LcOut>());
+    B2S_CUDA(c, cudaStreamSynchronize(c->stream));   // host inputs may be released by the caller after return
+    return B2S_OK;
 }
 
 int32_t r1cs_upload_lcmap(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness, const uint64_t* const args[3],
@@ -52,98 +188,19 @@ int32_t r1cs_upload_lcmap(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t
                           const void* pool, uint32_t pool_len, b2s_r1cs** out) {
     return dispatch_curve(c, [&](auto curve) -> int32_t {
         using FrP = typename decltype(curve)::FrP;
-        constexpr size_t FR_BYTES = 32;
-        const uint64_t n_vars = n_instance + n_witness;
         if (n_instance == 0) return fail(c, B2S_ERR_INVALID_ARG, "r1cs: n_instance counts the constant One and must be >= 1");
-        if (n_lcs == 0 || !lc_offsets || lc_offsets[0] != 0) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: offsets must start with 0 (LC 0 is the empty LC)");
-        if (pool_len < 2 || !pool) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: the interner pool holds at least ONE and -ONE");
-        if (3 * n_rows >= (1ull << 32)) return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "lcmap: too many rows");
-        for (uint64_t j = 0; j < n_lcs; j++)
-            if (lc_offsets[j + 1] < lc_offsets[j]) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: offsets not monotone at %llu", (unsigned long long)j);
-        const uint64_t total = lc_offsets[n_lcs];
-        {   // pool[0] must be ONE: the SpMV kernel skips the multiplication for id 0 (sr1cs/mod.rs:42-46)
-            uint32_t one[8];
-            for (int i = 0; i < 8; i++) one[i] = FrP::r1(i);
-            if (memcmp(pool, one, FR_BYTES) != 0) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: pool[0] is not ONE (Montgomery form)");
-        }
+        const LcMapHost lm{n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len};
+        B2S_TRY(lcmap_validate(c, lm, 3 * n_rows));
         uint32_t logd = 0;
         while ((1ull << logd) < n_rows + n_instance) logd++;
         if (logd > (uint32_t)FrP::TWO_ADICITY || logd > 27) return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "r1cs: domain 2^%u unsupported", logd);
 
-        // zero flags of the pool (byte comparison on the host; the pool is one entry per DISTINCT coefficient)
-        std::vector<uint8_t> is_zero(pool_len);
-        {
-            const uint8_t* p = reinterpret_cast<const uint8_t*>(pool);
-            static const uint8_t zeros[FR_BYTES] = {0};
-            for (uint32_t i = 0; i < pool_len; i++) is_zero[i] = memcmp(p + (size_t)i * FR_BYTES, zeros, FR_BYTES) == 0;
-        }
-
-        b2s_r1cs* m = new b2s_r1cs();
+        std::unique_ptr<b2s_r1cs> m(new b2s_r1cs());
         m->n_rows = n_rows; m->n_instance = n_instance; m->n_witness = n_witness; m->log_domain = logd;
-        m->pool_size = pool_len;
-        int32_t st = [&]() -> int32_t {
-            DevBuf d_off, d_vars, d_coeffs, d_zero, d_args[3], d_counts, d_offsets, d_task, d_err;
-            B2S_TRY(m->pool.alloc(c, (size_t)pool_len * FR_BYTES));
-            B2S_CUDA(c, cudaMemcpyAsync(m->pool.p, pool, (size_t)pool_len * FR_BYTES, cudaMemcpyHostToDevice, c->stream));
-            B2S_TRY(d_off.alloc(c, (n_lcs + 1) * 8));
-            B2S_CUDA(c, cudaMemcpyAsync(d_off.p, lc_offsets, (n_lcs + 1) * 8, cudaMemcpyHostToDevice, c->stream));
-            B2S_TRY(d_vars.alloc(c, total * 8));
-            B2S_TRY(d_coeffs.alloc(c, total * 4));
-            if (total) {
-                B2S_CUDA(c, cudaMemcpyAsync(d_vars.p, lc_vars, total * 8, cudaMemcpyHostToDevice, c->stream));
-                B2S_CUDA(c, cudaMemcpyAsync(d_coeffs.p, lc_coeffs, total * 4, cudaMemcpyHostToDevice, c->stream));
-            }
-            B2S_TRY(d_zero.alloc(c, pool_len));
-            B2S_CUDA(c, cudaMemcpyAsync(d_zero.p, is_zero.data(), pool_len, cudaMemcpyHostToDevice, c->stream));
-            LcArgs la{};
-            for (int k = 0; k < 3; k++) {
-                B2S_TRY(d_args[k].alloc(c, n_rows * 8));
-                if (n_rows) B2S_CUDA(c, cudaMemcpyAsync(d_args[k].p, args[k], n_rows * 8, cudaMemcpyHostToDevice, c->stream));
-                la.a[k] = d_args[k].as<uint64_t>();
-                B2S_TRY(m->row_ptr[k].alloc(c, (n_rows + 1) * 8));
-            }
-            View v{d_off.as<uint64_t>(), d_vars.as<uint64_t>(), d_coeffs.as<uint32_t>(), d_zero.as<uint8_t>(), n_lcs, pool_len, n_instance, n_vars};
-            const uint64_t n3 = 3 * n_rows;
-            B2S_TRY(d_err.alloc(c, 16));         // [0..3] error bits, [8..15] 64-bit nonzero total
-            B2S_CUDA(c, cudaMemsetAsync(d_err.p, 0, 16, c->stream));
-            unsigned long long* d_total64 = reinterpret_cast<unsigned long long*>(d_err.as<uint8_t>() + 8);
-            uint32_t h_tot[4] = {0, 0, 0, 0};   // offsets[0], [n_rows], [2 n_rows], [3 n_rows]
-            uint32_t h_err = 0;
-            unsigned long long h_total64 = 0;
-            if (n_rows) {
-                B2S_TRY(d_counts.alloc(c, n3 * 4));
-                B2S_TRY(d_offsets.alloc(c, (n3 + 1) * 4));
-                B2S_TRY(d_task.alloc(c, (n3 + 1) * 4));
-                B2S_LAUNCH(c, lcmap_count_kernel, cdiv(n3, 256), 256, 0, v, la, n_rows, d_counts.as<uint32_t>(), d_err.as<uint32_t>(), d_total64);
-                B2S_TRY(scan_counts(c, d_counts.as<uint32_t>(), (uint32_t)n3, 1u, d_offsets.as<uint32_t>(), d_task.as<uint32_t>()));
-                for (int k = 1; k <= 3; k++)
-                    B2S_CUDA(c, cudaMemcpyAsync(&h_tot[k], d_offsets.as<uint32_t>() + (uint64_t)k * n_rows, 4, cudaMemcpyDeviceToHost, c->stream));
-            }
-            B2S_CUDA(c, cudaMemcpyAsync(&h_err, d_err.p, 4, cudaMemcpyDeviceToHost, c->stream));
-            B2S_CUDA(c, cudaMemcpyAsync(&h_total64, d_total64, 8, cudaMemcpyDeviceToHost, c->stream));
-            B2S_CUDA(c, cudaStreamSynchronize(c->stream));
-            if (h_err & (lcmap::ERR_NESTED_LC))
-                return fail(c, B2S_ERR_INVALID_ARG, "lcmap: a linear combination refers to another one -- call finalize() (inline_all_lcs) first");
-            if (h_err & lcmap::ERR_COLUMN) return fail(c, B2S_ERR_ASSIGNMENT_MISSING, "lcmap: a variable index is outside the %llu variables", (unsigned long long)n_vars);
-            if (h_err) return fail(c, B2S_ERR_INVALID_ARG, "lcmap: malformed input (error bits 0x%x: 1 tag, 2 lc index, 16 coefficient id)", h_err);
-            if (h_total64 >> 32) return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "lcmap: %llu nonzeros in A, B, C together; the limit is 2^32 - 1", h_total64);
-            LcOut lo{};
-            for (int k = 0; k < 3; k++) {
-                m->nnz[k] = (uint64_t)(h_tot[k + 1] - h_tot[k]);
-                B2S_TRY(m->col[k].alloc(c, m->nnz[k] * 4));
-                B2S_TRY(m->coeff_id[k].alloc(c, m->nnz[k] * 4));
-                lo.row_ptr[k] = m->row_ptr[k].as<uint64_t>(); lo.col[k] = m->col[k].as<uint32_t>(); lo.coeff_id[k] = m->coeff_id[k].as<uint32_t>();
-            }
-            if (n_rows) {
-                B2S_LAUNCH(c, lcmap_fill_kernel, cdiv(n3 + 1, 256), 256, 0, v, la, n_rows, (const uint32_t*)d_offsets.as<uint32_t>(), lo);
-            } else {
-                for (int k = 0; k < 3; k++) B2S_CUDA(c, cudaMemsetAsync(m->row_ptr[k].p, 0, 8, c->stream));
-            }
-            B2S_CUDA(c, cudaStreamSynchronize(c->stream));   // host inputs may be released by the caller after return
-            return B2S_OK;
-        }();
-        if (st != B2S_OK) { delete m; return st; }
-        *out = m;
+        std::vector<LcMatrix> mats;
+        for (int k = 0; k < 3; k++) mats.push_back({args[k], n_rows, &m->row_ptr[k], &m->col[k], &m->coeff_id[k], &m->nnz[k]});
+        B2S_TRY(lcmap_build(c, lm, n_instance, n_instance + n_witness, mats, "A, B, C", nullptr, m->pool, &m->pool_size));
+        *out = m.release();
         return B2S_OK;
     });
 }

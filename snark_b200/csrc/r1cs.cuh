@@ -1,8 +1,11 @@
 // Device-resident R1CS matrices, GR1CS predicates and Groth16 proving key (the handles behind b2s_r1cs / b2s_gr1cs / b2s_pk).
 #pragma once
 #include <cstring>
+#include <functional>
 #include <memory>
+#include <string>
 #include <unordered_map>
+#include <vector>
 
 #include "common.cuh"
 
@@ -90,6 +93,10 @@ int32_t coeff_pool_upload(Ctx* c, const CoeffInterner& in, const char* who, DevB
 // gr1cs.cu
 int32_t gr1cs_upload(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_desc* preds,
                      b2s_gr1cs** out);
+// the same handle from the constraint system's LcMap: the argument matrices by lcmap_build, the pool kept as the caller's
+struct LcMapHost;
+int32_t gr1cs_upload_lcmap(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_lcmap_desc* preds,
+                           const LcMapHost& lm, b2s_gr1cs** out);
 // first_unsat / n_unsat (n_unsat may be null): n_assign x n_predicates, in `mem` like z
 int32_t gr1cs_check(Ctx* c, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
 int32_t r1cs_check(Ctx* c, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
@@ -145,7 +152,32 @@ inline bool pk_is_full(const b2s_pk* pk) {
 
 int32_t r1cs_upload(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness, const uint64_t* const row_ptr[3],
                     const uint32_t* const col[3], const void* const coeff[3], b2s_r1cs** out);
-// lcmap.cu: the same handle from the constraint system's LcMap, CSR built by kernels
+// lcmap.cu: argument matrices built on the device from the constraint system's flat LcMap (lcmap.cuh), shared by
+// b2s_r1cs_upload_lcmap (A, B, C) and b2s_gr1cs_upload_lcmap (every argument of every predicate)
+struct LcMapHost {               // host pointers, as the caller holds them
+    uint64_t n_lcs;
+    const uint64_t* offsets;     // n_lcs + 1
+    const uint64_t* vars;        // offsets[n_lcs] raw Variables
+    const uint32_t* coeffs;      // offsets[n_lcs] ids into pool
+    const void* pool;            // pool_len Montgomery Fr, pool[0] = ONE
+    uint32_t pool_len;
+};
+// one argument matrix: n_rows raw Variables in (host), a CSR whose coefficient ids index the caller's pool out
+struct LcMatrix {
+    const uint64_t* args;
+    uint64_t n_rows;
+    DevBuf* row_ptr;             // uint64[n_rows + 1]
+    DevBuf* col;                 // uint32[nnz]
+    DevBuf* coeff_id;            // uint32[nnz]
+    uint64_t* nnz;
+};
+// The checks of the LcMap itself, made before anything is allocated; n_slots: the rows of all matrices together.
+int32_t lcmap_validate(Ctx* c, const LcMapHost& lm, uint64_t n_slots);
+// Builds every matrix of `mats` with one count, scan and fill over all their rows and copies the pool as it is to `pool`.
+// where(m, row), when set, prefixes the message of a rejected argument; `what` names the matrices in the nonzero limit's.
+int32_t lcmap_build(Ctx* c, const LcMapHost& lm, uint64_t n_instance, uint64_t n_vars, const std::vector<LcMatrix>& mats,
+                    const char* what, const std::function<std::string(size_t, uint64_t)>& where, DevBuf& pool, uint32_t* pool_size);
+// the same handle as r1cs_upload from the constraint system's LcMap
 int32_t r1cs_upload_lcmap(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness, const uint64_t* const args[3],
                           uint64_t n_lcs, const uint64_t* lc_offsets, const uint64_t* lc_vars, const uint32_t* lc_coeffs,
                           const void* pool, uint32_t pool_len, b2s_r1cs** out);

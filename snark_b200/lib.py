@@ -62,6 +62,15 @@ class PredicateDesc(ctypes.Structure):
     ]
 
 
+class PredicateLcmapDesc(ctypes.Structure):
+    _fields_ = [
+        ("arity", c_uint32), ("n_terms", c_uint32),
+        ("term_coeffs", c_void_p), ("term_offsets", c_void_p), ("factor_var", c_void_p), ("factor_pow", c_void_p),
+        ("n_rows", c_uint64),
+        ("args", c_void_p * GR1CS_MAX_ARITY),
+    ]
+
+
 def _mont_limbs(r, xs):
     """Python ints -> uint32[len(xs) * 8] Montgomery limbs mod r"""
     out = np.zeros((len(xs), 8), dtype=np.uint32)
@@ -69,6 +78,16 @@ def _mont_limbs(r, xs):
         v = (x % r) * (1 << 256) % r
         out[i] = [(v >> (32 * j)) & 0xFFFFFFFF for j in range(8)]
     return out.reshape(-1)
+
+
+def _set_poly(d, r, terms, keep):
+    """the polynomial fields of a predicate descriptor from terms [(coeff, [(argument, exponent), ...])]; the arrays go to keep"""
+    offs = np.zeros(len(terms) + 1, dtype=np.uint32)
+    offs[1:] = np.cumsum([len(mono) for _, mono in terms])
+    arrs = [_mont_limbs(r, [c for c, _ in terms]), offs, np.array([v for _, mono in terms for v, _ in mono], dtype=np.uint32),
+            np.array([e for _, mono in terms for _, e in mono], dtype=np.uint32)]
+    keep += arrs
+    d.term_coeffs, d.term_offsets, d.factor_var, d.factor_pow = (a.ctypes.data for a in arrs)
 
 
 def _csr(r, matrix):
@@ -117,6 +136,8 @@ SIGNATURES = {
     "b2s_r1cs_domain_size": (c_uint64, [c_void_p]),
     "b2s_witness_map_sim": (c_int32, [c_void_p, c_void_p, c_void_p, c_int32, c_uint32, c_void_p]),
     "b2s_gr1cs_upload": (c_int32, [c_void_p, c_uint64, c_uint64, c_uint32, c_void_p, POINTER(c_void_p)]),
+    "b2s_gr1cs_upload_lcmap": (c_int32, [c_void_p, c_uint64, c_uint64, c_uint32, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p,
+                                         c_void_p, c_uint32, POINTER(c_void_p)]),
     "b2s_gr1cs_free": (None, [c_void_p, c_void_p]),
     "b2s_gr1cs_check": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_void_p]),
     "b2s_r1cs_check": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_void_p]),
@@ -439,19 +460,41 @@ class Backend:
         keep = []
         for d, label in zip(descs, labels):
             arity, terms, mats = predicates[label]
-            offs = np.zeros(len(terms) + 1, dtype=np.uint32)
-            offs[1:] = np.cumsum([len(mono) for _, mono in terms])
-            arrs = [_mont_limbs(r, [c for c, _ in terms]), offs, np.array([v for _, mono in terms for v, _ in mono], dtype=np.uint32),
-                    np.array([e for _, mono in terms for _, e in mono], dtype=np.uint32)]
-            keep += arrs
             d.arity, d.n_terms, d.n_rows = arity, len(terms), len(mats[0]) if mats else 0
-            d.term_coeffs, d.term_offsets, d.factor_var, d.factor_pow = (a.ctypes.data for a in arrs)
+            _set_poly(d, r, terms, keep)
             for j, m in enumerate(mats[:GR1CS_MAX_ARITY]):
                 csr = _csr(r, m)
                 keep += csr
                 d.row_ptr[j], d.col[j], d.coeff[j] = (a.ctypes.data for a in csr)
         h = c_void_p()
         self._ck(self.lib.b2s_gr1cs_upload(self.h, n_instance, n_witness, len(labels), descs, ctypes.byref(h)))
+        return Gr1cs(h, labels, n_instance + n_witness)
+
+    def gr1cs_upload_lcmap(self, n_instance, n_witness, predicates, lcmap):
+        """The same Gr1cs, built on the device from the constraint system's LcMap.  predicates: {label: (arity, terms)} as for
+        gr1cs_upload without the matrices; lcmap: the flat storage of every predicate -- offsets (n_lcs + 1), vars
+        (raw Variables), coeffs (ids into pool), pool (Python ints, pool[0] = 1) and args {label: one sequence of raw Variables
+        per argument, one Variable per constraint}; lists or numpy arrays.  Uploaded in sorted label order."""
+        r = FR_MODULUS[self.curve]
+        labels = sorted(predicates)
+        descs = (PredicateLcmapDesc * max(len(labels), 1))()
+        keep = []
+        for d, label in zip(descs, labels):
+            arity, terms = predicates[label]
+            args = [np.ascontiguousarray(a, dtype=np.uint64) for a in lcmap["args"][label]]
+            keep += args
+            d.arity, d.n_terms, d.n_rows = arity, len(terms), len(args[0]) if args else 0
+            _set_poly(d, r, terms, keep)
+            for j, a in enumerate(args[:GR1CS_MAX_ARITY]):
+                d.args[j] = a.ctypes.data
+        off = np.ascontiguousarray(lcmap["offsets"], dtype=np.uint64)
+        lc_vars = np.ascontiguousarray(lcmap["vars"], dtype=np.uint64)
+        lc_coeffs = np.ascontiguousarray(lcmap["coeffs"], dtype=np.uint32)
+        pool = _mont_limbs(r, lcmap["pool"])
+        h = c_void_p()
+        self._ck(self.lib.b2s_gr1cs_upload_lcmap(self.h, n_instance, n_witness, len(labels), descs, len(off) - 1, off.ctypes.data,
+                                                 lc_vars.ctypes.data, lc_coeffs.ctypes.data, pool.ctypes.data, len(lcmap["pool"]),
+                                                 ctypes.byref(h)))
         return Gr1cs(h, labels, n_instance + n_witness)
 
     def gr1cs_free(self, g):
