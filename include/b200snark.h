@@ -243,6 +243,44 @@ int32_t b2s_gr1cs_check(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, con
 int32_t b2s_r1cs_check(b2s_ctx* ctx, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem,
                        uint64_t* first_unsat, uint64_t* n_unsat);
 
+/* ---- R1CS -> square R1CS (Sr1csAdapter, relations/src/sr1cs/mod.rs:18-265) ----------------------------------------------
+ *   b2s_r1cs_to_sr1cs     Sr1csAdapter::r1cs_to_sr1cs (sr1cs/mod.rs:124-183), built on the device.  Row i of a * b = c becomes
+ *                         (a + b)^2 = 4c + s_i (row 2i) and (a - b)^2 = s_i (row 2i + 1), one new witness s_i per row.  Scanning
+ *                         the rows in order (A_i, B_i, C_i as stored, then s_i), every column other than ONE gets the next
+ *                         witness the first time it occurs, public and private alike; unused columns are dropped.  Each used
+ *                         public column p_k (increasing p) gets the input 1 + k and the row 2m + k: w(p_k) - x_k = 0 squared.
+ *                         Result: one predicate "SR1CS" of arity 2, polynomial x0^2 - x1, 2m + P rows; n_instance = 1 + P,
+ *                         n_witness = (used columns other than ONE) + m; witness w at column 1 + P + w.  Repeated columns
+ *                         stay and the order of terms within a row may differ from the reference's; row sums are exactly its.
+ *                         The pool becomes [pool | -pool | 4 pool].  The handle records what b2s_sr1cs_assignment needs and
+ *                         holds no pointer to m, which may be freed.  A handle whose C was left empty for the circom
+ *                         reduction (b2s_zkey_load) converts a * b = 0.  B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE for 2^32 or
+ *                         more variables or constraints in the result, or for 2^32 or more nonzeros plus rows in m.
+ *   b2s_sr1cs_assignment  with the call above, Sr1csAdapter::r1cs_to_sr1cs_with_assignment (sr1cs/mod.rs:191-265): z holds
+ *                         n_assign rows of m's n_instance + n_witness Montgomery Fr, out_z receives n_assign rows of the
+ *                         result's n_instance + n_witness: z'[0] = 1, z'[1 + k] = z[p_k], a column's witness z[col], and
+ *                         s_i = (<A_i, z> - <B_i, z>)^2 (ONE terms read 1).  z and out_z share `mem`; host batches go through
+ *                         bounded device scratch in chunks.  n_assign == 0 -> B2S_OK.  B2S_ERR_INVALID_ARG for a handle
+ *                         that b2s_r1cs_to_sr1cs did not make.
+ *   b2s_gr1cs_info        the shape of any b2s_gr1cs handle: n_vars[0] = n_instance, n_vars[1] = n_witness, *n_predicates, and
+ *                         for the first min(cap, n_predicates) predicates (upload order) their arity, rows and nonzeros.
+ *   b2s_gr1cs_export      argument `arg` of predicate `pred` as to_matrices() holds it, in CSR to HOST buffers of the given
+ *                         byte capacities: row_ptr (n_rows + 1 u64), col (nnz u32), coeff (nnz Montgomery Fr, pool ids
+ *                         resolved).  B2S_ERR_INVALID_ARG for a buffer too small or an index out of range.
+ * A handle from another curve's ctx, or a null pointer, is B2S_ERR_INVALID_ARG. */
+typedef struct b2s_gr1cs_pred_info {
+    uint32_t arity;
+    uint32_t reserved;
+    uint64_t n_rows;
+    uint64_t nnz[B2S_GR1CS_MAX_ARITY];     /* argument j < arity */
+} b2s_gr1cs_pred_info;
+int32_t b2s_r1cs_to_sr1cs(b2s_ctx* ctx, const b2s_r1cs* m, b2s_gr1cs** out);
+int32_t b2s_sr1cs_assignment(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, void* out_z);
+int32_t b2s_gr1cs_info(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_vars[2], uint32_t* n_predicates, b2s_gr1cs_pred_info* preds,
+                       uint32_t cap);
+int32_t b2s_gr1cs_export(b2s_ctx* ctx, const b2s_gr1cs* g, uint32_t pred, uint32_t arg, uint64_t* row_ptr, uint64_t cap_row_ptr,
+                         uint32_t* col, uint64_t cap_col, void* coeff, uint64_t cap_coeff);
+
 /* ---- Groth16 (ark-groth16 ProvingKey / create_proof_with_reduction, SURVEY App. A.1) ------------
  * Query vectors are affine point arrays in HOST or DEVICE memory (`mem`); they are copied to the GPU.
  *   a_query, b_g1_query, b_g2_query: n_vars = n_instance + n_witness points

@@ -7,7 +7,7 @@ use ark_groth16::{Groth16, PreparedVerifyingKey, Proof, ProvingKey, VerifyingKey
 use ark_ff::PrimeField;
 use ark_relations::utils::variable::{VarKind, Variable};
 use ark_relations::gr1cs::{
-    predicate::{polynomial_constraint::PolynomialPredicate, Predicate}, ConstraintSynthesizer, ConstraintSystem, Label, Matrix, OptimizationGoal, SynthesisError,
+    predicate::{polynomial_constraint::{PolynomialPredicate, SR1CS_PREDICATE_LABEL}, Predicate}, ConstraintSynthesizer, ConstraintSystem, Label, Matrix, OptimizationGoal, SynthesisError,
     R1CS_PREDICATE_LABEL,
 };
 use ark_snark::{CircuitSpecificSetupSNARK, SNARK};
@@ -155,6 +155,23 @@ extern "C" {
                            n_unsat: *mut u64) -> i32;
     pub fn b2s_r1cs_check(ctx: *mut B2sCtx, m: *const B2sR1cs, n_assign: u64, z: *const c_void, mem: i32, first_unsat: *mut u64,
                           n_unsat: *mut u64) -> i32;
+    /// Sr1csAdapter::r1cs_to_sr1cs (relations/src/sr1cs/mod.rs:124-183)
+    pub fn b2s_r1cs_to_sr1cs(ctx: *mut B2sCtx, m: *const B2sR1cs, out: *mut *mut B2sGr1cs) -> i32;
+    /// with b2s_r1cs_to_sr1cs: Sr1csAdapter::r1cs_to_sr1cs_with_assignment (sr1cs/mod.rs:191-265)
+    pub fn b2s_sr1cs_assignment(ctx: *mut B2sCtx, g: *const B2sGr1cs, n_assign: u64, z: *const c_void, mem: i32,
+                                out_z: *mut c_void) -> i32;
+    pub fn b2s_gr1cs_info(ctx: *mut B2sCtx, g: *const B2sGr1cs, n_vars: *mut u64, n_predicates: *mut u32,
+                          preds: *mut B2sGr1csPredInfo, cap: u32) -> i32;
+    pub fn b2s_gr1cs_export(ctx: *mut B2sCtx, g: *const B2sGr1cs, pred: u32, arg: u32, row_ptr: *mut u64, cap_row_ptr: u64,
+                            col: *mut u32, cap_col: u64, coeff: *mut c_void, cap_coeff: u64) -> i32;
+}
+#[repr(C)]
+#[derive(Clone, Copy, Default)]
+pub struct B2sGr1csPredInfo {
+    pub arity: u32,
+    pub reserved: u32,
+    pub n_rows: u64,
+    pub nnz: [u64; B2S_GR1CS_MAX_ARITY],
 }
 #[repr(C)]
 pub struct B2sGroup {
@@ -711,4 +728,79 @@ fn poly_terms<F: PrimeField>(p: &PolynomialPredicate<F>) -> (u32, Vec<F>, Vec<u3
 
 impl<F: PrimeField> Drop for Gr1csB200<F> {
     fn drop(&mut self) { unsafe { b2s_gr1cs_free(self.ctx, self.g); b2s_ctx_destroy(self.ctx); } }
+}
+
+impl<F: PrimeField> Gr1csB200<F> {
+    /// `to_matrices()` of one argument of one predicate (upload order), read back from the device: (row_ptr, col, coeff)
+    pub fn export(&self, pred: u32, arg: u32) -> Result<(Vec<u64>, Vec<u32>, Vec<F>), B200Error> {
+        let (mut nv, mut np) = ([0u64; 2], 0u32);
+        check(self.ctx, unsafe { b2s_gr1cs_info(self.ctx, self.g, nv.as_mut_ptr(), &mut np, core::ptr::null_mut(), 0) })?;
+        let mut info = vec![B2sGr1csPredInfo::default(); np as usize];
+        check(self.ctx, unsafe { b2s_gr1cs_info(self.ctx, self.g, nv.as_mut_ptr(), &mut np, info.as_mut_ptr(), np) })?;
+        let p = info.get(pred as usize).ok_or(B200Error::Backend(ERR_INVALID_ARG))?;
+        if arg >= p.arity { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        let nnz = p.nnz[arg as usize] as usize;
+        let (mut rp, mut col, mut co) = (vec![0u64; p.n_rows as usize + 1], vec![0u32; nnz], vec![F::zero(); nnz]);
+        check(self.ctx, unsafe {
+            b2s_gr1cs_export(self.ctx, self.g, pred, arg, rp.as_mut_ptr(), (rp.len() * 8) as u64, col.as_mut_ptr(), (nnz * 4) as u64,
+                             co.as_mut_ptr().cast(), (nnz * core::mem::size_of::<F>()) as u64)
+        })?;
+        Ok((rp, col, co))
+    }
+}
+
+/// `Sr1csAdapter` (relations/src/sr1cs/mod.rs:18-265) on the GPU: the square R1CS of `cs`'s R1CS predicate, built on the
+/// device, and the conversion of assignments.  `gr1cs` is the converted system (predicate "SR1CS", x0^2 - x1), checked and
+/// exported like any other.
+pub struct Sr1csB200<F: PrimeField> {
+    pub gr1cs: Gr1csB200<F>,
+    /// n_instance + n_witness of the source: the length of every assignment `assignment` takes
+    pub src_vars: usize,
+}
+
+impl<F: PrimeField> Sr1csB200<F> {
+    /// `r1cs_to_sr1cs(cs)`: uploads the R1CS predicate of `cs.to_matrices()`, converts it and frees the upload
+    pub fn r1cs_to_sr1cs(curve_id: i32, cs: &ConstraintSystem<F>) -> Result<Self, B200Error> {
+        Gr1csB200::<F>::check_curve(curve_id)?;
+        let mats = cs.to_matrices()?;
+        let r1cs = mats.get(R1CS_PREDICATE_LABEL).ok_or(B200Error::Backend(ERR_INVALID_ARG))?;
+        let csr: Vec<_> = r1cs.iter().map(to_csr).collect();
+        let src_vars = cs.num_instance_variables() + cs.num_witness_variables();
+        let mut ctx: *mut B2sCtx = core::ptr::null_mut();
+        check(ctx, unsafe { b2s_ctx_create(curve_id, 0, &mut ctx) })?;
+        let rp: Vec<*const u64> = csr.iter().map(|m| m.0.as_ptr()).collect();
+        let col: Vec<*const u32> = csr.iter().map(|m| m.1.as_ptr()).collect();
+        let co: Vec<*const c_void> = csr.iter().map(|m| m.2.as_ptr().cast()).collect();
+        let mut m: *mut B2sR1cs = core::ptr::null_mut();
+        let mut g: *mut B2sGr1cs = core::ptr::null_mut();
+        let mut st = unsafe {
+            b2s_r1cs_upload(ctx, csr[0].0.len() as u64 - 1, cs.num_instance_variables() as u64, cs.num_witness_variables() as u64,
+                            rp.as_ptr(), col.as_ptr(), co.as_ptr(), &mut m)
+        };
+        if st == 0 {
+            st = unsafe { b2s_r1cs_to_sr1cs(ctx, m, &mut g) };
+            unsafe { b2s_r1cs_free(ctx, m) };
+        }
+        let mut nv = [0u64; 2];
+        let mut np = 0u32;
+        if st == 0 { st = unsafe { b2s_gr1cs_info(ctx, g, nv.as_mut_ptr(), &mut np, core::ptr::null_mut(), 0) }; }
+        if let Err(e) = check(ctx, st) {
+            unsafe { b2s_gr1cs_free(ctx, g); b2s_ctx_destroy(ctx) };
+            return Err(e);
+        }
+        let gr1cs = Gr1csB200 { ctx, g, labels: vec![SR1CS_PREDICATE_LABEL.to_string()], n_vars: (nv[0] + nv[1]) as usize,
+                                _f: core::marker::PhantomData };
+        Ok(Sr1csB200 { gr1cs, src_vars })
+    }
+
+    /// the assignment `r1cs_to_sr1cs_with_assignment` gives the converted system for the source's z = instance || witness:
+    /// instance' || witness'.  A z whose length is not `src_vars` is `SynthesisError::AssignmentMissing`.
+    pub fn assignment(&self, z: &[F]) -> Result<Vec<F>, B200Error> {
+        if z.len() != self.src_vars { return Err(SynthesisError::AssignmentMissing.into()); }
+        let mut out = vec![F::zero(); self.gr1cs.n_vars];
+        check(self.gr1cs.ctx, unsafe {
+            b2s_sr1cs_assignment(self.gr1cs.ctx, self.gr1cs.g, 1, z.as_ptr().cast(), 0, out.as_mut_ptr().cast())
+        })?;
+        Ok(out)
+    }
 }

@@ -439,6 +439,33 @@ int32_t b2s_r1cs_check(b2s_ctx* ctx, const b2s_r1cs* m, uint64_t n_assign, const
     return r1cs_check(ctx, m, n_assign, z, mem, first_unsat, n_unsat);
 }
 
+int32_t b2s_r1cs_to_sr1cs(b2s_ctx* ctx, const b2s_r1cs* m, b2s_gr1cs** out) {
+    LOCK(ctx);
+    if (!m || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_to_sr1cs: null argument");
+    *out = nullptr;
+    return r1cs_to_sr1cs(ctx, m, out);
+}
+
+int32_t b2s_sr1cs_assignment(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, void* out_z) {
+    LOCK(ctx);
+    if (!g || (n_assign && (!z || !out_z))) return fail(ctx, B2S_ERR_INVALID_ARG, "sr1cs_assignment: null argument");
+    return sr1cs_assignment(ctx, g, n_assign, z, mem, out_z);
+}
+
+int32_t b2s_gr1cs_info(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_vars[2], uint32_t* n_predicates, b2s_gr1cs_pred_info* preds,
+                       uint32_t cap) {
+    LOCK(ctx);
+    if (!g || !n_vars || !n_predicates || (cap && !preds)) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_info: null argument");
+    return gr1cs_info(ctx, g, n_vars, n_predicates, preds, cap);
+}
+
+int32_t b2s_gr1cs_export(b2s_ctx* ctx, const b2s_gr1cs* g, uint32_t pred, uint32_t arg, uint64_t* row_ptr, uint64_t cap_row_ptr,
+                         uint32_t* col, uint64_t cap_col, void* coeff, uint64_t cap_coeff) {
+    LOCK(ctx);
+    if (!g || !row_ptr || (cap_col && !col) || (cap_coeff && !coeff)) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_export: null argument");
+    return gr1cs_export(ctx, g, pred, arg, row_ptr, cap_row_ptr, col, cap_col, coeff, cap_coeff);
+}
+
 int32_t b2s_pk_upload(b2s_ctx* ctx, const b2s_pk_desc* desc, int32_t mem, b2s_pk** out) {
     LOCK(ctx);
     if (!desc || !out) return fail(ctx, B2S_ERR_INVALID_ARG, "pk_upload: null argument");

@@ -45,6 +45,10 @@ struct b2s_gr1cs {
     b2s::DevBuf pool;                     // Fr[pool_size], shared by every predicate; id 0 == ONE
     uint32_t pool_size = 0;
     std::vector<std::unique_ptr<b2s::Gr1csPredicate>> preds;   // upload order
+    // set by b2s_r1cs_to_sr1cs only: orig[new column] = the source column it copies (ONE and squares: 0), the source's
+    // n_instance + n_witness and rows; what b2s_sr1cs_assignment needs besides the predicate itself
+    b2s::DevBuf sr1cs_orig;               // uint32[n_instance + n_witness]
+    uint64_t sr1cs_src_vars = 0, sr1cs_rows = 0;
 };
 
 namespace b2s {
@@ -100,6 +104,12 @@ int32_t gr1cs_upload_lcmap(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint
 // first_unsat / n_unsat (n_unsat may be null): n_assign x n_predicates, in `mem` like z
 int32_t gr1cs_check(Ctx* c, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
 int32_t r1cs_check(Ctx* c, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
+// sr1cs.cu: the square R1CS of an R1CS handle, its assignments, and the read-back of any GR1CS handle
+int32_t r1cs_to_sr1cs(Ctx* c, const b2s_r1cs* m, b2s_gr1cs** out);
+int32_t sr1cs_assignment(Ctx* c, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, void* out_z);
+int32_t gr1cs_info(Ctx* c, const b2s_gr1cs* g, uint64_t* n_vars, uint32_t* n_predicates, b2s_gr1cs_pred_info* preds, uint32_t cap);
+int32_t gr1cs_export(Ctx* c, const b2s_gr1cs* g, uint32_t pred, uint32_t arg, uint64_t* row_ptr, uint64_t cap_row_ptr, uint32_t* col,
+                     uint64_t cap_col, void* coeff, uint64_t cap_coeff);
 // The five query vectors of a proving key, in the order of b2s_pk_query's `which`.
 enum PkQueryId { Q_A, Q_B_G1, Q_B_G2, Q_H, Q_L, PK_QUERIES };
 // Where the scalars of a query's MSM start: z + off, z + n_instance + off (the witness), or the h shard (HSource).

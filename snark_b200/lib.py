@@ -62,6 +62,10 @@ class PredicateDesc(ctypes.Structure):
     ]
 
 
+class Gr1csPredInfo(ctypes.Structure):
+    _fields_ = [("arity", c_uint32), ("reserved", c_uint32), ("n_rows", c_uint64), ("nnz", c_uint64 * GR1CS_MAX_ARITY)]
+
+
 class PredicateLcmapDesc(ctypes.Structure):
     _fields_ = [
         ("arity", c_uint32), ("n_terms", c_uint32),
@@ -102,10 +106,11 @@ class Gr1cs:
     """A device-resident GR1CS (b2s_gr1cs), the labels of its predicates in upload (BTreeMap) order and the number of
     variables (n_instance + n_witness) every assignment holds."""
 
-    def __init__(self, handle, labels, n_vars):
+    def __init__(self, handle, labels, n_vars, src_vars=None):
         self.h = handle
         self.labels = labels
         self.n_vars = n_vars
+        self.src_vars = src_vars   # the source's n_instance + n_witness, for a handle from r1cs_to_sr1cs
 
 
 # name -> (restype, argtypes): every symbol include/b200snark.h declares
@@ -141,6 +146,10 @@ SIGNATURES = {
     "b2s_gr1cs_free": (None, [c_void_p, c_void_p]),
     "b2s_gr1cs_check": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_void_p]),
     "b2s_r1cs_check": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p, c_void_p]),
+    "b2s_r1cs_to_sr1cs": (c_int32, [c_void_p, c_void_p, POINTER(c_void_p)]),
+    "b2s_sr1cs_assignment": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p]),
+    "b2s_gr1cs_info": (c_int32, [c_void_p, c_void_p, POINTER(c_uint64), POINTER(c_uint32), POINTER(Gr1csPredInfo), c_uint32]),
+    "b2s_gr1cs_export": (c_int32, [c_void_p, c_void_p, c_uint32, c_uint32, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_uint64]),
     "b2s_pk_upload": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, POINTER(c_void_p)]),
     "b2s_pk_upload_qap": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_pk_free": (None, [c_void_p, c_void_p]),
@@ -540,6 +549,61 @@ class Backend:
             if f != NOT_FOUND:
                 return label, int(f)
         return None
+
+    # ---- R1CS -> square R1CS (Sr1csAdapter) -----------------------------------------------------------------------------
+    def r1cs_to_sr1cs(self, m):
+        """b2s_r1cs_to_sr1cs: the square R1CS of a matrix handle of this Backend as a Gr1cs with the one predicate "SR1CS"
+        (x0^2 - x1).  The source handle may be freed afterwards."""
+        src_vars = self._r1cs_vars.get(m.value if isinstance(m, c_void_p) else m)
+        if src_vars is None:
+            raise ValueError("r1cs_to_sr1cs: not a live matrix handle of this Backend")
+        h = c_void_p()
+        self._ck(self.lib.b2s_r1cs_to_sr1cs(self.h, m, ctypes.byref(h)))
+        info = self.gr1cs_info(Gr1cs(h, ["SR1CS"], 0))
+        return Gr1cs(h, ["SR1CS"], info["n_instance"] + info["n_witness"], src_vars)
+
+    def sr1cs_assignment(self, g, z, out=None):
+        """b2s_sr1cs_assignment: z (n_assign, src_vars * 8) 32-bit limbs of the source's assignments, HOST numpy or CUDA
+        torch tensor -> the converted assignments (n_assign, g.n_vars * 8) in the same memory (written into `out` if given)."""
+        width = 8 * (g.src_vars or 0)
+        if len(z.shape) != 2 or z.shape[1] != width:
+            raise ValueError(f"z must be (n_assign, {width}) 32-bit limbs, got shape {tuple(z.shape)}")
+        if out is None:
+            if isinstance(z, np.ndarray):
+                out = np.zeros((z.shape[0], 8 * g.n_vars), dtype=np.uint32)
+            else:
+                import torch
+
+                out = torch.zeros((z.shape[0], 8 * g.n_vars), dtype=z.dtype, device=z.device)
+                torch.cuda.current_stream(z.device).synchronize()
+        (pz, po), mem = _ptrs(z, out)
+        self._ck(self.lib.b2s_sr1cs_assignment(self.h, g.h, z.shape[0], pz, mem, po))
+        return out
+
+    def gr1cs_info(self, g):
+        """b2s_gr1cs_info: {"n_instance", "n_witness", "predicates": [(arity, n_rows, [nnz per argument])]} of any Gr1cs."""
+        n_vars = (c_uint64 * 2)()
+        n_pred = c_uint32()
+        self._ck(self.lib.b2s_gr1cs_info(self.h, g.h, n_vars, ctypes.byref(n_pred), None, 0))
+        preds = (Gr1csPredInfo * max(n_pred.value, 1))()
+        self._ck(self.lib.b2s_gr1cs_info(self.h, g.h, n_vars, ctypes.byref(n_pred), preds, n_pred.value))
+        return {"n_instance": int(n_vars[0]), "n_witness": int(n_vars[1]),
+                "predicates": [(p.arity, int(p.n_rows), [int(x) for x in p.nnz[:p.arity]]) for p in preds[:n_pred.value]]}
+
+    def gr1cs_export(self, g, pred, arg, info=None):
+        """b2s_gr1cs_export: argument `arg` of predicate `pred` -> (row_ptr uint64[n_rows + 1], col uint32[nnz], coeff
+        uint32[nnz * 8] Montgomery limbs)."""
+        info = info or self.gr1cs_info(g)
+        n_rows, nnz = 0, 0
+        if pred < len(info["predicates"]):
+            _, n_rows, nnzs = info["predicates"][pred]
+            nnz = nnzs[arg] if arg < len(nnzs) else 0
+        row_ptr = np.zeros(n_rows + 1, dtype=np.uint64)
+        col = np.zeros(max(nnz, 1), dtype=np.uint32)
+        coeff = np.zeros(max(nnz, 1) * 8, dtype=np.uint32)
+        self._ck(self.lib.b2s_gr1cs_export(self.h, g.h, pred, arg, row_ptr.ctypes.data, row_ptr.nbytes, col.ctypes.data, 4 * nnz,
+                                           coeff.ctypes.data, 32 * nnz))
+        return row_ptr, col[:nnz], coeff[:8 * nnz]
 
     # ---- Groth16 ------------------------------------------------------------------------------
     def pk_upload(self, desc: PkDesc, mem=MEM_HOST, qap=QAP_LIBSNARK):
