@@ -656,8 +656,13 @@ static RoundPlan plan_rounds(Ctx* c, uint64_t T, uint32_t G, bool is_g1, uint32_
     while ((1ull << ba_auto) < per_bucket) ba_auto++;
     // a round has a fixed price -- one latency-bound inversion level plus a dozen small launches -- and
     // saves 4 (G1) / 11 (G2) base multiplications on each of its T / 2^(r+1) additions: keep the rounds that pay.  Sliced
-    // rounds pay the fixed price once per slice, so a slice of t entries keeps the rounds that pay for t.
-    const double min_adds = is_g1 ? 6.0e6 : 2.5e6;
+    // rounds pay the fixed price once per slice, so a slice of t entries keeps the rounds that pay for t.  With Fermat
+    // inversions the level alone took 0.72 ms (G1), ~0.8-0.9 ms with the small launches (halve, singles, 3 scan and 3 rank
+    // kernels, memset: ~0.08 ms), which at 2.6e10 Fq products/s is 6e6 G1 (2.5e6 G2) additions' saving.  Divsteps
+    // inversions and BA_K2 = 16 bring the G1 level to <= 0.19 ms (2.70 ms over the >= 14 levels of a 2^24 proof on an H100),
+    // so ~0.27 ms a round with the launches, ~1.7e6 additions' saving; G2 (three Fq products per Fq2 product in the chain)
+    // is priced at ~0.3 ms.  1.5e6 / 0.75e6 give a 2^24 heavy list 3 (G1) / 4 (G2) rounds run in one piece, DESIGN.md 3.1 and 4.
+    const double min_adds = is_g1 ? 1.5e6 : 0.75e6;
     auto pays = [&](uint64_t t) {
         uint32_t p = 0;
         while (p < 16 && (double)(t >> (p + 1)) > min_adds) p++;

@@ -19,7 +19,7 @@
 //   * pass 1 (msm_ba_p1_kernel): per lane, prefix products of the denominators d = x2 - x1 down its K rows
 //     (x coordinates only), prefix to HBM (coalesced), lane total to tot[].
 //   * inversion (msm_ba_inv_kernel): the lane totals are inverted with the same trick one level up, K2 totals
-//     per Fermat inversion -- one inversion per 32 K K2 / 32 additions instead of one per K.
+//     per inversion -- one inversion per 32 K K2 / 32 additions instead of one per K.
 //   * pass 2 (msm_ba_p2_kernel): backwards down the rows: 1/d from the running inverse and the stored prefix,
 //     then the addition itself; results to HBM (coalesced, bucket order).
 //   * operands never wait in registers: each lane stages its own points / x's / prefix for the next rows in a
@@ -38,7 +38,11 @@ enum : uint32_t { BA_COPY1 = 0, BA_COPY2 = 1, BA_ADD = 2, BA_DBL = 3, BA_INF = 4
 enum : uint32_t { BA_F_VALID = 1u, BA_F_SINGLE = 2u };
 
 static constexpr uint32_t BA_KMIN = 16, BA_KMAX = 256;   // rows per unit (chosen on the device from the round's size)
-static constexpr uint32_t BA_K2 = 32;                     // lane totals per Fermat inversion
+// lane totals per inversion.  The kernel is a few warps per SM, so its time is one thread's chain: K2 products, one
+// divsteps inversion (~1100 divsteps) and 2 K2 products back.  32 made the 96 dependent products the longest part once
+// the inversion stopped being a 608-product Fermat chain; 16 halves them and still keeps the ~17 k inversions of a
+// 2^24 round few enough that their instruction count does not make the kernel issue-bound.
+static constexpr uint32_t BA_K2 = 16;
 static constexpr uint32_t BA_P1_STAGES = 3, BA_P2_STAGES = 2;
 
 __host__ __device__ constexpr uint32_t ba_slot_bytes(uint32_t n) { return ((((n + 15u) / 16u) | 1u)) * 16u; }

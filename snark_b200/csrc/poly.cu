@@ -6,8 +6,8 @@
 // work over vectors of |H| ... 4|K| field elements: products and sums of evaluation vectors, batched inversion
 // (ark-ff `batch_inversion`), geometric sequences (domain elements, coset points), Horner evaluation.  These kernels are that
 // layer; the transforms and commitments go through b2s_ntt / b2s_msm_g1 / b2s_fixed_base_g1, the matrix products through
-// b2s_spmv.  All HBM-bound streaming kernels (32 B per element per operand) except the batched inversion (~27 multiplications
-// per element: one Fermat inversion per 16 elements) and the geometric sequence (~7 per element).
+// b2s_spmv.  All HBM-bound streaming kernels (32 B per element per operand) except the batched inversion (3 multiplications
+// per element and one divsteps inversion per 16 elements) and the geometric sequence (~7 per element).
 #define B2S_INLINE_MUL 1   // Fr only in this unit
 #include "common.cuh"
 

@@ -73,6 +73,16 @@ def field_struct(name, p, n, extra=""):
     s += fn("mod", p)
     s += fn("r1", R % p)
     s += fn("r2", R * R % p)
+    # inversion by divsteps (ff.cuh, Fp::inverse): p in signed 30-bit limbs, with room for the (-2p, p) range of the
+    # Bezout coefficients; p^-1 mod 2^30; R^3 mod p, which one Montgomery product turns the plain inverse of a
+    # Montgomery-form input into the Montgomery form of the inverse
+    il = (p.bit_length() + 2 + 29) // 30
+    s += "    static constexpr int INV_LIMBS = %d;\n" % il
+    s += "    static constexpr uint32_t INV_PINV30 = 0x%08xu;\n" % pow(p, -1, 1 << 30)
+    s += "    B2S_HD static constexpr int32_t inv_mod30(int i) { constexpr int32_t t[%d] = {%s}; return t[i]; }\n" % (
+        il, ", ".join("0x%08x" % ((p >> (30 * i)) & ((1 << 30) - 1)) for i in range(il)))
+    assert p >> (30 * il) == 0
+    s += fn("inv_final", R ** 3 % p)
     s += extra
     s += "};\n\n"
     return s

@@ -1,8 +1,10 @@
 // Micro-benchmarks that set the ALU roofline for the field arithmetic: how many Montgomery
-// multiplications / mixed additions per second the chip sustains when nothing else is in the way.
+// multiplications / mixed additions per second the chip sustains when nothing else is in the way, and the latency
+// and throughput of the field inversion against the Fermat chain it replaced (`microbench inv` runs only that case).
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -DB2S_INLINE_MUL -I snark_b200/csrc -o build/microbench tools/microbench.cu
 #define B2S_INLINE_MUL 1
 #include <cstdio>
+#include <string>
 #include <cuda_runtime.h>
 #include "curves.cuh"
 using namespace b2s;
@@ -33,6 +35,34 @@ __global__ void madd_chain(XYZZ<F>* out, const Affine<F>* in, int iters) {
         q.x = q.x + acc.zz;  // keep the operand changing (not a curve point; the formulas do not care)
     }
     out[i] = acc;
+}
+
+// inversion: each thread runs `iters` dependent steps of one kind -- 0: inverse() (divsteps), 1: the Fermat chain
+// pow_words(p - 2), 2: one Montgomery product
+struct Words { uint32_t w[12]; };
+
+template <class F, int OP>
+__global__ void inv_chain(F* out, const F* in, int iters, Words pm2) {
+    int i = blockIdx.x * blockDim.x + threadIdx.x;
+    F x = in[i], y = in[i + 1];
+    for (int it = 0; it < iters; it++) {
+        if (OP == 0) x = x.inverse();
+        if (OP == 1) x = x.pow_words(pm2.w, F::N);
+        if (OP == 2) x = x * y;
+    }
+    out[i] = x;
+}
+
+template <class P>
+Words p_minus_2(const Fp<P>*) {
+    Words e{};
+    uint64_t borrow = 2;
+    for (int i = 0; i < P::N; i++) {
+        const uint64_t d = (uint64_t)P::mod(i) - borrow;
+        e.w[i] = (uint32_t)d;
+        borrow = (d >> 63) & 1;
+    }
+    return e;
 }
 
 template <class K, class... A>
@@ -75,8 +105,38 @@ void bench_madd(const char* name, int threads, int blocks_per_sm) {
     cudaFree(in); cudaFree(out);
 }
 
-int main() {
+// latency: one warp, each lane a chain of dependent operations; throughput: 4 CTAs of 128 threads per SM
+template <class F, int OP>
+double bench_inv_one(bool latency, int iters) {
+    int sms; cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    const int blocks = latency ? 1 : sms * 4, threads = latency ? 32 : 128;
+    size_t n = (size_t)blocks * threads + 2;
+    F *in, *out; cudaMalloc(&in, n * sizeof(F)); cudaMalloc(&out, n * sizeof(F));
+    cudaMemset(in, 0x11, n * sizeof(F));   // 0x11.. words: below p for every field here
+    float ms = time_kernel(inv_chain<F, OP>, dim3(blocks), dim3(threads), out, in, iters, p_minus_2((const F*)nullptr));
+    cudaFree(in); cudaFree(out);
+    const double ops = (double)blocks * threads * iters;
+    return latency ? ms * 1e3 / iters : ops / ms * 1e3;   // us per operation, or operations per second
+}
+
+template <class F>
+void bench_inv(const char* name) {
+    const double li = bench_inv_one<F, 0>(true, 200), lp = bench_inv_one<F, 1>(true, 10), lm = bench_inv_one<F, 2>(true, 20000);
+    printf("%-10s latency  : inverse %.2f us  pow(p-2) %.2f us  mul %.4f us  (pow / inverse = %.1fx, inverse = %.0f muls)\n",
+           name, li, lp, lm, lp / li, li / lm);
+    const double ti = bench_inv_one<F, 0>(false, 8), tp = bench_inv_one<F, 1>(false, 1), tm = bench_inv_one<F, 2>(false, 4000);
+    printf("%-10s throughput: inverse %.3e/s  pow(p-2) %.3e/s  mul %.3e/s  (inverse / pow = %.1fx)\n", name, ti, tp, tm, ti / tp);
+}
+
+int main(int argc, char** argv) {
     using BF = Bls12_381::Fq; using BR = Bls12_381::Fr; using NF = Bn254::Fq;
+    bench_inv<BF>("bls_fq");
+    bench_inv<BR>("bls_fr");
+    if (argc > 1 && std::string(argv[1]) == "inv") {
+        cudaError_t e = cudaDeviceSynchronize();
+        printf("status: %s\n", cudaGetErrorString(e));
+        return e != cudaSuccess;
+    }
     for (int bps : {1, 2, 4}) {
         bench_mul<BF, 1>("bls_fq", 128, bps);
         bench_mul<BF, 2>("bls_fq", 128, bps);
