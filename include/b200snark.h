@@ -281,6 +281,54 @@ int32_t b2s_gr1cs_info(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_vars[2], uin
 int32_t b2s_gr1cs_export(b2s_ctx* ctx, const b2s_gr1cs* g, uint32_t pred, uint32_t arg, uint64_t* row_ptr, uint64_t cap_row_ptr,
                          uint32_t* col, uint64_t cap_col, void* coeff, uint64_t cap_coeff);
 
+/* ---- instance outlining (ConstraintSystem::finalize with an InstanceOutliner, constraint_system.rs:689-707, 826-863;
+ *      instance_outliner.rs:40-80) -----------------------------------------------------------------------------------------
+ * The LcMap uploads above, with the instance variables outlined on the device as finalize() does when an outliner is set.
+ * The caller runs inline_all_lcs() (not finalize() with an outliner) and passes the LcMap and arguments as they stand then;
+ * n_instance and n_witness are the counts before outlining (W = n_witness).  The result is the handle of the outlined system:
+ *   - n_instance more witnesses: witness W copies One, witness W + i copies Instance(i), i >= 1; the copy of variable i is at
+ *     column n_instance + W + i.
+ *   - every term of every stored LC that is One or Instance(i) reads as the copy of 0 or i (Instance(0) as One).  A bare
+ *     argument (a single (ONE, v), which the system never stores as an LC) keeps its column, so instances may still occur
+ *     outside the tie rows, as they do upstream.
+ *   - n_instance tie rows appended to predicate `pred` (upload index; the predicate the outliner's label names), not rewritten:
+ *       B2S_OUTLINE_R1CS  (outline_r1cs, arity 3)   row 0: w_W * w_W = One;  row i: w_W * w_{W+i} = Instance(i); bare arguments
+ *       B2S_OUTLINE_SR1CS (outline_sr1cs, arity 2)  row i: argument 0 the LC [(ONE, Instance(i)), (-ONE, w_{W+i})] (appended to
+ *                                                   the LcMap; Instance(0) is column 0), argument 1 SymbolicLc(0), the empty LC
+ * Rows and the order of terms within them are exactly those of to_matrices() on the host-outlined system.  Variables of the
+ * LcMap are checked against the outlined system's n_instance + W + n_instance.  Rejected before anything is allocated, with
+ * B2S_ERR_INVALID_ARG and b2s_last_error naming the cause: a null descriptor, an unknown strategy, pred out of range, a target
+ * arity other than the strategy's, and for B2S_OUTLINE_SR1CS a pool whose pool[1] is not -ONE (field_interner.rs:32-33);
+ * B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE for the 2^32 limits on slots, nonzeros and variables counted with the tie rows and the
+ * copies; otherwise as the upload without outlining.
+ *   b2s_gr1cs_upload_lcmap_outline  b2s_gr1cs_upload_lcmap, outlined.
+ *   b2s_r1cs_upload_lcmap_outline   b2s_r1cs_upload_lcmap, outlined: B2S_OUTLINE_R1CS with pred 0 only.  The result is an
+ *                                   ordinary b2s_r1cs of n_rows + n_instance rows and n_witness + n_instance witnesses (domain
+ *                                   next_pow2(n_rows + 2 n_instance), B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE above the curve's
+ *                                   limit): setup, proving, checks and b2s_r1cs_to_sr1cs take it as any other.
+ *   b2s_gr1cs_outline_assignment /
+ *   b2s_r1cs_outline_assignment     the assignment of the outlined system, as outlining appends to witness_assignment in prove
+ *                                   mode: z holds n_assign rows of n_instance + W Montgomery Fr (z[0] = ONE), out_z receives
+ *                                   n_assign rows of n_instance + W + n_instance: z || (ONE, z[1], ..., z[n_instance - 1]).  z and
+ *                                   out_z share `mem`; host batches go through bounded device scratch in chunks.  n_assign == 0
+ *                                   -> B2S_OK.  B2S_ERR_INVALID_ARG for a handle no outlining upload made. */
+#define B2S_OUTLINE_R1CS 1
+#define B2S_OUTLINE_SR1CS 2
+typedef struct b2s_outline {
+    int32_t strategy;                      /* B2S_OUTLINE_R1CS or B2S_OUTLINE_SR1CS */
+    uint32_t pred;                         /* upload index of the predicate that receives the tie rows */
+} b2s_outline;
+int32_t b2s_gr1cs_upload_lcmap_outline(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates,
+                                       const b2s_predicate_lcmap_desc* preds, uint64_t n_lcs, const uint64_t* lc_offsets,
+                                       const uint64_t* lc_vars, const uint32_t* lc_coeffs, const void* pool, uint32_t pool_len,
+                                       const b2s_outline* outline, b2s_gr1cs** out);
+int32_t b2s_r1cs_upload_lcmap_outline(b2s_ctx* ctx, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness,
+                                      const uint64_t* const args[3], uint64_t n_lcs, const uint64_t* lc_offsets,
+                                      const uint64_t* lc_vars, const uint32_t* lc_coeffs, const void* pool, uint32_t pool_len,
+                                      const b2s_outline* outline, b2s_r1cs** out);
+int32_t b2s_gr1cs_outline_assignment(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, void* out_z);
+int32_t b2s_r1cs_outline_assignment(b2s_ctx* ctx, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, void* out_z);
+
 /* ---- Groth16 (ark-groth16 ProvingKey / create_proof_with_reduction, SURVEY App. A.1) ------------
  * Query vectors are affine point arrays in HOST or DEVICE memory (`mem`); they are copied to the GPU.
  *   a_query, b_g1_query, b_g2_query: n_vars = n_instance + n_witness points

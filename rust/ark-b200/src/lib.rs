@@ -39,6 +39,22 @@ pub struct B2sPredicateLcmapDesc {
     pub args: [*const u64; B2S_GR1CS_MAX_ARITY],
 }
 
+/// `b2s_outline`: the outlining strategy and the upload index (label order) of the predicate that receives the tie rows
+#[repr(C)]
+pub struct B2sOutline {
+    pub strategy: i32,
+    pub pred: u32,
+}
+
+/// Which `InstanceOutliner` function the upload stands in for.  An `InstanceOutliner` holds its strategy as an opaque
+/// `Rc<dyn Fn>`, so the caller names it here instead of setting it on the cs: `Outliner::R1cs` is `outline_r1cs` and
+/// `Outliner::Sr1cs` is `outline_sr1cs` (instance_outliner.rs:40-80); `pred_label` is the outliner's label.
+#[derive(Clone, Copy, Debug, PartialEq, Eq)]
+pub enum Outliner {
+    R1cs = 1,
+    Sr1cs = 2,
+}
+
 #[repr(C)]
 #[derive(Default)]
 pub struct B2sZkeyInfo { pub n_vars: u64, pub n_public: u64, pub domain_size: u64, pub n_coeffs: u64 }
@@ -150,6 +166,14 @@ extern "C" {
     pub fn b2s_gr1cs_upload_lcmap(ctx: *mut B2sCtx, n_instance: u64, n_witness: u64, n_predicates: u32,
                                   preds: *const B2sPredicateLcmapDesc, n_lcs: u64, lc_offsets: *const u64, lc_vars: *const u64,
                                   lc_coeffs: *const u32, pool: *const c_void, pool_len: u32, out: *mut *mut B2sGr1cs) -> i32;
+    /// b2s_gr1cs_upload_lcmap with instance outlining (ConstraintSystem::finalize with an InstanceOutliner)
+    pub fn b2s_gr1cs_upload_lcmap_outline(ctx: *mut B2sCtx, n_instance: u64, n_witness: u64, n_predicates: u32,
+                                          preds: *const B2sPredicateLcmapDesc, n_lcs: u64, lc_offsets: *const u64, lc_vars: *const u64,
+                                          lc_coeffs: *const u32, pool: *const c_void, pool_len: u32, outline: *const B2sOutline,
+                                          out: *mut *mut B2sGr1cs) -> i32;
+    /// z || (ONE, z[1], ..., z[n_instance - 1]): what outlining appends to witness_assignment in prove mode
+    pub fn b2s_gr1cs_outline_assignment(ctx: *mut B2sCtx, g: *const B2sGr1cs, n_assign: u64, z: *const c_void, mem: i32,
+                                        out_z: *mut c_void) -> i32;
     pub fn b2s_gr1cs_free(ctx: *mut B2sCtx, g: *mut B2sGr1cs);
     pub fn b2s_gr1cs_check(ctx: *mut B2sCtx, g: *const B2sGr1cs, n_assign: u64, z: *const c_void, mem: i32, first_unsat: *mut u64,
                            n_unsat: *mut u64) -> i32;
@@ -581,6 +605,8 @@ pub struct Gr1csB200<F: PrimeField> {
     pub labels: Vec<Label>,
     /// n_instance + n_witness: the length of every assignment
     pub n_vars: usize,
+    /// of an outlined upload: n_instance + n_witness before outlining, the length `outline_assignment` takes (0 otherwise)
+    pub src_vars: usize,
     _f: core::marker::PhantomData<F>,
 }
 
@@ -636,6 +662,33 @@ impl<F: PrimeField> Gr1csB200<F> {
     /// caller until it has a one-line accessor: `pool` is its `vec` (pool[0] = ONE, pool[1] = -ONE) and `coeff_ids` the
     /// index each `InternedField` of the LcMap names in it, flat in the order of `cs.lc_map.iter()`.
     pub fn upload_lcmap(curve_id: i32, cs: &ConstraintSystem<F>, pool: &[F], coeff_ids: &[u32]) -> Result<Self, B200Error> {
+        Self::lcmap_upload(curve_id, cs, pool, coeff_ids, None)
+    }
+
+    /// `upload_lcmap` of the system `cs.finalize()` would give with an `InstanceOutliner { pred_label, func }` set, the
+    /// outlining done on the GPU.  Recipe: run `cs.inline_all_lcs()` (public) instead of `finalize()`, set no outliner on
+    /// the cs, and pass the outliner's strategy and label here.  The handle has `cs.num_instance_variables()` more witnesses
+    /// (the copies of One and of every instance) and as many tie rows in `pred_label`'s predicate; prove-mode assignments
+    /// of the outlined system come from `outline_assignment`.  A label the cs has no predicate for is
+    /// `B200Error::Backend(B2S_ERR_INVALID_ARG)` (upstream `finalize()` skips outlining then).
+    pub fn upload_lcmap_outlined(curve_id: i32, cs: &ConstraintSystem<F>, pool: &[F], coeff_ids: &[u32], outliner: Outliner,
+                                 pred_label: &str) -> Result<Self, B200Error> {
+        Self::lcmap_upload(curve_id, cs, pool, coeff_ids, Some((outliner, pred_label)))
+    }
+
+    /// z = instance || witness of the system before outlining -> the outlined system's z (z || copies), on the GPU
+    pub fn outline_assignment(&self, z: &[F]) -> Result<Vec<F>, B200Error> {
+        if self.src_vars == 0 { return Err(B200Error::Backend(ERR_INVALID_ARG)); }
+        if z.len() != self.src_vars { return Err(B200Error::Synthesis(SynthesisError::AssignmentMissing)); }
+        let mut out = vec![F::zero(); self.n_vars];
+        check(self.ctx, unsafe {
+            b2s_gr1cs_outline_assignment(self.ctx, self.g, 1, z.as_ptr().cast(), 0 /* B2S_MEM_HOST */, out.as_mut_ptr().cast())
+        })?;
+        Ok(out)
+    }
+
+    fn lcmap_upload(curve_id: i32, cs: &ConstraintSystem<F>, pool: &[F], coeff_ids: &[u32], outline: Option<(Outliner, &str)>)
+        -> Result<Self, B200Error> {
         Self::check_curve(curve_id)?;
         let raw = |v: &Variable| -> u64 {
             ((v.kind() as u64) << 61) | v.index().unwrap_or(0) as u64
@@ -669,11 +722,28 @@ impl<F: PrimeField> Gr1csB200<F> {
                 for (j, col) in a.iter().take(B2S_GR1CS_MAX_ARITY).enumerate() { d.args[j] = col.as_ptr(); }
                 d
             }).collect();
-        Self::create(curve_id, cs, labels, |ctx, g| unsafe {
-            b2s_gr1cs_upload_lcmap(ctx, cs.num_instance_variables() as u64, cs.num_witness_variables() as u64, descs.len() as u32,
-                                   descs.as_ptr(), (offsets.len() - 1) as u64, offsets.as_ptr(), vars.as_ptr(), coeff_ids.as_ptr(),
-                                   pool.as_ptr().cast(), pool.len() as u32, g)
-        })
+        let ol = match outline {
+            None => None,
+            Some((o, label)) => {
+                let pred = labels.iter().position(|l| l.as_str() == label).ok_or(B200Error::Backend(ERR_INVALID_ARG))?;
+                Some(B2sOutline { strategy: o as i32, pred: pred as u32 })
+            }
+        };
+        let mut h = Self::create(curve_id, cs, labels, |ctx, g| unsafe {
+            let (n_inst, n_wit, n_pred) = (cs.num_instance_variables() as u64, cs.num_witness_variables() as u64, descs.len() as u32);
+            let (n_lcs, pool_len) = ((offsets.len() - 1) as u64, pool.len() as u32);
+            match &ol {
+                None => b2s_gr1cs_upload_lcmap(ctx, n_inst, n_wit, n_pred, descs.as_ptr(), n_lcs, offsets.as_ptr(), vars.as_ptr(),
+                                               coeff_ids.as_ptr(), pool.as_ptr().cast(), pool_len, g),
+                Some(o) => b2s_gr1cs_upload_lcmap_outline(ctx, n_inst, n_wit, n_pred, descs.as_ptr(), n_lcs, offsets.as_ptr(),
+                                                          vars.as_ptr(), coeff_ids.as_ptr(), pool.as_ptr().cast(), pool_len, o, g),
+            }
+        })?;
+        if ol.is_some() {
+            h.src_vars = h.n_vars;
+            h.n_vars += cs.num_instance_variables();
+        }
+        Ok(h)
     }
 
     fn check_curve(curve_id: i32) -> Result<(), B200Error> {
@@ -692,7 +762,7 @@ impl<F: PrimeField> Gr1csB200<F> {
         let st = upload(ctx, &mut g);
         if st != 0 { unsafe { b2s_ctx_destroy(ctx) }; }
         check(ctx, st)?;
-        Ok(Gr1csB200 { ctx, g, labels, n_vars, _f: core::marker::PhantomData })
+        Ok(Gr1csB200 { ctx, g, labels, n_vars, src_vars: 0, _f: core::marker::PhantomData })
     }
 
     /// The reference's answer without a `ConstraintLayer`: `Some("{label} - {index}")` for the first unsatisfied constraint
@@ -789,7 +859,7 @@ impl<F: PrimeField> Sr1csB200<F> {
             return Err(e);
         }
         let gr1cs = Gr1csB200 { ctx, g, labels: vec![SR1CS_PREDICATE_LABEL.to_string()], n_vars: (nv[0] + nv[1]) as usize,
-                                _f: core::marker::PhantomData };
+                                src_vars: 0, _f: core::marker::PhantomData };
         Ok(Sr1csB200 { gr1cs, src_vars })
     }
 

@@ -330,7 +330,30 @@ int32_t b2s_r1cs_upload_lcmap(b2s_ctx* ctx, uint64_t n_rows, uint64_t n_instance
         if (!args[k] && n_rows) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_upload_lcmap: null argument array %d", k);
     if (n_lcs && lc_offsets[n_lcs] != 0 && (!lc_vars || !lc_coeffs)) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_upload_lcmap: null LC arrays");
     *out = nullptr;
-    return r1cs_upload_lcmap(ctx, n_rows, n_instance, n_witness, args, n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len, out);
+    return r1cs_upload_lcmap(ctx, n_rows, n_instance, n_witness, args, n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len, nullptr, out);
+}
+
+int32_t b2s_r1cs_upload_lcmap_outline(b2s_ctx* ctx, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness,
+                                      const uint64_t* const args[3], uint64_t n_lcs, const uint64_t* lc_offsets,
+                                      const uint64_t* lc_vars, const uint32_t* lc_coeffs, const void* pool, uint32_t pool_len,
+                                      const b2s_outline* outline, b2s_r1cs** out) {
+    LOCK(ctx);
+    if (!out || !args || !lc_offsets || !pool || !outline) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_upload_lcmap_outline: null argument");
+    for (int k = 0; k < 3; k++)
+        if (!args[k] && n_rows) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_upload_lcmap_outline: null argument array %d", k);
+    if (n_lcs && lc_offsets[n_lcs] != 0 && (!lc_vars || !lc_coeffs))
+        return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_upload_lcmap_outline: null LC arrays");
+    *out = nullptr;
+    return r1cs_upload_lcmap(ctx, n_rows, n_instance, n_witness, args, n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len, outline, out);
+}
+
+int32_t b2s_r1cs_outline_assignment(b2s_ctx* ctx, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, void* out_z) {
+    LOCK(ctx);
+    if (!m || (n_assign && (!z || !out_z))) return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_outline_assignment: null argument");
+    if (!m->outline_copies)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "r1cs_outline_assignment: the handle was not made by b2s_r1cs_upload_lcmap_outline");
+    const uint64_t n_src = m->n_instance + m->n_witness - m->outline_copies;
+    return outline_assignment(ctx, n_src, m->outline_copies, n_assign, z, mem, out_z);
 }
 
 void b2s_r1cs_free(b2s_ctx* ctx, b2s_r1cs* m) {
@@ -413,7 +436,33 @@ int32_t b2s_gr1cs_upload_lcmap(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_wit
     if (n_lcs && lc_offsets[n_lcs] != 0 && (!lc_vars || !lc_coeffs)) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_upload_lcmap: null LC arrays");
     *out = nullptr;
     return gr1cs_upload_lcmap(ctx, n_instance, n_witness, n_predicates, preds, LcMapHost{n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len},
-                              out);
+                              nullptr, out);
+}
+
+int32_t b2s_gr1cs_upload_lcmap_outline(b2s_ctx* ctx, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates,
+                                       const b2s_predicate_lcmap_desc* preds, uint64_t n_lcs, const uint64_t* lc_offsets,
+                                       const uint64_t* lc_vars, const uint32_t* lc_coeffs, const void* pool, uint32_t pool_len,
+                                       const b2s_outline* outline, b2s_gr1cs** out) {
+    LOCK(ctx);
+    if (!out || (!preds && n_predicates) || !lc_offsets || !pool || !outline)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_upload_lcmap_outline: null argument");
+    if (n_lcs && lc_offsets[n_lcs] != 0 && (!lc_vars || !lc_coeffs))
+        return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_upload_lcmap_outline: null LC arrays");
+    *out = nullptr;
+    return gr1cs_upload_lcmap(ctx, n_instance, n_witness, n_predicates, preds, LcMapHost{n_lcs, lc_offsets, lc_vars, lc_coeffs, pool, pool_len},
+                              outline, out);
+}
+
+int32_t b2s_gr1cs_outline_assignment(b2s_ctx* ctx, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, void* out_z) {
+    LOCK(ctx);
+    if (!g || (n_assign && (!z || !out_z))) return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_outline_assignment: null argument");
+    if (g->curve != ctx->curve)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_outline_assignment: the handle was made on a ctx of curve %d, this ctx is curve %d",
+                    g->curve, ctx->curve);
+    if (!g->outline_copies)
+        return fail(ctx, B2S_ERR_INVALID_ARG, "gr1cs_outline_assignment: the handle was not made by b2s_gr1cs_upload_lcmap_outline");
+    const uint64_t n_src = g->n_instance + g->n_witness - g->outline_copies;
+    return outline_assignment(ctx, n_src, g->outline_copies, n_assign, z, mem, out_z);
 }
 
 void b2s_gr1cs_free(b2s_ctx* ctx, b2s_gr1cs* g) {

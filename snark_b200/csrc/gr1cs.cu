@@ -295,29 +295,45 @@ int32_t gr1cs_upload(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n
 }
 
 int32_t gr1cs_upload_lcmap(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_lcmap_desc* preds,
-                           const LcMapHost& lm, b2s_gr1cs** out) {
+                           const LcMapHost& lm, const b2s_outline* ol, b2s_gr1cs** out) {
     B2S_TRY(check_vars(c, n_instance, n_witness));
+    // outlining: n_instance copies (witnesses n_witness ..) and n_instance tie rows in predicate ol->pred
+    const uint64_t n_tie = ol ? n_instance : 0;
+    if (ol) {
+        const uint32_t target_arity = ol->pred < n_predicates ? preds[ol->pred].arity : 0;
+        B2S_TRY(outline_validate(c, "gr1cs_upload_lcmap_outline", *ol, n_predicates, target_arity, lm));
+        B2S_TRY(check_vars(c, n_instance, n_witness + n_tie));
+    }
     uint64_t n_slots = 0;   // (argument, row) slots of all predicates, saturated at 2^32 (lcmap_validate rejects that)
     for (uint32_t p = 0; p < n_predicates; p++) {
         const b2s_predicate_lcmap_desc& d = preds[p];
         B2S_TRY(check_poly(c, p, d));
         for (uint32_t j = 0; j < d.arity; j++)
             if (!d.args[j] && d.n_rows) return fail(c, B2S_ERR_INVALID_ARG, "gr1cs: predicate %u: null argument array %u", p, j);
-        n_slots = std::min<uint64_t>(n_slots + d.arity * d.n_rows, 1ull << 32);
+        const uint64_t rows = d.n_rows + (ol && p == ol->pred ? n_tie : 0);
+        if (rows >= (1ull << 32))
+            return fail(c, B2S_ERR_POLYNOMIAL_DEGREE_TOO_LARGE, "gr1cs: predicate %u: %llu constraints with the tie rows; the limit is 2^32 - 1", p,
+                        (unsigned long long)rows);
+        n_slots = std::min<uint64_t>(n_slots + d.arity * rows, 1ull << 32);
     }
     B2S_TRY(lcmap_validate(c, lm, n_slots));
     std::unique_ptr<b2s_gr1cs> g(new b2s_gr1cs());
     g->curve = c->curve;
     g->n_instance = n_instance;
-    g->n_witness = n_witness;
+    g->n_witness = n_witness + n_tie;
+    g->outline_copies = n_tie;
     std::vector<LcMatrix> mats;
     std::vector<std::pair<uint32_t, uint32_t>> arg_of;   // (predicate, argument) of each matrix, for messages
+    LcOutline lo{ol ? ol->strategy : 0, n_witness, 0};
     for (uint32_t p = 0; p < n_predicates; p++) {
         const b2s_predicate_lcmap_desc& d = preds[p];
         std::unique_ptr<Gr1csPredicate> pr;
         B2S_TRY(upload_poly(c, d, pr));
+        const uint64_t tie = ol && p == ol->pred ? n_tie : 0;
+        if (tie) lo.first_mat = mats.size();
+        pr->n_rows = d.n_rows + tie;
         for (uint32_t j = 0; j < d.arity; j++) {
-            mats.push_back({d.args[j], d.n_rows, &pr->row_ptr[j], &pr->col[j], &pr->coeff_id[j], &pr->nnz[j]});
+            mats.push_back({d.args[j], d.n_rows, &pr->row_ptr[j], &pr->col[j], &pr->coeff_id[j], &pr->nnz[j], tie});
             arg_of.emplace_back(p, j);
         }
         g->preds.push_back(std::move(pr));
@@ -328,7 +344,8 @@ int32_t gr1cs_upload_lcmap(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint
                  (unsigned long long)row);
         return std::string(buf);
     };
-    B2S_TRY(lcmap_build(c, lm, n_instance, n_instance + n_witness, mats, "the arguments of all predicates", where, g->pool, &g->pool_size));
+    B2S_TRY(lcmap_build(c, lm, n_instance, n_instance + n_witness + n_tie, mats, "the arguments of all predicates", where, g->pool,
+                        &g->pool_size, ol ? &lo : nullptr));
     *out = g.release();
     return B2S_OK;
 }

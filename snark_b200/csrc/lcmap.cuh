@@ -16,6 +16,11 @@
 // done by a counting kernel, an exclusive scan (row_ptr) and a fill kernel.  The per-row logic lives in the
 // host/device functions below so that tests can run exactly the kernels' code on the CPU
 // (tests/native/host_ff.cpp: ht_lcmap_*, tests/test_host_lcmap.py).
+//
+// Instance outlining (ConstraintSystem::perform_instance_outlining, constraint_system.rs:826-863) is folded into the same
+// walk: with remap_lcs > 0, every term of an LC j < remap_lcs that is One or Instance(i) reads as the witness copy of
+// variable 0 or i, at column copy0 (+ i).  Bare arguments and the LCs at or past remap_lcs (the tie LCs the outlining
+// strategy appends after the rewrite) keep their columns, as upstream.
 #pragma once
 #include <cstdint>
 
@@ -49,6 +54,8 @@ struct View {
     uint64_t n_lcs;
     uint32_t pool_len;
     uint64_t n_instance, n_vars;
+    uint64_t remap_lcs = 0;       // outlining: LCs below this index are rewritten (0: none is)
+    uint64_t copy0 = 0;           // outlining: the column of the copy of variable 0 (One / Instance(0))
 };
 
 B2S_LC_HD uint32_t tag_of(uint64_t var) { return (uint32_t)(var >> TAG_SHIFT); }
@@ -59,7 +66,7 @@ B2S_LC_HD uint64_t payload_of(uint64_t var) { return var & PAYLOAD_MASK; }
 template <class Fn>
 B2S_LC_HD uint32_t for_each_kept_term(const View& v, uint64_t arg, Fn&& f) {
     uint32_t err = 0;
-    auto plain = [&](uint64_t var, uint32_t coeff_id) {
+    auto plain = [&](uint64_t var, uint32_t coeff_id, bool remap) {
         const uint32_t tag = tag_of(var);
         if (tag == TAG_ZERO) return;
         if (tag == TAG_LC) { err |= ERR_NESTED_LC; return; }
@@ -68,15 +75,16 @@ B2S_LC_HD uint32_t for_each_kept_term(const View& v, uint64_t arg, Fn&& f) {
         if (v.pool_is_zero[coeff_id]) return;
         const uint64_t col = tag == TAG_ONE ? 0 : tag == TAG_INSTANCE ? payload_of(var) : payload_of(var) + v.n_instance;
         if (col >= v.n_vars || (tag == TAG_INSTANCE && col >= v.n_instance)) { err |= ERR_COLUMN; return; }
-        f((uint32_t)col, coeff_id);
+        f((uint32_t)(remap && tag != TAG_WITNESS ? v.copy0 + col : col), coeff_id);
     };
     const uint32_t tag = tag_of(arg);
     if (tag == TAG_ZERO) return 0;
     if (tag > TAG_LC) return ERR_BAD_TAG;
-    if (tag != TAG_LC) { plain(arg, 0u); return err; }       // LinearCombination::from(var): coefficient ONE = id 0
+    if (tag != TAG_LC) { plain(arg, 0u, false); return err; }   // LinearCombination::from(var): coefficient ONE = id 0
     const uint64_t j = payload_of(arg);
     if (j >= v.n_lcs) return ERR_LC_INDEX;
-    for (uint64_t e = v.lc_offsets[j]; e < v.lc_offsets[j + 1]; e++) plain(v.lc_vars[e], v.lc_coeffs[e]);
+    const bool remap = j < v.remap_lcs;
+    for (uint64_t e = v.lc_offsets[j]; e < v.lc_offsets[j + 1]; e++) plain(v.lc_vars[e], v.lc_coeffs[e], remap);
     return err;
 }
 

@@ -20,6 +20,8 @@ struct b2s_r1cs {
     b2s::DevBuf coeff_id[3];          // uint32[nnz]
     b2s::DevBuf pool;                 // Fr[pool_size]
     uint32_t pool_size = 0;
+    // set by b2s_r1cs_upload_lcmap_outline only: the instance variables copied into witnesses (b2s_r1cs_outline_assignment)
+    uint64_t outline_copies = 0;
 };
 
 namespace b2s {
@@ -49,6 +51,8 @@ struct b2s_gr1cs {
     // n_instance + n_witness and rows; what b2s_sr1cs_assignment needs besides the predicate itself
     b2s::DevBuf sr1cs_orig;               // uint32[n_instance + n_witness]
     uint64_t sr1cs_src_vars = 0, sr1cs_rows = 0;
+    // set by b2s_gr1cs_upload_lcmap_outline only: the instance variables copied into witnesses (b2s_gr1cs_outline_assignment)
+    uint64_t outline_copies = 0;
 };
 
 namespace b2s {
@@ -99,8 +103,9 @@ int32_t gr1cs_upload(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n
                      b2s_gr1cs** out);
 // the same handle from the constraint system's LcMap: the argument matrices by lcmap_build, the pool kept as the caller's
 struct LcMapHost;
+// ol: instance outlining as finalize() does it with an InstanceOutliner (lcmap.cuh), or null for none
 int32_t gr1cs_upload_lcmap(Ctx* c, uint64_t n_instance, uint64_t n_witness, uint32_t n_predicates, const b2s_predicate_lcmap_desc* preds,
-                           const LcMapHost& lm, b2s_gr1cs** out);
+                           const LcMapHost& lm, const b2s_outline* ol, b2s_gr1cs** out);
 // first_unsat / n_unsat (n_unsat may be null): n_assign x n_predicates, in `mem` like z
 int32_t gr1cs_check(Ctx* c, const b2s_gr1cs* g, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
 int32_t r1cs_check(Ctx* c, const b2s_r1cs* m, uint64_t n_assign, const void* z, int32_t mem, uint64_t* first_unsat, uint64_t* n_unsat);
@@ -172,25 +177,41 @@ struct LcMapHost {               // host pointers, as the caller holds them
     const void* pool;            // pool_len Montgomery Fr, pool[0] = ONE
     uint32_t pool_len;
 };
-// one argument matrix: n_rows raw Variables in (host), a CSR whose coefficient ids index the caller's pool out
+// one argument matrix: n_rows raw Variables in (host), a CSR whose coefficient ids index the caller's pool out.  n_tie
+// more rows follow the caller's: the tie rows of instance outlining, whose arguments lcmap_build makes on the device.
 struct LcMatrix {
     const uint64_t* args;
     uint64_t n_rows;
-    DevBuf* row_ptr;             // uint64[n_rows + 1]
+    DevBuf* row_ptr;             // uint64[n_rows + n_tie + 1]
     DevBuf* col;                 // uint32[nnz]
     DevBuf* coeff_id;            // uint32[nnz]
     uint64_t* nnz;
+    uint64_t n_tie = 0;
+};
+// Instance outlining in lcmap_build: W = the witnesses before outlining, n_instance copies follow them; the tie rows go
+// to the matrices mats[first_mat + j], j < arity of the strategy (3 for B2S_OUTLINE_R1CS, 2 for B2S_OUTLINE_SR1CS)
+struct LcOutline {
+    int32_t strategy;
+    uint64_t n_witness;
+    size_t first_mat;
 };
 // The checks of the LcMap itself, made before anything is allocated; n_slots: the rows of all matrices together.
 int32_t lcmap_validate(Ctx* c, const LcMapHost& lm, uint64_t n_slots);
+// The checks of an outlining descriptor against the target predicate's arity and the pool (B2S_OUTLINE_SR1CS reads
+// pool[1] as -ONE), made before anything is allocated; `who` prefixes the messages.
+int32_t outline_validate(Ctx* c, const char* who, const b2s_outline& ol, uint32_t n_predicates, uint32_t target_arity, const LcMapHost& lm);
 // Builds every matrix of `mats` with one count, scan and fill over all their rows and copies the pool as it is to `pool`.
 // where(m, row), when set, prefixes the message of a rejected argument; `what` names the matrices in the nonzero limit's.
+// ol, when set, outlines the instance variables (n_vars then counts the copies).
 int32_t lcmap_build(Ctx* c, const LcMapHost& lm, uint64_t n_instance, uint64_t n_vars, const std::vector<LcMatrix>& mats,
-                    const char* what, const std::function<std::string(size_t, uint64_t)>& where, DevBuf& pool, uint32_t* pool_size);
-// the same handle as r1cs_upload from the constraint system's LcMap
+                    const char* what, const std::function<std::string(size_t, uint64_t)>& where, DevBuf& pool, uint32_t* pool_size,
+                    const LcOutline* ol = nullptr);
+// the same handle as r1cs_upload from the constraint system's LcMap; ol: instance outlining (B2S_OUTLINE_R1CS), or null
 int32_t r1cs_upload_lcmap(Ctx* c, uint64_t n_rows, uint64_t n_instance, uint64_t n_witness, const uint64_t* const args[3],
                           uint64_t n_lcs, const uint64_t* lc_offsets, const uint64_t* lc_vars, const uint32_t* lc_coeffs,
-                          const void* pool, uint32_t pool_len, b2s_r1cs** out);
+                          const void* pool, uint32_t pool_len, const b2s_outline* ol, b2s_r1cs** out);
+// z' = z || (ONE, z[1], ..., z[n_copies - 1]) for n_assign rows of n_src elements, in `mem` like z
+int32_t outline_assignment(Ctx* c, uint64_t n_src, uint64_t n_copies, uint64_t n_assign, const void* z, int32_t mem, void* out_z);
 // out_k: device arrays with at least n_rows elements each
 int32_t spmv_run(Ctx* c, const b2s_r1cs* m, const void* z_dev, void* out_a, void* out_b, void* out_c);
 // h_dev: device array of domain elements (output); z_dev: n_instance + n_witness elements; qap: the reduction (libsnark: h's

@@ -39,6 +39,8 @@ class PkDesc(ctypes.Structure):
 
 GR1CS_MAX_ARITY = 8
 NOT_FOUND = np.uint64(0xFFFFFFFFFFFFFFFF)   # first_unsat of a satisfied predicate
+# instance outlining strategies (b2s_outline): ark-relations' outline_r1cs / outline_sr1cs
+OUTLINE_R1CS, OUTLINE_SR1CS = 1, 2
 # scalar-field moduli, for the Montgomery form of the Python-int coefficients gr1cs_upload takes
 FR_MODULUS = {BLS12_381: 0x73EDA753299D7D483339D80809A1D80553BDA402FFFE5BFEFFFFFFFF00000001,
               BN254: 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001,
@@ -73,6 +75,11 @@ class PredicateLcmapDesc(ctypes.Structure):
         ("n_rows", c_uint64),
         ("args", c_void_p * GR1CS_MAX_ARITY),
     ]
+
+
+class Outline(ctypes.Structure):
+    """b2s_outline: the strategy (OUTLINE_R1CS / OUTLINE_SR1CS) and the upload index of the predicate that gets the tie rows"""
+    _fields_ = [("strategy", c_int32), ("pred", c_uint32)]
 
 
 def _mont_limbs(r, xs):
@@ -150,6 +157,12 @@ SIGNATURES = {
     "b2s_sr1cs_assignment": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p]),
     "b2s_gr1cs_info": (c_int32, [c_void_p, c_void_p, POINTER(c_uint64), POINTER(c_uint32), POINTER(Gr1csPredInfo), c_uint32]),
     "b2s_gr1cs_export": (c_int32, [c_void_p, c_void_p, c_uint32, c_uint32, c_void_p, c_uint64, c_void_p, c_uint64, c_void_p, c_uint64]),
+    "b2s_gr1cs_upload_lcmap_outline": (c_int32, [c_void_p, c_uint64, c_uint64, c_uint32, c_void_p, c_uint64, c_void_p, c_void_p, c_void_p,
+                                                 c_void_p, c_uint32, POINTER(Outline), POINTER(c_void_p)]),
+    "b2s_r1cs_upload_lcmap_outline": (c_int32, [c_void_p, c_uint64, c_uint64, c_uint64, POINTER(c_void_p), c_uint64, c_void_p, c_void_p,
+                                                c_void_p, c_void_p, c_uint32, POINTER(Outline), POINTER(c_void_p)]),
+    "b2s_gr1cs_outline_assignment": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p]),
+    "b2s_r1cs_outline_assignment": (c_int32, [c_void_p, c_void_p, c_uint64, c_void_p, c_int32, c_void_p]),
     "b2s_pk_upload": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, POINTER(c_void_p)]),
     "b2s_pk_upload_qap": (c_int32, [c_void_p, POINTER(PkDesc), c_int32, c_int32, POINTER(c_void_p)]),
     "b2s_pk_free": (None, [c_void_p, c_void_p]),
@@ -308,6 +321,7 @@ class Backend:
     def __init__(self, curve=BLS12_381, device=0):
         self.h = None
         self._r1cs_vars = {}   # n_instance + n_witness of each matrix handle, for the width check of r1cs_check
+        self._r1cs_src_vars = {}   # of an outlined matrix handle: the variables before outlining (outline_assignment's input)
         self.lib = load_library()
         h = c_void_p()
         st = self.lib.b2s_ctx_create(curve, device, ctypes.byref(h))
@@ -413,19 +427,27 @@ class Backend:
         self._r1cs_vars[h.value] = n_instance + n_witness
         return h
 
-    def r1cs_upload_lcmap(self, n_rows, n_instance, n_witness, args, lc_offsets, lc_vars, lc_coeffs, pool):
+    def r1cs_upload_lcmap(self, n_rows, n_instance, n_witness, args, lc_offsets, lc_vars, lc_coeffs, pool, outline=False):
         """The same handle, CSR built on the device from the constraint system's LcMap.  args: three uint64[n_rows] arrays
-        of raw Variables; lc_offsets uint64[n_lcs+1]; lc_vars uint64[], lc_coeffs uint32[]; pool uint32[pool_len*8]."""
+        of raw Variables; lc_offsets uint64[n_lcs+1]; lc_vars uint64[], lc_coeffs uint32[]; pool uint32[pool_len*8].
+        outline=True: b2s_r1cs_upload_lcmap_outline, the instance variables outlined by outline_r1cs (n_instance more
+        witnesses and rows; convert assignments with outline_assignment)."""
         a = (c_void_p * 3)(*[x.ctypes.data for x in args])
         h = c_void_p()
-        self._ck(self.lib.b2s_r1cs_upload_lcmap(self.h, n_rows, n_instance, n_witness, a, len(lc_offsets) - 1, lc_offsets.ctypes.data,
-                                                lc_vars.ctypes.data, lc_coeffs.ctypes.data, pool.ctypes.data, len(pool) // 8,
-                                                ctypes.byref(h)))
-        self._r1cs_vars[h.value] = n_instance + n_witness
+        common = (self.h, n_rows, n_instance, n_witness, a, len(lc_offsets) - 1, lc_offsets.ctypes.data, lc_vars.ctypes.data,
+                  lc_coeffs.ctypes.data, pool.ctypes.data, len(pool) // 8)
+        if outline:
+            self._ck(self.lib.b2s_r1cs_upload_lcmap_outline(*common, ctypes.byref(Outline(OUTLINE_R1CS, 0)), ctypes.byref(h)))
+            self._r1cs_vars[h.value] = 2 * n_instance + n_witness
+            self._r1cs_src_vars[h.value] = n_instance + n_witness
+        else:
+            self._ck(self.lib.b2s_r1cs_upload_lcmap(*common, ctypes.byref(h)))
+            self._r1cs_vars[h.value] = n_instance + n_witness
         return h
 
     def r1cs_free(self, m):
         self._r1cs_vars.pop(m.value if isinstance(m, c_void_p) else m, None)
+        self._r1cs_src_vars.pop(m.value if isinstance(m, c_void_p) else m, None)
         self.lib.b2s_r1cs_free(self.h, m)
 
     def domain_size(self, m):
@@ -479,11 +501,14 @@ class Backend:
         self._ck(self.lib.b2s_gr1cs_upload(self.h, n_instance, n_witness, len(labels), descs, ctypes.byref(h)))
         return Gr1cs(h, labels, n_instance + n_witness)
 
-    def gr1cs_upload_lcmap(self, n_instance, n_witness, predicates, lcmap):
+    def gr1cs_upload_lcmap(self, n_instance, n_witness, predicates, lcmap, outline=None):
         """The same Gr1cs, built on the device from the constraint system's LcMap.  predicates: {label: (arity, terms)} as for
         gr1cs_upload without the matrices; lcmap: the flat storage of every predicate -- offsets (n_lcs + 1), vars
         (raw Variables), coeffs (ids into pool), pool (Python ints, pool[0] = 1) and args {label: one sequence of raw Variables
-        per argument, one Variable per constraint}; lists or numpy arrays.  Uploaded in sorted label order."""
+        per argument, one Variable per constraint}; lists or numpy arrays.  Uploaded in sorted label order.
+        outline=(strategy, label): b2s_gr1cs_upload_lcmap_outline, the instance variables outlined as finalize() does with an
+        InstanceOutliner of that strategy (OUTLINE_R1CS / OUTLINE_SR1CS) whose tie rows go to predicate `label`; n_instance and
+        n_witness are the counts before outlining.  Convert assignments with outline_assignment."""
         r = FR_MODULUS[self.curve]
         labels = sorted(predicates)
         descs = (PredicateLcmapDesc * max(len(labels), 1))()
@@ -501,10 +526,15 @@ class Backend:
         lc_coeffs = np.ascontiguousarray(lcmap["coeffs"], dtype=np.uint32)
         pool = _mont_limbs(r, lcmap["pool"])
         h = c_void_p()
-        self._ck(self.lib.b2s_gr1cs_upload_lcmap(self.h, n_instance, n_witness, len(labels), descs, len(off) - 1, off.ctypes.data,
-                                                 lc_vars.ctypes.data, lc_coeffs.ctypes.data, pool.ctypes.data, len(lcmap["pool"]),
-                                                 ctypes.byref(h)))
-        return Gr1cs(h, labels, n_instance + n_witness)
+        common = (self.h, n_instance, n_witness, len(labels), descs, len(off) - 1, off.ctypes.data, lc_vars.ctypes.data, lc_coeffs.ctypes.data,
+                  pool.ctypes.data, len(lcmap["pool"]))
+        if outline is None:
+            self._ck(self.lib.b2s_gr1cs_upload_lcmap(*common, ctypes.byref(h)))
+            return Gr1cs(h, labels, n_instance + n_witness)
+        strategy, label = outline
+        pred = labels.index(label) if label in labels else len(labels)
+        self._ck(self.lib.b2s_gr1cs_upload_lcmap_outline(*common, ctypes.byref(Outline(strategy, pred)), ctypes.byref(h)))
+        return Gr1cs(h, labels, 2 * n_instance + n_witness, n_instance + n_witness)
 
     def gr1cs_free(self, g):
         self.lib.b2s_gr1cs_free(self.h, g.h)
@@ -578,6 +608,30 @@ class Backend:
                 torch.cuda.current_stream(z.device).synchronize()
         (pz, po), mem = _ptrs(z, out)
         self._ck(self.lib.b2s_sr1cs_assignment(self.h, g.h, z.shape[0], pz, mem, po))
+        return out
+
+    def outline_assignment(self, h, z, out=None):
+        """b2s_gr1cs_outline_assignment (h a Gr1cs) / b2s_r1cs_outline_assignment (h a matrix handle) of an outlined upload:
+        z (n_assign, src_vars * 8) 32-bit limbs of assignments before outlining, HOST numpy or CUDA torch tensor -> the
+        outlined assignments z || (ONE, z[1], ..., z[n_instance - 1]), (n_assign, n_vars * 8) in the same memory (written into
+        `out` if given)."""
+        if isinstance(h, Gr1cs):
+            fn, handle, src, n_vars = self.lib.b2s_gr1cs_outline_assignment, h.h, h.src_vars or 0, h.n_vars
+        else:
+            key = h.value if isinstance(h, c_void_p) else h
+            fn, handle, src, n_vars = self.lib.b2s_r1cs_outline_assignment, h, self._r1cs_src_vars.get(key, 0), self._r1cs_vars.get(key, 0)
+        if len(z.shape) != 2 or z.shape[1] != 8 * src:
+            raise ValueError(f"z must be (n_assign, {8 * src}) 32-bit limbs, got shape {tuple(z.shape)}")
+        if out is None:
+            if isinstance(z, np.ndarray):
+                out = np.zeros((z.shape[0], 8 * n_vars), dtype=np.uint32)
+            else:
+                import torch
+
+                out = torch.zeros((z.shape[0], 8 * n_vars), dtype=z.dtype, device=z.device)
+                torch.cuda.current_stream(z.device).synchronize()
+        (pz, po), mem = _ptrs(z, out)
+        self._ck(fn(self.h, handle, z.shape[0], pz, mem, po))
         return out
 
     def gr1cs_info(self, g):
